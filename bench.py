@@ -8,16 +8,19 @@
   --config 3            configs[2]: 1241x376 stereo pairs (KITTI shape), 2000 kp: extract L + R, stereo::compute, pose_optimizer
   --config 5            configs[4]: 1920x1080 perspective, 2000 kp, the config-4 pipeline, one stream per GPU
 
-One "step" = `frames_per_step` frames through the hot path on each of the --streams independent camera streams of a GPU
-(every stream owns its handles, CUDA streams and host thread; frames_per_step is calibrated in the warm-up so that the
-timed region lasts >= ~2 s and is reported in `config`).  Two measurements per run, over the SAME calls:
+One "step" = one frame through the hot path on each of the --streams independent camera streams of a GPU (every stream
+owns its handles, CUDA streams and host thread); --steps sets the number of timed steps.  Two measurements per run, over
+the SAME calls:
   value  every input already resident in HBM when the timed region starts (frames, BA graph): ovs_extract_device,
          ovs_robust_brute_force_match_device, ovs_frame_index_create_device, ovs_local_ba_prepare_device / run / fetch_device.
          The whole path is inside the timed region -- graph preparation, greedy replays, Levenberg loop -- only the
          host<->device copies of the inputs / results are not.
   e2e    the host-buffer C-ABI entry points a reference caller would use, every host<->device copy inside the timed region.
-`--impl reference` times the CPU oracle (the restated reference; the real one cannot be built here, see DESIGN.md) on the
-same workload with all usable host cores, as independent streams.  Prints ONE JSON line on rank 0."""
+`--impl reference` times the CPU oracle (the restated reference; the real one cannot be built, see DESIGN.md) on the
+same workload with all usable host cores, as independent streams.  Prints ONE JSON line on rank 0.
+
+`--dump-outputs DIR` writes what the value path returned in its last timed step, per rank and camera stream, as
+DIR/r<rank>_s<stream>_<name>.npy (float32 / float64, 64 MB in all).  The inputs depend only on the arguments, so two builds can be compared output for output."""
 import argparse
 import ctypes as C
 import json
@@ -46,6 +49,7 @@ CONFIGS = {
                  "(20k landmarks) + pose_optimizer + local_bundle_adjuster (50+10 KF / 20k landmarks)"),
 }
 K_FREE, K_FIXED, N_LM = 50, 10, 20000
+H100_HBM_GBS = 3350.0      # NVIDIA H100 SXM data sheet: the denominator of the bandwidth rooflines
 N_PROJ_LM = 20000          # landmarks projected into the frame by match_frame_and_landmarks
 
 
@@ -138,7 +142,7 @@ def make_landmark_sets(cfg, wl, ext):
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, gpu_index):
         super().__init__(daemon=True)
@@ -252,24 +256,25 @@ class CameraStream:
         return s, xy
 
     def _common_tail(self, leg, fidx, n, i, t):
-        """projection match (+ pose optimiser, local BA) of frame i on the frame index `fidx`; t = stage clock list."""
-        cfg, pose = self.cfg, self.wl["pose"]
+        """projection match of frame i on the frame index `fidx` -> (num_matches, matched landmark per keypoint); t = stage clock list."""
+        cfg = self.cfg
         s, xy = self._landmarks(i)
         if cfg["ba"]:
-            self.pj.match_frame_and_landmarks(fidx, self.sf, xy, None, s["level"], s["desc"], None, None, 5.0)
+            res = self.pj.match_frame_and_landmarks(fidx, self.sf, xy, None, s["level"], s["desc"], None, None, 5.0)
         else:
-            self.pj.match_current_and_last_frames(fidx, self.sf, 8, np.ones(len(xy), np.uint8), xy, None, s["level"], s["angle"], s["desc"], None, 20.0)
+            res = self.pj.match_current_and_last_frames(fidx, self.sf, 8, np.ones(len(xy), np.uint8), xy, None, s["level"], s["angle"], s["desc"], None, 20.0)
         fidx.close()
         t.append(time.perf_counter())
-        return pose
+        return res
 
     def step_device(self, i):
-        i = (i + 11 * self.sid) % self.ring            # streams walk the shared frame ring at different offsets
+        i = frame_of_step(i, self.sid, self.ring)
         cfg, L, sd = self.cfg, self.L, self.st_dev
         W, H = cfg["W"], cfg["H"]
         cur = i & 1
         t = [time.perf_counter()]
         n = self.ext.extract_device(self.d_frames[i].data_ptr(), W, H, W, self.d_kps[cur].data_ptr(), self.d_desc[cur].data_ptr(), self.cap)
+        out = self.last_out = {"n": n, "cur": cur}       # what this frame returned to the caller (--dump-outputs)
         sd["ext_us"] += np.array(list(self.ext.last_timings_us().values()))
         if cfg["stereo"]:
             nr = self.ext_r.extract_device(self.d_frames_r[i].data_ptr(), W, H, W, self.d_kps_r.data_ptr(), self.d_desc_r.data_ptr(), self.cap)
@@ -280,23 +285,23 @@ class CameraStream:
             # host once, the pyramids stay on the device
             kl = self.d_kps[cur][:n].cpu().numpy().view(self._kp_dtype()).reshape(-1); dl = self.d_desc[cur][:n].cpu().numpy()
             kr = self.d_kps_r[:nr].cpu().numpy().view(self._kp_dtype()).reshape(-1); dr = self.d_desc_r[:nr].cpu().numpy()
-            self.st.compute(self.ext, self.ext_r, kl, dl, kr, dr, pose["cam"]["focal_x_baseline"], pose["cam"]["focal_x_baseline"] / pose["cam"]["fx"])
+            out["stereo"] = self.st.compute(self.ext, self.ext_r, kl, dl, kr, dr, pose["cam"]["focal_x_baseline"], pose["cam"]["focal_x_baseline"] / pose["cam"]["fx"])
             t.append(time.perf_counter())
             stages = ["extract", "stereo_match"]
         else:
             stages = ["extract"]
             if cfg["ba"]:
                 if self.n_prev:
-                    self.mt.brute_force_match_device(self.d_desc[cur].data_ptr(), n, self.d_desc[cur ^ 1].data_ptr(), self.n_prev)
+                    out["bf_matches"] = self.mt.brute_force_match_device(self.d_desc[cur].data_ptr(), n, self.d_desc[cur ^ 1].data_ptr(), self.n_prev)
                     sd["match_us"] += self.mt.last_kernel_us(); sd["match_calls"] += 1
                 self.n_prev = n
                 t.append(time.perf_counter()); stages.append("brute_force_match")
             from openvslam_b200 import match
             fidx = match.frame_index.from_device(self.pj, n, self.d_kps[cur].data_ptr(), self.d_desc[cur].data_ptr(), self.grid)
-            self._common_tail("device", fidx, n, i, t); stages.append("projection_match")
+            out["projection"] = self._common_tail("device", fidx, n, i, t); stages.append("projection_match")
         xr = pose["obs_xr"] if cfg["stereo"] else None
-        _, _, _, pst = self.po.optimize(self.pcam, not cfg["stereo"], pose["pts_w"], pose["obs_xy"], xr, pose["inv_sigma_sq"], pose["poses"][0])
-        sd["pose_us"] += pst["device_us"]
+        out["pose"] = self.po.optimize(self.pcam, not cfg["stereo"], pose["pts_w"], pose["obs_xy"], xr, pose["inv_sigma_sq"], pose["poses"][0])
+        sd["pose_us"] += out["pose"][3]["device_us"]
         t.append(time.perf_counter()); stages.append("pose_optimizer")
         if cfg["ba"]:
             from openvslam_b200 import optimize
@@ -317,7 +322,7 @@ class CameraStream:
         return n
 
     def step_host(self, i):
-        i = (i + 11 * self.sid) % self.ring
+        i = frame_of_step(i, self.sid, self.ring)
         cfg = self.cfg
         pose = self.wl["pose"]
         from openvslam_b200 import match
@@ -382,10 +387,63 @@ class CameraStream:
             d2h += K * 96 + Lm * 24 + M + 512
         return h2d, d2h
 
+    def last_outputs(self):
+        """The arrays the value path returned to its caller for this stream's last frame, as float32 / float64 (exact for the
+        integer fields: keypoint levels, descriptor bytes and indices are all < 2^24)."""
+        o, f32 = self.last_out, np.float32
+        n, cur = o["n"], o["cur"]
+        kps = self.d_kps[cur][:n].cpu().numpy().view(self._kp_dtype()).reshape(-1)
+        res = {"keypoints": np.stack([kps[f].astype(f32) for f in kps.dtype.names], 1),
+               "descriptors": self.d_desc[cur][:n].cpu().numpy().astype(f32)}
+        if "bf_matches" in o:
+            res["bf_matches"] = o["bf_matches"].astype(f32)
+        if "projection" in o:
+            res["projection_matches"] = o["projection"][1].astype(f32)
+        if "stereo" in o:
+            res["stereo_x_right"], res["stereo_depth"] = o["stereo"][0].astype(f32), o["stereo"][1].astype(f32)
+        ninl, pose, flags, _ = o["pose"]
+        res["pose"] = np.asarray(pose, np.float64)
+        res["pose_outliers"] = np.asarray(flags).astype(f32)
+        res["pose_num_inliers"] = np.array([ninl], f32)
+        if self.cfg["ba"]:
+            res["ba_poses"], res["ba_points"] = (t.cpu().numpy().astype(np.float64) for t in self.d_ba_out[:2])
+            res["ba_outliers"] = self.d_ba_out[2].cpu().numpy().astype(f32)
+        return res
+
     def close(self):
         for h in (self.ext, self.ext_r, self.mt, self.pj, self.st, self.po, getattr(self, "lba", None), getattr(self, "pba", None)):
             if h is not None:
                 h.close()
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(path, cams, rank, world):
+    """DIR/r<rank>_s<stream>_<name>.npy for the last frame of every camera stream of this rank.  Every rank writes its own
+    files and gets an equal share of the 64 MB budget, so the dump of a multi-process run is 64 MB in all without any
+    coordination; a rank writes its streams in order while they fit in its share."""
+    os.makedirs(path, exist_ok=True)
+    budget, total = DUMP_LIMIT_BYTES // world, 0
+    for cs in cams:
+        arrays = cs.last_outputs()
+        size = sum(a.nbytes for a in arrays.values())
+        if total + size > budget:
+            print("--dump-outputs: rank %d, streams %d.. left out (64 MB limit)" % (rank, cs.sid), file=sys.stderr)
+            break
+        total += size
+        for name, a in arrays.items():
+            np.save(os.path.join(path, "r%d_s%d_%s.npy" % (rank, cs.sid, name)), a)
+
+
+def default_ring(cfg):
+    """Frames in the device ring: > 140 MB of frames, well beyond the L2 (50 MB on H100)."""
+    return max(12, int(140e6 / (cfg["W"] * cfg["H"])) // 6 * 6 + 6)
+
+
+def frame_of_step(step, sid, ring):
+    """Ring index of the frame that camera stream `sid` processes at step index `step` (warm-up steps included)."""
+    return (step + 11 * sid) % ring            # streams walk the shared frame ring at different offsets
 
 
 def run_ours(args):
@@ -400,7 +458,7 @@ def run_ours(args):
     dev = torch.device("cuda", local)
     W, H, NKP = cfg["W"], cfg["H"], cfg["NKP"]
     S = max(1, args.streams if args.streams > 0 else cfg["streams"])
-    ring = args.ring if args.ring > 0 else max(12, int(140e6 / (W * H)) // 6 * 6 + 6)      # > 126 MB of frames: larger than L2
+    ring = args.ring if args.ring > 0 else default_ring(cfg)
     wl = make_workload(cfg, rank, ring)
     wait = args.wait
     if wait == "auto":   # spin while every driving thread can own a core, yield-poll once they cannot
@@ -458,16 +516,12 @@ def run_ours(args):
         if errs:
             raise errs[0]
 
-    event_ms, fps_info = {}, {}
+    event_ms = {}
 
     def timed(name, steps, warmup, offset):
-        # warm-up (>= 3 frames per stream), also calibrates frames_per_step so that the timed region lasts >= ~2 s
-        t0 = time.perf_counter()
+        # warm-up: >= 3 frames per stream
         run_all(name, offset, offset + warmup)
         torch.cuda.synchronize()
-        per_frame = max_over_ranks((time.perf_counter() - t0) / warmup, dev, world)
-        fps = args.frames_per_step if args.frames_per_step > 0 else int(min(500, max(1, np.ceil(args.min_seconds / (steps * per_frame)))))
-        fps_info[name] = fps
         for cs in cams:
             cs.reset()
         barrier()
@@ -477,7 +531,7 @@ def run_ours(args):
         e0 = torch.cuda.Event(enable_timing=True); e1 = torch.cuda.Event(enable_timing=True)
         e0.record()
         t0 = time.perf_counter()
-        run_all(name, offset + warmup, offset + warmup + steps * fps)
+        run_all(name, offset + warmup, offset + warmup + steps)
         torch.cuda.synchronize()
         dt = time.perf_counter() - t0
         e1.record(); e1.synchronize()
@@ -489,12 +543,13 @@ def run_ours(args):
     if sampler:
         sampler.start()
     t_dev, launches = timed("step_device", args.steps, args.warmup, 0)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, cams, rank, world)
     dev_state = {k: (v.copy() if isinstance(v, np.ndarray) else v) for k, v in cams[0].st_dev.items()}   # per-kernel times: stream 0
     dev_stage = cams[0].stage_ms["device"].copy()
     t_e2e, _ = timed("step_host", args.steps, args.warmup, 7)
     host_stage = cams[0].stage_ms["host"].copy()
     clocks = sampler.stop() if sampler else None
-    fps_d, fps_h = fps_info["step_device"], fps_info["step_host"]
 
     # ---- per-frame latency of ONE stream alone on the GPU (what a live SLAM session sees): spin waits, the BA iteration
     #      replayed as a CUDA graph.  Reported next to the throughput figures, not part of `value`.
@@ -519,36 +574,19 @@ def run_ours(args):
         latency = {"streams": 1, "frames": nlat, "ms_per_frame_device_resident": round(1e3 * lat["step_device"], 4),
                    "ms_per_frame_e2e": round(1e3 * lat["step_host"], 4), "host_wait": "spin", "cuda_graphs": bool(cfg["ba"])}
 
-    value = aggregate_value(args.steps * fps_d * S, t_dev, world)
-    e2e = aggregate_value(args.steps * fps_h * S, t_e2e, world)
+    value = aggregate_value(args.steps * S, t_dev, world)
+    e2e = aggregate_value(args.steps * S, t_e2e, world)
     h2d, d2h = cams[0].bytes_per_frame()
 
     out = None
     if rank == 0:
-        peaks = {}
-        try:
-            peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-        except Exception:
-            pass
-        hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-        peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
+        hbm_peak = H100_HBM_GBS
+        peak_src = "NVIDIA H100 SXM data sheet (HBM3, 3.35 TB/s); not a measured figure"
         nf = max(dev_state["frames"], 1)
         ext_us = dev_state["ext_us"] / nf
         names = ("upload", "pyramid", "fast_score", "cell_nms_compact", "tree_distribute", "orient_describe", "download", "total_wall")
         stages = {"extract_" + n: round(float(v), 1) for n, v in zip(names, ext_us)}
         stages.update(pose_optimizer_kernel=round(dev_state["pose_us"] / nf, 1))
-        traffic = {}
-        for fn in ("r2_dram_traffic.json", "r1_dram_traffic.json"):
-            try:
-                for k, v in json.load(open(os.path.join(ROOT, "profiles", fn))).items():
-                    traffic.setdefault(k, v)
-            except Exception:
-                pass
-        ncu_metrics = {}
-        try:
-            ncu_metrics = json.load(open(os.path.join(ROOT, "profiles", "r2_ncu_metrics.json")))
-        except Exception:
-            pass
         # FAST score kernel: reads the pyramid once and writes the score map once
         lv, w_, h_ = [], W, H
         for l in range(8):
@@ -557,19 +595,18 @@ def run_ours(args):
         fast_us = float(ext_us[2])
         fast_gbs = fast_bytes / (fast_us * 1e-6) / 1e9 if fast_us > 0 else 0.0
         rl_fast = {"kernel": "k_fast_score", "bound": "hbm", "achieved": round(fast_gbs, 2), "peak": hbm_peak, "unit": "GB/s",
-                   "frac": round(fast_gbs / hbm_peak, 5), "traffic": traffic.get("k_fast_score"), "peak_source": peak_src,
+                   "frac": round(fast_gbs / hbm_peak, 5), "peak_source": peak_src,
                    "algorithmic_bytes_per_launch": fast_bytes, "avg_launch_us": round(fast_us, 2)}
         out = {
             "metric": METRIC, "value": round(value, 3), "unit": "frames/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": round(1e3 * t_dev / args.steps, 4), "ms_per_step_cuda_events": round(event_ms.get("step_device", 0.0) / args.steps, 4),
             "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
             "dtype": "u8 (extract, Hamming) + f64 (pose optimiser, local BA)", "data": "synthetic (seeded numpy frames and BA graph; no datasets offline)",
-            "config": {"workload": cfg["name"], "streams_per_gpu": S, "frames_per_step_per_stream": fps_d, "lm_speculation_width": spec, "lm_second_batch_width": spec2, "lm_cuda_graphs": bool(args.graphs), "ba_solver_cluster_ctas": cluster if cfg["ba"] else None, "host_wait": wait,
+            "config": {"workload": cfg["name"], "streams_per_gpu": S, "lm_speculation_width": spec, "lm_second_batch_width": spec2, "lm_cuda_graphs": bool(args.graphs), "ba_solver_cluster_ctas": cluster if cfg["ba"] else None, "host_wait": wait,
                        "host_cores": host_cores(),
-                       "step": "%d frame(s) on each of the %d independent camera streams of a GPU (own handles and CUDA streams, one host thread each); "
-                               "the driver's step count is kept, frames per step are calibrated in the warm-up so that the timed region lasts >= %.1f s"
-                               % (fps_d, S, args.min_seconds),
-                       "l2": "frame ring of %d x %.2f MB = %.0f MB > 126 MB L2" % (ring, W * H / 1e6, ring * W * H / 1e6),
+                       "step": "one frame on each of the %d independent camera streams of a GPU (own handles and CUDA streams, one host thread each)" % S,
+                       "l2": "frame ring of %d x %.2f MB = %.0f MB, L2 %.0f MB" % (ring, W * H / 1e6, ring * W * H / 1e6,
+                                                                            torch.cuda.get_device_properties(dev).L2_cache_size / 1e6),
                        "value_path": "whole path, inputs resident in HBM (extract_device, brute_force_match_device, frame_index_create_device, "
                                      "local_ba_prepare_device / run / fetch_device); the projection matcher's landmark arrays and the pose "
                                      "optimiser's observations are host-side map data in both legs",
@@ -577,10 +614,10 @@ def run_ours(args):
                        "timing": "barrier + synchronize on both sides, max over ranks; host clock of the region (every C-ABI call returns with its "
                                  "stream drained) cross-checked by CUDA events recorded while the device is idle (ms_per_step_cuda_events)"},
             "e2e": {"value": round(e2e, 3), "unit": "frames/s", "ms_per_step": round(1e3 * t_e2e / args.steps, 4),
-                    "ms_per_step_cuda_events": round(event_ms.get("step_host", 0.0) / args.steps, 4), "frames_per_step_per_stream": fps_h,
-                    "h2d_bytes_per_step": int(h2d) * S * fps_h, "d2h_bytes_per_step": int(d2h) * S * fps_h,
-                    "stage_ms_per_frame_stream0": {n: round(float(v) / (args.steps * fps_h), 3) for n, v in zip(STAGES, host_stage) if v > 0}},
-            "value_stage_ms_per_frame_stream0": {n: round(float(v) / (args.steps * fps_d), 3) for n, v in zip(STAGES, dev_stage) if v > 0},
+                    "ms_per_step_cuda_events": round(event_ms.get("step_host", 0.0) / args.steps, 4),
+                    "h2d_bytes_per_step": int(h2d) * S, "d2h_bytes_per_step": int(d2h) * S,
+                    "stage_ms_per_frame_stream0": {n: round(float(v) / args.steps, 3) for n, v in zip(STAGES, host_stage) if v > 0}},
+            "value_stage_ms_per_frame_stream0": {n: round(float(v) / args.steps, 3) for n, v in zip(STAGES, dev_stage) if v > 0},
             "single_stream_latency": latency,
             "gpu_launches": int(launches),
             "stage_us_per_frame": stages,
@@ -594,7 +631,7 @@ def run_ours(args):
             sol_us = dev_state["solver_us"] / sol_launches
             sol_flops = (nred ** 3 / 3.0 + 2.0 * nred ** 2) * dev_state["solver_trials"] / sol_launches
             sol_tf = sol_flops / (sol_us * 1e-6) / 1e12 if sol_us > 0 else 0.0
-            # FP64 tensor peak: MEASURED_PEAKS.json holds no FP64 figure -> measured now, on this GPU (ovs_probe_fp64_peaks)
+            # FP64 tensor peak: measured now, on this GPU (ovs_probe_fp64_peaks)
             dm, df = C.c_double(0), C.c_double(0)
             _lib.check(L.ovs_probe_fp64_peaks(local, C.byref(dm), C.byref(df)))
             fp64_peak = dm.value
@@ -602,18 +639,17 @@ def run_ours(args):
             ham_bytes = (NKP + NKP) * 32 + NKP * 8
             ham_gbs = ham_bytes / (ham_us * 1e-6) / 1e9 if ham_us > 0 else 0.0
             stages.update(match_hamming_kernel=round(ham_us, 1), local_ba_device=round(dev_state["ba_us"] / nf, 1))
-            frame_ms = 1e3 * t_dev / (args.steps * fps_d)
+            frame_ms = 1e3 * t_dev / args.steps
             out["roofline"] = {
                 "kernel": "k_ba_cholesky_solve", "bound": "tensor", "achieved": round(sol_tf, 4), "peak": round(fp64_peak, 2), "unit": "TFLOP/s",
-                "frac": round(sol_tf / fp64_peak, 5) if fp64_peak > 0 else None, "traffic": traffic.get("k_ba_cholesky_solve"),
-                "peak_source": "FP64 DMMA (mma.sync.m8n8k4.f64) whole-chip issue rate measured in this run by ovs_probe_fp64_peaks "
-                               "(MEASURED_PEAKS.json has no FP64 entry); DFMA pipe measured alongside: %.2f TFLOP/s" % df.value,
+                "frac": round(sol_tf / fp64_peak, 5) if fp64_peak > 0 else None,
+                "peak_source": "FP64 DMMA (mma.sync.m8n8k4.f64) whole-chip issue rate measured in this run by ovs_probe_fp64_peaks; "
+                               "DFMA pipe measured alongside: %.2f TFLOP/s" % df.value,
                 "algorithmic_flops_per_launch": round(sol_flops), "avg_launch_us": round(sol_us, 2),
                 "launches_per_frame": round(sol_launches / nf, 2), "share_of_stream_time": round(dev_state["solver_us"] / nf / (1e3 * frame_ms), 4),
                 "reduced_dim": nred, "systems_per_launch": round(dev_state["solver_trials"] / sol_launches, 2),
                 "lm_trials_per_frame": round(dev_state["ba_trials"] / nf, 2), "lm_iterations_per_frame": round(dev_state["ba_iterations"] / nf, 2),
-                "note": "latency bound, not throughput bound: n dependent pivots (fma -> shuffle -> rsqrt -> mul, ~120 clk each "
-                        "measured) put a floor of n x 120 clk = %.1f us under every launch" % (nred * 120 / 1.965e3)}
+                "note": "latency bound, not throughput bound: the n pivots form a dependent chain (fma -> shuffle -> rsqrt -> mul)"}
             # Schur complement (k_ba_schur_chunk + k_ba_schur_final), the GEMM north_star asks the tensor-pipe figure for.  Algorithmic
             # flops per co-observation record and damping value: Y_a = Hpl_a (Hll + lambda I)^-1 (6x3x3) + Y_a Hpl_b' (6x3x6) = 162 FMA.
             sch_us = dev_state["schur_us"] / sol_launches
@@ -621,16 +657,14 @@ def run_ours(args):
             sch_tf = sch_flops / (sch_us * 1e-6) / 1e12 if sch_us > 0 else 0.0
             out["roofline_schur"] = {
                 "kernel": "k_ba_schur_chunk+k_ba_schur_final", "bound": "tensor", "achieved": round(sch_tf, 4), "peak": round(fp64_peak, 2), "unit": "TFLOP/s",
-                "frac": round(sch_tf / fp64_peak, 5) if fp64_peak > 0 else None, "traffic": traffic.get("k_ba_schur_chunk"),
+                "frac": round(sch_tf / fp64_peak, 5) if fp64_peak > 0 else None,
                 "algorithmic_flops_per_launch": round(sch_flops), "co_observations": int(dev_state["co_observations"]), "avg_launch_us": round(sch_us, 2),
                 "share_of_stream_time": round(dev_state["schur_us"] / nf / (1e3 * frame_ms), 4),
-                "ncu": ncu_metrics.get("k_ba_schur_chunk"),
-                "note": "DMMA m8n8k4 issues 6x6 blocks as 8x8 (56 % of the MMA flops are algorithmic) and B200 runs DMMA at the DFMA rate; the kernel "
-                        "is bound by the gathers of the Jacobian blocks and the shared-memory fragment traffic (profiles/README.md)"}
+                "note": "DMMA m8n8k4 issues 6x6 blocks as 8x8 (56 % of the MMA flops are algorithmic)"}
             out["roofline_hamming"] = {
                 "kernel": "k_hamming_topk+k_topk_merge", "bound": "hbm", "achieved": round(ham_gbs, 3), "peak": hbm_peak, "unit": "GB/s",
-                "frac": round(ham_gbs / hbm_peak, 7), "algorithmic_bytes_per_launch": ham_bytes, "traffic": traffic.get("k_hamming_topk"),
-                "avg_launch_us": round(ham_us, 2), "ncu": ncu_metrics.get("k_hamming_topk"),
+                "frac": round(ham_gbs / hbm_peak, 7), "algorithmic_bytes_per_launch": ham_bytes,
+                "avg_launch_us": round(ham_us, 2),
                 "operand_stream_gbs_not_hbm": round(NKP * NKP * 64 / (ham_us * 1e-6) / 1e9, 1) if ham_us > 0 else None,
                 "popc32_per_s_not_hbm": round(8.0 * NKP * NKP / (ham_us * 1e-6), 0) if ham_us > 0 else None}
             out["roofline_fast_score"] = rl_fast
@@ -770,7 +804,7 @@ def run_reference(args):
         "data": "synthetic", "config": {"workload": cfg["name"]},
         "cpu_baseline": {"value": round(fps, 4), "unit": "frames/s", "cores": threads, "kind": "port",
                          "sample": "%d independent streams x %d frames through oracle/ (restated CPU path, gcc -O3 -march=x86-64-v3; the reference itself "
-                                   "cannot be built: no source in /root/reference), %.1f s" % (threads, per_thread + 1, dt)},
+                                   "cannot be built: its source is not available), %.1f s" % (threads, per_thread + 1, dt)},
         "e2e": {"value": round(fps, 4), "unit": "frames/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
     }
 
@@ -778,14 +812,12 @@ def run_reference(args):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--steps", type=int, default=100)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--config", type=int, default=4, choices=sorted(CONFIGS), help="BASELINE.json configs[n-1]; 4 = the metric's configuration")
-    ap.add_argument("--ring", type=int, default=0, help="frames in the device ring (0: just above 126 MB, the L2 size)")
+    ap.add_argument("--ring", type=int, default=0, help="frames in the device ring (0: just above 140 MB, beyond the L2)")
     ap.add_argument("--streams", type=int, default=0, help="independent camera streams per GPU (0: the config's default, 8; config 5: 1)")
-    ap.add_argument("--frames-per-step", type=int, default=0, help="frames per stream per step (0: calibrated so that the timed region lasts --min-seconds)")
-    ap.add_argument("--min-seconds", type=float, default=2.0)
     ap.add_argument("--spec", type=int, default=0, help="local BA speculation width 1..4 (0 = default 4)")
     ap.add_argument("--spec2", type=int, default=0, help="local BA: width of a statically enqueued second trial batch (0 = none)")
     ap.add_argument("--graphs", action="store_true", help="local BA: replay the Levenberg iteration as a CUDA graph in the throughput legs too (default: only in the single-stream latency pass)")
@@ -796,7 +828,10 @@ def main():
     ap.add_argument("--no-latency", action="store_true", help="skip the single-stream latency pass")
     ap.add_argument("--cpu-budget", type=float, default=20.0)
     ap.add_argument("--ref-threads", type=int, default=0, help="CPU arm: independent streams (0 = one per usable host core, cgroup quota respected)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default="", help="write the value path's outputs of the last timed step as DIR/r<rank>_s<stream>_<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     out = run_reference(args) if args.impl == "reference" else run_ours(args)
     if out is not None:

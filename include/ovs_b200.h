@@ -1,5 +1,5 @@
 /*
- * ovs_b200.h -- C ABI of the B200-native OpenVSLAM hot path (libovs_b200.so).
+ * ovs_b200.h -- C ABI of the H100-native OpenVSLAM hot path (libovs_b200.so).
  *
  * This is the drop-in boundary of SURVEY.md section 8(b): plain pointers and sizes, int
  * return codes, no exceptions, no torch / OpenCV / Eigen types.  The reference has no
@@ -19,7 +19,7 @@
  *    stereo frame constructor runs two extractor instances on two threads).
  *  - *_host entry points take HOST buffers (copies are inside the call); *_device entry points
  *    take DEVICE buffers and leave results on the device.
- *  - there is no CPU fallback: if no sm_100 device is present, *_create fails.
+ *  - there is no CPU fallback: if no sm_90 (H100) device is present, *_create fails.
  */
 #ifndef OVS_B200_H
 #define OVS_B200_H
@@ -41,7 +41,7 @@ extern "C" {
 #define OVS_ERR_NUMERIC (-7)       /* linear solve failed (not positive definite) */
 
 const char* ovs_last_error(void);
-/* Library / build identification: "ovs_b200 <version> sm_100a". */
+/* Library / build identification: "ovs_b200 <version> sm_90a". */
 const char* ovs_version(void);
 /* Number of CUDA kernels launched by this library in the calling process so far. */
 uint64_t ovs_kernel_launch_count(void);
@@ -410,8 +410,8 @@ int ovs_debug_sort_pairs(int device, const uint32_t* keys, const uint64_t* vals,
 /* CTAs per thread-block cluster of the reduced-system solver on this device (8, or 16 when 4 such clusters can be co-resident). */
 int ovs_optimizer_cluster_width(const ovs_optimizer* h);
 /* Local / global BA: CTAs per cluster of the reduced-system solver (1, 2, 4 or 8; default 8).  8 gives the lowest latency of a
- * single call; 2 gives the most calls per second when several optimisers share the GPU (measured on B200, 8 concurrent local
- * BAs: +13 % calls/s, +8 % latency per call).  The result does not depend on the width. */
+ * single call; 2 is meant for several optimisers sharing the GPU: each call occupies fewer SMs, so more calls run at once.
+ * The result does not depend on the width. */
 int ovs_optimizer_set_cluster_width(ovs_optimizer* h, int width);
 /* Local BA: the launch sequence of one Levenberg iteration is static (damping values, ring slots and the accept / reject
  * walk live in device memory), so it can be captured once per run and replayed as ONE CUDA graph per iteration.  Trims
@@ -423,8 +423,7 @@ int ovs_optimizer_set_graphs(ovs_optimizer* h, int enable);
 int ovs_optimizer_set_host_sync(ovs_optimizer* h, int mode);
 /* Local BA: number of Levenberg damping trials evaluated speculatively per launch sequence (1..4, default 4).  The
  * result is the sequential algorithm's for every width; 4 minimises the latency of one session (a rejected trial costs
- * no extra round trip) and, measured on B200, is also the fastest setting with 8 sessions per GPU; smaller widths
- * trade latency for less speculative GPU work. */
+ * no extra round trip); smaller widths trade latency for less speculative GPU work. */
 int ovs_optimizer_set_speculation(ovs_optimizer* h, int width);
 /* Local BA: a second trial batch of `width` (1..4) damping values enqueued statically behind the first batch of every
  * iteration (0 = off, the default).  Its kernels return at their first instruction when the first batch decided the

@@ -1,4 +1,4 @@
-"""Builds libovs_b200.so (sm_100a only) in-tree with nvcc.  `python -m openvslam_b200.build`."""
+"""Builds libovs_b200.so (sm_90a, H100) in-tree with nvcc.  `python -m openvslam_b200.build`."""
 import os
 import subprocess
 import sys
@@ -9,7 +9,7 @@ LIBDIR = os.path.join(HERE, "lib")
 SO = os.path.join(LIBDIR, "libovs_b200.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "--fmad=false",            # parity-critical float code must not be contracted (belt and braces:
                                # that code also uses __fmul_rn/__fadd_rn explicitly)
     "-Xcompiler", "-fPIC", "-Xcompiler", "-O2", "-shared",
@@ -24,7 +24,8 @@ def needs_build():
     if not os.path.exists(SO):
         return True
     t = os.path.getmtime(SO)
-    deps = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(HERE, "..", "include", "ovs_b200.h")]
+    # this file too: a change of NVCC_FLAGS (the target architecture) must rebuild a library built with the old flags
+    deps = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(HERE, "..", "include", "ovs_b200.h"), os.path.abspath(__file__)]
     return any(os.path.getmtime(d) > t for d in deps)
 
 

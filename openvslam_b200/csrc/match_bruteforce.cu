@@ -5,7 +5,7 @@
 // k_hamming_topk    every query descriptor against a chunk of train descriptors staged in
 //                   shared memory (broadcast 128-bit reads); each thread keeps its query in 8
 //                   registers and a sorted top-4 of (distance << 16 | train index) keys.
-//                   Grid = query blocks x train chunks so that 4000 x 4000 fills 148 SMs.
+//                   Grid = query blocks x train chunks so that 4000 x 4000 fills the 132 SMs of an H100.
 // k_topk_merge      merges the per-chunk top-4 lists of a query.
 //
 // A sorted (distance, index) top-4 is what the reference's sequential `<` scan needs: best =
@@ -29,7 +29,7 @@ constexpr int kTrainTile = 128;  // descriptors staged per shared-memory tile (4
 // 256-bit Hamming distance with FOUR population counts instead of eight: the eight 32-bit difference words go through a
 // carry-save adder tree (bitwise full adders: sum = a ^ b ^ c, carry = majority(a, b, c), one LOP3 each), which leaves four words
 // holding the bit counts' ones, twos, fours and eights; distance = popc(ones) + 2 popc(twos) + 4 popc(fours) + 8 popc(eights).
-// POPC issues at a quarter of the ALU rate on sm_100, so it -- not the logic -- bounds a brute-force Hamming kernel
+// POPC issues at a quarter of the integer ALU rate on sm_90, so it -- not the logic -- bounds a brute-force Hamming kernel
 // (Harley-Seal, restricted to one descriptor pair so the result is exactly match::compute_descriptor_distance_32's).
 __device__ __forceinline__ int hamming256(const uint4& qa, const uint4& qb, const uint4& ta, const uint4& tb) {
     const unsigned x0 = qa.x ^ ta.x, x1 = qa.y ^ ta.y, x2 = qa.z ^ ta.z, x3 = qa.w ^ ta.w;

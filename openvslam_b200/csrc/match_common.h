@@ -11,7 +11,7 @@ struct ovs_index_buf { uint8_t* base = nullptr; size_t cap = 0; };
 struct ovs_matcher {
     int device = 0;
     cudaStream_t stream = nullptr;
-    int num_sms = 148;
+    int num_sms = 132;
     // grow-only device / pinned scratch
     uint8_t* d_q = nullptr; size_t d_q_cap = 0;
     uint8_t* d_t = nullptr; size_t d_t_cap = 0;

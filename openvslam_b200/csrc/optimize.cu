@@ -1,4 +1,4 @@
-// optimize.cu -- B200 (sm_100a) implementation of openvslam::optimize::pose_optimizer::optimize and
+// optimize.cu -- H100 (sm_90a) implementation of openvslam::optimize::pose_optimizer::optimize and
 // openvslam::optimize::local_bundle_adjuster::optimize (optimize/pose_optimizer.cc,
 // optimize/local_bundle_adjuster.cc), replacing the g2o call they make: Levenberg-Marquardt with
 // g2o's damping schedule, Huber kernel, landmarks marginalised by the Schur complement, dense
@@ -350,15 +350,14 @@ __device__ __forceinline__ void dmma_m8n8k4(double& d0, double& d1, double a, do
 // co-observation carries both edge indices, the landmark and the "either edge excluded" flag (no index chasing); the
 // (Hll + lambda I)^-1 of the NEXT damping value is in flight while the current one is multiplied; four independent DMMA
 // accumulator chains; the partial blocks of all damping values stay in registers and meet in ONE cross-warp reduction.
-// 4 blocks per SM on purpose (registers): with 5, eight concurrent camera streams lose 10 % -- the solver's clusters need
-// eight SMs of one GPC with their whole shared memory free at the same time, and denser Schur blocks starve them.
+// 4 blocks per SM on purpose (registers): the solver's clusters need several SMs of one GPC with their whole shared memory
+// free at the same time, and denser Schur blocks starve them when several camera streams share the GPU.
 // Shared-memory layout of the DMMA operands: FRAGMENT ORDER.  A warp's 32 co-observations form 8 groups of four; the K = 12 slots
 // of a group are walked by three DMMAs; element (row r, K slot 4 t + k) of group g sits at g * pitch + t * rows * 4 + r * 4 + k
 // (rows = 6 for Y, 7 for W: Hpl_b and the bl column), so the lanes of a DMMA read consecutive doubles (2 wavefronts, the minimum
 // for 64-bit accesses).  The pitches are = 4 or 12 mod 16, which makes the producer side conflict free as well (lane = co-observation
 // 4 g + en writes element (r, kc) to K slot 3 en + kc: the sixteen lanes of a half warp hit banks 4 g' + k, all different).
-// The record-per-lane layout this replaces cost 3-4 wavefronts per fragment load (3.7 M bank conflicts per launch; the kernel runs at
-// 93 % of the L1TEX peak, two thirds of it shared-memory wavefronts).  41 KB per block: the solver's clusters need SMs with free
+// A record-per-lane layout costs 3-4 wavefronts per fragment load.  41 KB per block: the solver's clusters need SMs with free
 // shared memory while eight streams share the GPU, a larger footprint here costs more there than it saves.
 constexpr int kSGY = 76, kSGW = 84;
 __global__ void __launch_bounds__(128, 4) k_ba_schur_chunk(BaDev P, const LmCtl* __restrict__ ctl, const int* __restrict__ nchunks,
@@ -2860,7 +2859,7 @@ extern "C" int ovs_optimizer_cluster_width(const ovs_optimizer* h) { return h ? 
 
 // CTAs per thread-block cluster of the reduced-system solver: 8 (default) minimises the latency of one call; a process that
 // runs several optimisers concurrently on one GPU gets more calls per second with 2 (the solver is latency bound: a wider
-// cluster shortens it by 8 % but occupies 4x the SMs, which the other streams' kernels could use).  Same results for every width.
+// cluster shortens it little but occupies 4x the SMs, which the other streams' kernels could use).  Same results for every width.
 extern "C" int ovs_optimizer_set_cluster_width(ovs_optimizer* h, int width) {
     OVS_REQUIRE(h && (width == 1 || width == 2 || width == 4 || width == 8), OVS_ERR_INVALID_ARG, "cluster width must be 1, 2, 4 or 8");
     h->chol_cluster = width;
@@ -2991,7 +2990,7 @@ extern "C" int ovs_optimizer_create(int device, ovs_optimizer** out) {
         if (const char* e = getenv("OVS_B200_LM_HOST_SYNC")) h->lm_host_sync = atoi(e) ? 1 : 0;   // development aid
         if (const char* e = getenv("OVS_B200_SPEC2")) h->spec_width2 = std::min(kSpec, std::max(0, atoi(e)));   // development aid
         if (const char* e = getenv("OVS_B200_SPEC")) h->spec_width = std::min(kSpec, std::max(1, atoi(e)));   // development aid: 0 = plain launches
-        int want = kCholCluster;   // measured on B200: 16-CTA clusters are no faster (the pivot chain, not the trailing update, bounds a step)
+        int want = kCholCluster;   // the pivot chain, not the trailing update, bounds a block step: wider clusters mostly occupy more SMs
         if (const char* e = getenv("OVS_B200_CHOL_CLUSTER")) want = atoi(e);
         if (want > kCholCluster && cudaFuncSetAttribute(k_ba_cholesky_solve, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess) {
             cudaLaunchConfig_t cfg = {};

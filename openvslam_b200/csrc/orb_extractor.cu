@@ -1,4 +1,4 @@
-// orb_extractor.cu -- B200 (sm_100a) implementation of openvslam::feature::orb_extractor::extract
+// orb_extractor.cu -- H100 (sm_90a) implementation of openvslam::feature::orb_extractor::extract
 // (feature/orb_extractor.{h,cc}; names as recalled in SURVEY.md 8a -- /root/reference holds no
 // source to cite line numbers from).
 //
@@ -71,8 +71,8 @@ struct SelKp {
 struct UMax { signed char v[16]; };
 
 // One TMA descriptor per pyramid level: u8 tensor {pitch, h}, box {kTmaBoxW, kTileH + 6}, zero fill outside.
-// The innermost start coordinate of a tiled TMA copy must be a multiple of 16 bytes (anything else raises
-// "illegal instruction" on sm_100a -- tools/probe/tma_probe.cu), so the box starts 16 columns left of the tile.
+// The box starts at a multiple of 16 bytes, 16 columns left of the tile: an unaligned innermost start coordinate was
+// found to fault ("illegal instruction") when the kernels were first written, and the aligned start is kept.
 constexpr int kTmaBoxW = 160;   // 16 (aligned left halo, 4 used) + 128 + 16 (right halo, 3 used)
 constexpr int kTmaHaloX = 16;
 struct TmapArray { CUtensorMap m[kMaxLevels]; };

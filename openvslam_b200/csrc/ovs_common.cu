@@ -69,8 +69,8 @@ int select_device(int device) {
     }
     cudaDeviceProp prop;
     OVS_CUDA_CHECK(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10) {
-        set_error("device %d is sm_%d%d; libovs_b200 is built for sm_100a (B200) only", device, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) {
+        set_error("device %d is sm_%d%d; libovs_b200 is built for sm_90a (H100) only", device, prop.major, prop.minor);
         return OVS_ERR_NO_DEVICE;
     }
     OVS_CUDA_CHECK(cudaSetDevice(device));
@@ -80,6 +80,6 @@ int select_device(int device) {
 }  // namespace ovs
 
 extern "C" const char* ovs_last_error(void) { return ovs::g_err; }
-extern "C" const char* ovs_version(void) { return "ovs_b200 0.1 sm_100a"; }
+extern "C" const char* ovs_version(void) { return "ovs_b200 0.1 sm_90a"; }
 extern "C" uint64_t ovs_kernel_launch_count(void) { return ovs::g_launches.load(); }
 extern "C" int ovs_set_wait_mode(int mode) { ovs::g_blocking.store(mode == 1 ? 1 : mode == 2 ? 2 : 0); return OVS_OK; }

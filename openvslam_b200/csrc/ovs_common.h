@@ -12,7 +12,7 @@ namespace ovs {
 void set_error(const char* fmt, ...);
 void count_launch(int n = 1);
 
-// Checks that `device` exists and is a Blackwell sm_100 part; selects it.  No CPU fallback.
+// Checks that `device` exists and is a Hopper sm_90 part (H100); selects it.  No CPU fallback.
 int select_device(int device);
 
 // Host waits.  Default: spin (cudaStreamSynchronize), the lowest latency for one camera stream per GPU.  With

@@ -1,6 +1,6 @@
 // probe.cu -- measured FP64 peaks of the device the library runs on: the whole-chip issue rate of independent
 // mma.sync.m8n8k4.f64 (DMMA) and of independent DFMA.  bench.py reports the Cholesky / Schur rooflines against the DMMA
-// figure measured in the same run (MEASURED_PEAKS.json carries no FP64 number).
+// figure measured in the same run.
 #include "ovs_common.h"
 
 namespace {

@@ -179,6 +179,6 @@ int main() {
         return 0;
     } catch (const std::exception& e) {
         std::fprintf(stderr, "%s\n", e.what());
-        return std::string(e.what()).find("no CPU fallback") != std::string::npos || std::string(e.what()).find("sm_100a") != std::string::npos ? 2 : 1;
+        return std::string(e.what()).find("no CPU fallback") != std::string::npos || std::string(e.what()).find("sm_90a") != std::string::npos ? 2 : 1;
     }
 }

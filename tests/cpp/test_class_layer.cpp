@@ -134,7 +134,7 @@ int main() {
         if (!(rms1 < 0.5 && rms1 < 0.2 * rms0) || poses[24 + 9] != -0.6) return 1;
     } catch (const std::exception& e) {
         std::printf("exception: %s\n", e.what());
-        return std::string(e.what()).find("no CPU fallback") != std::string::npos || std::string(e.what()).find("sm_100a") != std::string::npos ? 2 : 1;
+        return std::string(e.what()).find("no CPU fallback") != std::string::npos || std::string(e.what()).find("sm_90a") != std::string::npos ? 2 : 1;
     }
     std::printf("class layer ok\n");
     return 0;

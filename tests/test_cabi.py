@@ -26,12 +26,12 @@ def test_exports_every_declared_symbol(lib):
 
 
 def test_version_and_error_string(lib):
-    assert b"sm_100a" in lib.ovs_version()
+    assert b"sm_90a" in lib.ovs_version()
     assert isinstance(lib.ovs_last_error(), bytes)
 
 
 def test_no_cpu_fallback(lib):
-    """Without a usable B200 handle creation returns OVS_ERR_NO_DEVICE; it never falls back."""
+    """Without a usable H100 handle creation returns OVS_ERR_NO_DEVICE; it never falls back."""
     import torch
     if torch.cuda.is_available():
         pytest.skip("GPU present")

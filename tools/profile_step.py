@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""One hot-path step (extract, brute-force match, pose optimiser, local BA) for ncu captures.
+"""One hot-path step (extract, brute-force match, pose optimiser, local BA) to run under a profiler (e.g. torch.profiler).
 usage: python tools/profile_step.py [ba|extract|match|pose|all] [repeat]"""
 import os, sys
 import numpy as np
