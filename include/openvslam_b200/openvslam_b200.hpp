@@ -3,7 +3,7 @@
 //
 //   openvslam::feature::orb_params / orb_extractor        (src/openvslam/feature/orb_params.h, orb_extractor.h)
 //   openvslam::match::robust / projection / area / stereo (src/openvslam/match/*.h)
-//   openvslam::optimize::pose_optimizer / local_bundle_adjuster (src/openvslam/optimize/*.h)
+//   openvslam::optimize::pose_optimizer / local_bundle_adjuster / transform_optimizer (src/openvslam/optimize/*.h)
 // [file names as recalled in SURVEY.md 8(a); /root/reference holds no source, so no line numbers].
 //
 // The reference's methods take cv::Mat / cv::KeyPoint / Eigen / data::frame / data::keyframe.  None of
@@ -455,6 +455,34 @@ public:
 #endif
 private:
     const unsigned int num_first_iter_, num_second_iter_;
+    ovs_optimizer* h_ = nullptr;
+};
+
+class transform_optimizer {
+public:
+    explicit transform_optimizer(const bool fix_scale, const unsigned int num_iter = 10, const int device = 0)
+        : fix_scale_(fix_scale), num_iter_(num_iter) { detail::check(ovs_optimizer_create(device, &h_)); }
+    ~transform_optimizer() { ovs_optimizer_destroy(h_); }
+    transform_optimizer(const transform_optimizer&) = delete;
+    transform_optimizer& operator=(const transform_optimizer&) = delete;
+    //! optimize(keyfrm_1, keyfrm_2, matched_lms_in_keyfrm_2, g2o_Sim3_12, chi_sq) on the flattened correspondences (see
+    //! include/ovs_b200.h).  sim3_12 = {R row-major (9), t (3), s}, updated only when the return value is non-zero;
+    //! is_inlier[i] = 0 where the reference sets matched_lms_in_keyfrm_2 to nullptr.  Returns the inlier count.
+    unsigned int optimize(const ovs_camera& camera_1, const ovs_camera& camera_2, const double* cam_pose_1w, const double* cam_pose_2w,
+                          const int num_pairs, const double* pos_w_1, const float* undist_xy_1, const float* inv_level_sigma_sq_1,
+                          const double* pos_w_2, const float* undist_xy_2, const float* inv_level_sigma_sq_2, double* sim3_12,
+                          const float chi_sq, std::vector<std::uint8_t>& is_inlier) const {
+        is_inlier.assign(std::max(1, num_pairs), 0);
+        int n = 0;
+        detail::check(ovs_transform_optimize_host(h_, &camera_1, &camera_2, cam_pose_1w, cam_pose_2w, num_pairs, pos_w_1, undist_xy_1,
+                                                  inv_level_sigma_sq_1, pos_w_2, undist_xy_2, inv_level_sigma_sq_2, fix_scale_ ? 1 : 0, chi_sq,
+                                                  5, static_cast<int>(num_iter_), sim3_12, is_inlier.data(), &n, nullptr));
+        is_inlier.resize(num_pairs);
+        return static_cast<unsigned int>(n);
+    }
+private:
+    const bool fix_scale_;
+    const unsigned int num_iter_;
     ovs_optimizer* h_ = nullptr;
 };
 

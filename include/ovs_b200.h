@@ -358,6 +358,30 @@ int ovs_pose_optimize_host(ovs_optimizer* h, const ovs_camera* cam, int setup_is
                            double* pose_cw, uint8_t* outlier_flags, int num_trials, int num_each_iter,
                            int* num_inliers, ovs_ba_stats* stats);
 
+/* transform_optimizer::optimize(keyfrm_1, keyfrm_2, matched_lms_in_keyfrm_2, g2o_Sim3_12, chi_sq)
+ * (optimize/transform_optimizer.cc, loop closure) on plain arrays: one Sim3 vertex S_12 (camera 2 -> camera 1,
+ * S p = s R p + t) and, per correspondence i, a forward edge (lm_2 through S_12 into keyframe 1) and a backward edge
+ * (lm_1 through S_12^-1 into keyframe 2), Huber delta (double)sqrtf(chi_sq).  The caller keeps the pairs the reference keeps
+ * (both landmarks valid, lm_2 observed in keyframe 2):
+ *  cam_1 / cam_2: keyfrm_x->camera_;  pose_1w[12] / pose_2w[12]: keyfrm_x->get_cam_pose() as {R row-major, t};
+ *  pos_w_1[n*3]: lm_1->get_pos_in_world(), lm_1 = keyframe 1's landmark at keypoint idx_i;
+ *  obs_xy_1[n*2]: keyfrm_1->undist_keypts_[idx_i].pt;  inv_sigma_sq_1[n]: keyfrm_1->inv_level_sigma_sq_[its octave];
+ *  pos_w_2 / obs_xy_2 / inv_sigma_sq_2: the same for lm_2 = matched_lms_in_keyfrm_2[idx_i] and its keypoint in keyframe 2;
+ *  fix_scale: the constructor's fix_scale (camera not monocular): update[6] = 0 inside the update, the damped system stays 7x7;
+ *  chi_sq: the reference passes 10;  num_first_iter / num_iter: the two rounds (5, and the constructor's num_iter, 10);
+ *  sim3_12[13]: g2o_Sim3_12 as {R row-major (9), t (3), s > 0}, overwritten only when the call succeeds;
+ *  inlier_out[n]: 1 while matched_lms_in_keyfrm_2[idx_i] stays set, 0 where the reference nulls it;
+ *  *num_inliers: the return value (0 when fewer than 10 pairs survive the first round).
+ * stats: num_rounds, iterations, trials, round_iterations, lambda_init per round, last_lambda, last_chi2, final_chi2 (plain
+ * chi2 of the surviving pairs' stored errors) and device_us.  n == 0 returns at once without a launch.
+ * Like ovs_pose_optimize_host this call reuses the handle's device buffers: a local-BA problem prepared on the same handle is
+ * invalidated (ovs_local_ba_run / _fetch then fail with OVS_ERR_INVALID_ARG until it is prepared again). */
+int ovs_transform_optimize_host(ovs_optimizer* h, const ovs_camera* cam_1, const ovs_camera* cam_2, const double* pose_1w,
+                                const double* pose_2w, int n, const double* pos_w_1, const float* obs_xy_1, const float* inv_sigma_sq_1,
+                                const double* pos_w_2, const float* obs_xy_2, const float* inv_sigma_sq_2, int fix_scale, float chi_sq,
+                                int num_first_iter, int num_iter, double* sim3_12, uint8_t* inlier_out, int* num_inliers,
+                                ovs_ba_stats* stats);
+
 /* local_bundle_adjuster::optimize(curr_keyfrm, force_stop_flag) (optimize/local_bundle_adjuster.cc) on
  * the graph the reference builds: K keyframe vertices (local keyframes free, "fixed" keyframes and
  * keyframe id 0 fixed), L landmark vertices (marginalised), M reprojection edges.

@@ -25,6 +25,9 @@
 // Pose optimiser: the whole optimize() (num_trials rounds x num_each_iter LM iterations, outlier
 // re-classification between rounds) is ONE kernel on an 8-CTA cluster (edges sliced over the CTAs, 6x6 normal equations
 // reduced through distributed shared memory in a fixed order); the system is 6x6.
+//
+// Transform optimiser (loop closure, optimize::transform_optimizer): the same shape with one Sim3 vertex and a 7x7
+// system -- both rounds, the outlier cut, the early exit and the write-back are ONE kernel, k_sim3_optimize.
 #include <algorithm>
 #include <cfloat>
 #include <cmath>
@@ -39,6 +42,7 @@
 
 #include "ba_math.cuh"
 #include "ovs_common.h"
+#include "sim3_math.cuh"
 
 namespace {
 
@@ -2270,6 +2274,315 @@ extern "C" int ovs_pose_optimize_host(ovs_optimizer* h, const ovs_camera* cam, i
         stats->num_iterations = (int)hstats[0]; stats->num_trials = (int)hstats[1]; stats->num_rounds = (int)hstats[2];
         stats->final_chi2 = hstats[3];
         for (int r = 0; r < 8 && r < stats->num_rounds; ++r) stats->lambda_init[r] = hstats[5 + r];
+        float ms = 0; cudaEventElapsedTime(&ms, h->ev[0], h->ev[1]);
+        stats->device_us = ms * 1000.f;
+    }
+    return OVS_OK;
+}
+
+// ----------------------------------------------------------------------- transform optimiser
+namespace {
+
+constexpr int kSim3Threads = 256;
+constexpr int kSim3Cluster = 8;
+constexpr int kSim3Stride = kSim3Threads * kSim3Cluster;   // pairs per grid-stride step: thread g takes pairs g, g + 2048, ...
+constexpr int kSim3Sums = 36;                              // H (28, packed 7x7), b (7), robust chi2
+
+struct Sim3OptArgs {
+    CameraD cam1, cam2;
+    double pose1[12], pose2[12];   // cam_pose_1w, cam_pose_2w
+    int n;
+    const double* pw1; const float2* xy1; const float* w1;   // lm_1 (world), keyframe 1's keypoint, its inv_level_sigma_sq
+    const double* pw2; const float2* xy2; const float* w2;   // lm_2 (world), keyframe 2's keypoint, its inv_level_sigma_sq
+    double* sim3;                  // 13, in / out (written only when the call succeeds)
+    unsigned char* inlier;         // n, out
+    int fix_scale, num_first_iter, num_iter;
+    double delta, chi_sq;
+    // [0] iterations [1] trials [2] rounds [3] final chi2 [4] inliers (the return value) [5..6] lambda_init per round
+    // [7..8] iterations per round [9] last lambda [10] last chi2
+    double* stats;
+};
+
+// transform_optimizer::optimize: the whole call is ONE kernel on a cluster of kSim3Cluster CTAs, organised as
+// k_pose_optimize: every CTA owns a grid-stride slice of the pairs (both edges of a pair in one thread), the 7x7 system and the
+// chi2 are reduced across the cluster through distributed shared memory in a fixed order (warp, then warps, then ranks), so
+// every CTA holds the same bits and takes the same Levenberg decision.  err (n x 4: e12, e21) keeps the errors of the last
+// evaluated trial, which the outlier tests read as g2o's chi2() does; level (n) is 1 for the pairs cut so far.
+__global__ void __cluster_dims__(kSim3Cluster, 1, 1) __launch_bounds__(kSim3Threads, 1)
+k_sim3_optimize(Sim3OptArgs A, double* __restrict__ err, unsigned char* __restrict__ level) {
+    constexpr int NW = kSim3Threads / 32;
+    constexpr int NS = kSim3Sums;
+    __shared__ double sm_red[NS][NW];
+    __shared__ double s_slots[2][kSim3Cluster][NS];
+    __shared__ double s_sys[NS], s_S[13], s_cand[13], s_x[7];
+    __shared__ int s_flag;
+    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    const unsigned my_rank = cluster_rank();
+    const int gtid = (int)my_rank * kSim3Threads + tid;
+    const int n = A.n;
+    if (tid < 13) s_S[tid] = A.sim3[tid];
+    for (int i = gtid; i < n; i += kSim3Stride) { level[i] = 0; A.inlier[i] = 0; }
+    cluster_sync_mem();     // every CTA of the cluster is running before anyone writes into its shared memory
+
+    int parity = 0;
+    auto reduce_all = [&](const double* acc, int count) {
+        __syncthreads();
+        for (int k = 0; k < count; ++k) {
+            const double v = warp_sum(acc[k]);
+            if (lane == 0) sm_red[k][wid] = v;
+        }
+        __syncthreads();
+        if (tid < count) {
+            double t = 0;
+#pragma unroll
+            for (int k = 0; k < NW; ++k) t += sm_red[tid][k];
+#pragma unroll
+            for (unsigned r = 0; r < (unsigned)kSim3Cluster; ++r) st_dsmem(&s_slots[parity][my_rank][tid], r, t);
+        }
+        cluster_sync_mem();
+        if (tid < count) {
+            double v = 0;
+#pragma unroll
+            for (int r = 0; r < kSim3Cluster; ++r) v += s_slots[parity][r][tid];
+            s_sys[tid] = v;
+        }
+        parity ^= 1;
+        __syncthreads();
+    };
+
+    // computeActiveErrors + buildSystem at S in one pass: errors to err[], this thread's share of {H, b, robust chi2}
+    auto build_local = [&](const double* Sp, double* acc) {
+#pragma unroll
+        for (int k = 0; k < NS; ++k) acc[k] = 0;
+        double S[13];
+#pragma unroll
+        for (int k = 0; k < 13; ++k) S[k] = Sp[k];
+        for (int i = gtid; i < n; i += kSim3Stride) {
+            if (level[i]) continue;
+#pragma unroll 1
+            for (int edge = 0; edge < 2; ++edge) {
+                const double* pose = edge == 0 ? A.pose2 : A.pose1;
+                const double* pwp = (edge == 0 ? A.pw2 : A.pw1) + 3 * (size_t)i;
+                const float2 xy = edge == 0 ? A.xy1[i] : A.xy2[i];
+                const double w = (double)(edge == 0 ? A.w1[i] : A.w2[i]);
+                const double pw[3] = {pwp[0], pwp[1], pwp[2]};
+                double pc[3];
+                ovs::mat3_vec(pose, pw, pc);
+                pc[0] += pose[9]; pc[1] += pose[10]; pc[2] += pose[11];
+                const double obs[2] = {(double)xy.x, (double)xy.y};
+                double e[2], J[14];
+                if (edge == 0) ovs::sim3_edge_forward(A.cam1, S, pc, obs, e, J);
+                else ovs::sim3_edge_backward(A.cam2, S, pc, obs, e, J);
+                err[4 * (size_t)i + 2 * edge] = e[0]; err[4 * (size_t)i + 2 * edge + 1] = e[1];
+                const double chi = w * (e[0] * e[0] + e[1] * e[1]);
+                double r0, r1;
+                ovs::huber(chi, A.delta, &r0, &r1);
+                acc[35] += r0;
+                const double ww = r1 * w;
+                for (int a = 0; a < 7; ++a) {
+                    acc[28 + a] -= J[a] * ww * e[0] + J[7 + a] * ww * e[1];
+                    for (int c = a; c < 7; ++c) acc[ovs::sym7(a, c)] += J[a] * ww * J[c] + J[7 + a] * ww * J[7 + c];
+                }
+            }
+        }
+    };
+
+    // pairs still active that fail chi_sq on the stored errors go to level 1; returns this thread's count of them
+    auto cut_outliers = [&]() {
+        double bad = 0;
+        for (int i = gtid; i < n; i += kSim3Stride) {
+            if (level[i]) continue;
+            const double* e = err + 4 * (size_t)i;
+            const double c12 = (double)A.w1[i] * (e[0] * e[0] + e[1] * e[1]);
+            const double c21 = (double)A.w2[i] * (e[2] * e[2] + e[3] * e[3]);
+            if (A.chi_sq < c12 || A.chi_sq < c21) { level[i] = 1; bad += 1.0; }
+        }
+        return bad;
+    };
+
+    int total_iters = 0, total_trials = 0, rounds = 0;
+    double last_lambda = 0, last_chi = 0;
+    // SparseOptimizer::optimize(iterations) with a fresh initializeOptimization (lambda_init again).  As in k_pose_optimize
+    // the pass that evaluates a trial also forms H and b at the candidate, which an accepted trial hands to the next iteration.
+    auto lm_round = [&](int iterations) {
+        double lambda = 0, ni = 2;
+        bool ok = true, have_sys = false;
+        int it = 0;
+        double Hs[28], bs[7], currentChi = 0;
+        for (; it < iterations && ok; ++it) {
+            if (!have_sys) {
+                double acc[NS];
+                build_local(s_S, acc);
+                reduce_all(acc, NS);
+#pragma unroll
+                for (int k = 0; k < 28; ++k) Hs[k] = s_sys[k];
+#pragma unroll
+                for (int k = 0; k < 7; ++k) bs[k] = s_sys[28 + k];
+                currentChi = s_sys[35];
+                have_sys = true;
+            }
+            if (it == 0) {
+                double md = 0;
+                for (int k = 0; k < 7; ++k) md = fmax(md, fabs(Hs[ovs::sym7(k, k)]));
+                lambda = 1e-5 * md;
+                ni = 2;
+                if (gtid == 0) A.stats[5 + rounds] = lambda;
+            }
+            double rho = 0;
+            int qmax = 0;
+            do {
+                if (tid == 0) {
+                    double xs[7];
+                    const bool ok2 = ovs::solve7(Hs, lambda, bs, xs);
+                    s_flag = ok2 ? 1 : 0;
+                    if (ok2) {
+                        for (int k = 0; k < 7; ++k) s_x[k] = xs[k];
+                        double out[13];
+                        ovs::sim3_oplus(s_S, xs, A.fix_scale != 0, out);
+                        for (int k = 0; k < 13; ++k) s_cand[k] = out[k];
+                    } else {
+                        for (int k = 0; k < 13; ++k) s_cand[k] = s_S[k];
+                    }
+                }
+                __syncthreads();
+                const bool ok2 = s_flag != 0;
+                {
+                    double acc[NS];
+                    build_local(s_cand, acc);
+                    reduce_all(acc, NS);
+                }
+                double tempChi = s_sys[35];
+                if (!ok2) tempChi = DBL_MAX;
+                rho = currentChi - tempChi;
+                double scale = 0;
+                if (ok2) for (int k = 0; k < 7; ++k) scale += s_x[k] * (lambda * s_x[k] + bs[k]);   // all seven components
+                scale += 1e-3;
+                rho /= scale;
+                const bool accept = rho > 0 && isfinite(tempChi);
+                if (accept) {
+                    double alpha = 1. - pow((2 * rho - 1), 3);
+                    alpha = fmin(alpha, 2. / 3.);
+                    lambda *= fmax(1. / 3., alpha);
+                    ni = 2;
+                    currentChi = tempChi;
+#pragma unroll
+                    for (int k = 0; k < 28; ++k) Hs[k] = s_sys[k];
+#pragma unroll
+                    for (int k = 0; k < 7; ++k) bs[k] = s_sys[28 + k];
+                } else {
+                    lambda *= ni;
+                    ni *= 2;
+                }
+                __syncthreads();                    // s_sys, s_x, s_S, s_cand have been read by every thread
+                if (accept && tid < 13) s_S[tid] = s_cand[tid];
+                __syncthreads();
+                ++qmax; ++total_trials;
+            } while (rho < 0 && qmax < 10);
+            last_lambda = lambda; last_chi = currentChi;
+            if (qmax == 10 || rho == 0) ok = false;
+        }
+        if (gtid == 0) A.stats[7 + rounds] = it;
+        total_iters += it; ++rounds;
+    };
+
+    lm_round(A.num_first_iter);
+    double cnt[1] = {cut_outliers()};
+    reduce_all(cnt, 1);
+    const int num_outliers = (int)(s_sys[0] + 0.5);
+    const bool success = n - num_outliers >= 10;     // otherwise: return 0, g2o_Sim3_12 untouched
+    int num_inliers = 0;
+    if (success) {
+        lm_round(A.num_iter);
+        cnt[0] = cut_outliers();
+        reduce_all(cnt, 1);
+        num_inliers = n - num_outliers - (int)(s_sys[0] + 0.5);
+    }
+    double fc[1] = {0};
+    for (int i = gtid; i < n; i += kSim3Stride) {
+        A.inlier[i] = level[i] ? 0 : 1;
+        if (level[i]) continue;
+        const double* e = err + 4 * (size_t)i;
+        fc[0] += (double)A.w1[i] * (e[0] * e[0] + e[1] * e[1]) + (double)A.w2[i] * (e[2] * e[2] + e[3] * e[3]);
+    }
+    reduce_all(fc, 1);
+    if (gtid == 0) {
+        A.stats[0] = total_iters; A.stats[1] = total_trials; A.stats[2] = rounds; A.stats[3] = s_sys[0]; A.stats[4] = num_inliers;
+        A.stats[9] = last_lambda; A.stats[10] = last_chi;
+    }
+    if (success && gtid < 13) A.sim3[gtid] = s_S[gtid];
+}
+
+}  // namespace
+
+extern "C" int ovs_transform_optimize_host(ovs_optimizer* h, const ovs_camera* cam_1, const ovs_camera* cam_2, const double* pose_1w,
+                                           const double* pose_2w, int n, const double* pos_w_1, const float* obs_xy_1,
+                                           const float* inv_sigma_sq_1, const double* pos_w_2, const float* obs_xy_2,
+                                           const float* inv_sigma_sq_2, int fix_scale, float chi_sq, int num_first_iter, int num_iter,
+                                           double* sim3_12, uint8_t* inlier_out, int* num_inliers, ovs_ba_stats* stats) {
+    OVS_REQUIRE(h && cam_1 && cam_2 && pose_1w && pose_2w && sim3_12 && num_inliers && n >= 0, OVS_ERR_INVALID_ARG, "bad argument");
+    OVS_REQUIRE(n == 0 || (pos_w_1 && obs_xy_1 && inv_sigma_sq_1 && pos_w_2 && obs_xy_2 && inv_sigma_sq_2 && inlier_out),
+                OVS_ERR_INVALID_ARG, "null argument");
+    OVS_REQUIRE((cam_1->model == ovs::kCamPerspective || cam_1->model == ovs::kCamEquirectangular) &&
+                (cam_2->model == ovs::kCamPerspective || cam_2->model == ovs::kCamEquirectangular), OVS_ERR_INVALID_ARG, "unknown camera model");
+    OVS_REQUIRE(num_first_iter >= 0 && num_iter >= 0, OVS_ERR_INVALID_ARG, "bad iteration counts");
+    OVS_REQUIRE(sim3_12[12] > 0.0 && std::isfinite(sim3_12[12]), OVS_ERR_INVALID_ARG, "the Sim3 scale must be positive");
+    OVS_REQUIRE(chi_sq > 0.0f && std::isfinite(chi_sq), OVS_ERR_INVALID_ARG, "chi_sq must be positive");
+    if (stats) memset(stats, 0, sizeof(*stats));
+    for (int i = 0; i < n; ++i) inlier_out[i] = 0;
+    *num_inliers = 0;
+    if (n == 0) return OVS_OK;   // fewer than 10 pairs can survive: the reference returns 0 and leaves g2o_Sim3_12 as it is
+    OVS_CUDA_CHECK(cudaSetDevice(h->device));
+    // carved from the same arenas as the pose optimiser: a prepared local-BA problem on this handle is gone
+    invalidate_plan(h);
+    if (h->pending) { OVS_CUDA_CHECK(ovs::sync_stream(h->stream)); h->pending = false; }
+    const size_t N = (size_t)n;
+    const size_t hbytes = 256 * 12 + N * 2 * (24 + 8 + 4) + N + 13 * 8 + 16 * 8;   // 256: alignment of each take
+    const size_t dbytes = hbytes + N * 32 + N + 4096;
+    int rc = ensure_arenas(h, dbytes, hbytes);
+    if (rc != OVS_OK) return rc;
+    Arena H{h->h_arena, 0, h->h_cap}, D{h->d_arena, 0, h->d_cap};
+    double* hp1 = H.take<double>(3 * N); float* hxy1 = H.take<float>(2 * N); float* hw1 = H.take<float>(N);
+    double* hp2 = H.take<double>(3 * N); float* hxy2 = H.take<float>(2 * N); float* hw2 = H.take<float>(N);
+    double* hS = H.take<double>(13); double* hstats = H.take<double>(16); uint8_t* hout = H.take<uint8_t>(N);
+    const size_t in_bytes = H.off;
+    double* dp1 = D.take<double>(3 * N); float* dxy1 = D.take<float>(2 * N); float* dw1 = D.take<float>(N);
+    double* dp2 = D.take<double>(3 * N); float* dxy2 = D.take<float>(2 * N); float* dw2 = D.take<float>(N);
+    double* dS = D.take<double>(13); double* dstats = D.take<double>(16); uint8_t* dout = D.take<uint8_t>(N);
+    double* derr = D.take<double>(4 * N); uint8_t* dlevel = D.take<uint8_t>(N);
+    memcpy(hp1, pos_w_1, 24 * N); memcpy(hxy1, obs_xy_1, 8 * N); memcpy(hw1, inv_sigma_sq_1, 4 * N);
+    memcpy(hp2, pos_w_2, 24 * N); memcpy(hxy2, obs_xy_2, 8 * N); memcpy(hw2, inv_sigma_sq_2, 4 * N);
+    memcpy(hS, sim3_12, 13 * 8);
+    memset(hstats, 0, 128);
+    cudaStream_t st = h->stream;
+    // both arenas were carved with the same sequence, so one contiguous copy moves all inputs
+    OVS_CUDA_CHECK(cudaMemcpyAsync(h->d_arena, h->h_arena, in_bytes, cudaMemcpyHostToDevice, st));
+    Sim3OptArgs A;
+    A.cam1 = to_cam(cam_1); A.cam2 = to_cam(cam_2);
+    memcpy(A.pose1, pose_1w, 96); memcpy(A.pose2, pose_2w, 96);
+    A.n = n;
+    A.pw1 = dp1; A.xy1 = (const float2*)dxy1; A.w1 = dw1; A.pw2 = dp2; A.xy2 = (const float2*)dxy2; A.w2 = dw2;
+    A.sim3 = dS; A.inlier = dout; A.fix_scale = fix_scale ? 1 : 0; A.num_first_iter = num_first_iter; A.num_iter = num_iter;
+    A.delta = (double)sqrtf(chi_sq); A.chi_sq = (double)chi_sq;
+    A.stats = dstats;
+    OVS_CUDA_CHECK(cudaEventRecord(h->ev[0], st));
+    k_sim3_optimize<<<kSim3Cluster, kSim3Threads, 0, st>>>(A, derr, dlevel);
+    OVS_LAUNCH_CHECK();
+    OVS_CUDA_CHECK(cudaEventRecord(h->ev[1], st));
+    OVS_CUDA_CHECK(cudaMemcpyAsync(hS, dS, 13 * 8, cudaMemcpyDeviceToHost, st));
+    OVS_CUDA_CHECK(cudaMemcpyAsync(hstats, dstats, 128, cudaMemcpyDeviceToHost, st));
+    OVS_CUDA_CHECK(cudaMemcpyAsync(hout, dout, N, cudaMemcpyDeviceToHost, st));
+    OVS_CUDA_CHECK(ovs::sync_stream(st));
+    memcpy(sim3_12, hS, 13 * 8);     // the device wrote it back only on success: otherwise these are the input bits
+    memcpy(inlier_out, hout, N);
+    *num_inliers = (int)hstats[4];
+    if (stats) {
+        stats->num_iterations = (int)hstats[0]; stats->num_trials = (int)hstats[1]; stats->num_rounds = (int)hstats[2];
+        stats->final_chi2 = hstats[3];
+        for (int r = 0; r < 2 && r < stats->num_rounds; ++r) {
+            stats->lambda_init[r] = hstats[5 + r];
+            stats->round_iterations[r] = (int)hstats[7 + r];
+        }
+        stats->last_lambda = hstats[9]; stats->last_chi2 = hstats[10];
         float ms = 0; cudaEventElapsedTime(&ms, h->ev[0], h->ev[1]);
         stats->device_us = ms * 1000.f;
     }

@@ -1,5 +1,5 @@
-"""Host-side mirror of openvslam::optimize::{pose_optimizer, local_bundle_adjuster}
-(src/openvslam/optimize/pose_optimizer.h, local_bundle_adjuster.h; names as in SURVEY.md 8a)
+"""Host-side mirror of openvslam::optimize::{pose_optimizer, local_bundle_adjuster, global_bundle_adjuster,
+transform_optimizer} (src/openvslam/optimize/*.h; names as in SURVEY.md 8a)
 over the C ABI of libovs_b200.so.  The reference classes take data::frame / data::keyframe; here the
 same quantities are passed as flat arrays (see include/ovs_b200.h for the field-by-field mapping)."""
 import ctypes as C
@@ -158,6 +158,37 @@ class global_bundle_adjuster(_optimizer_handle):
                                                  len(points), points.ctypes.data_as(C.c_void_p), len(obs_kf), pk, pl, po, px, pi, self.num_iter_,
                                                  int(self.use_huber_kernel_), C.byref(fs) if fs is not None else None, C.byref(st)))
         return poses, points, _stats(st)
+
+
+class transform_optimizer(_optimizer_handle):
+    """openvslam::optimize::transform_optimizer(fix_scale, num_iter = 10): the Sim3 refinement of a loop candidate.
+    num_first_iter is the first round's iteration count (the reference's 5)."""
+
+    def __init__(self, fix_scale, num_iter=10, num_first_iter=5, device=0):
+        super().__init__(device)
+        self.fix_scale_ = bool(fix_scale)
+        self.num_iter_ = int(num_iter)
+        self.num_first_iter_ = int(num_first_iter)
+
+    def optimize(self, cam_1, cam_2, pose_1w, pose_2w, pos_w_1, obs_xy_1, inv_sigma_sq_1, pos_w_2, obs_xy_2, inv_sigma_sq_2, sim3_12,
+                 chi_sq=10.0):
+        """One row per correspondence (see include/ovs_b200.h); sim3_12 = {R row-major (9), t (3), s}.
+        -> (num_inliers, sim3_12[13] (the input when num_inliers == 0), inlier_flags[n], stats)."""
+        p1 = np.array(pose_1w, np.float64).reshape(12); p2 = np.array(pose_2w, np.float64).reshape(12)
+        w1, pw1 = _p(np.asarray(pos_w_1).reshape(-1, 3), np.float64); x1, px1 = _p(obs_xy_1, np.float32); s1, ps1 = _p(inv_sigma_sq_1, np.float32)
+        w2, pw2 = _p(np.asarray(pos_w_2).reshape(-1, 3), np.float64); x2, px2 = _p(obs_xy_2, np.float32); s2, ps2 = _p(inv_sigma_sq_2, np.float32)
+        n = len(s1)
+        if not (len(w1) == len(w2) == len(s2) == n and x1.size == x2.size == 2 * n):
+            raise ValueError("transform_optimizer: every per-pair array needs n rows")
+        S = np.array(sim3_12, np.float64).reshape(13).copy()
+        flags = np.zeros(max(n, 1), np.uint8)
+        ninl = C.c_int(0); st = BaStats()
+        _lib.check(_lib.lib().ovs_transform_optimize_host(self._h, C.byref(cam_1), C.byref(cam_2), p1.ctypes.data_as(C.c_void_p),
+                                                          p2.ctypes.data_as(C.c_void_p), n, pw1, px1, ps1, pw2, px2, ps2,
+                                                          int(self.fix_scale_), C.c_float(chi_sq), self.num_first_iter_, self.num_iter_,
+                                                          S.ctypes.data_as(C.c_void_p), flags.ctypes.data_as(C.c_void_p), C.byref(ninl),
+                                                          C.byref(st)))
+        return ninl.value, S, flags[:n].astype(bool), _stats(st)
 
 
 class prepared_local_ba(_optimizer_handle):
