@@ -3,7 +3,7 @@
 //
 //   openvslam::feature::orb_params / orb_extractor        (src/openvslam/feature/orb_params.h, orb_extractor.h)
 //   openvslam::match::robust / projection / area / stereo (src/openvslam/match/*.h)
-//   openvslam::optimize::pose_optimizer / local_bundle_adjuster / transform_optimizer (src/openvslam/optimize/*.h)
+//   openvslam::optimize::pose_optimizer / local_bundle_adjuster / transform_optimizer / graph_optimizer (src/openvslam/optimize/*.h)
 // [file names as recalled in SURVEY.md 8(a); /root/reference holds no source, so no line numbers].
 //
 // The reference's methods take cv::Mat / cv::KeyPoint / Eigen / data::frame / data::keyframe.  None of
@@ -479,6 +479,28 @@ public:
                                                   5, static_cast<int>(num_iter_), sim3_12, is_inlier.data(), &n, nullptr));
         is_inlier.resize(num_pairs);
         return static_cast<unsigned int>(n);
+    }
+private:
+    const bool fix_scale_;
+    const unsigned int num_iter_;
+    ovs_optimizer* h_ = nullptr;
+};
+
+class graph_optimizer {
+public:
+    explicit graph_optimizer(const bool fix_scale, const unsigned int num_iter = 50, const int device = 0)
+        : fix_scale_(fix_scale), num_iter_(num_iter) { detail::check(ovs_optimizer_create(device, &h_)); }
+    ~graph_optimizer() { ovs_optimizer_destroy(h_); }
+    graph_optimizer(const graph_optimizer&) = delete;
+    graph_optimizer& operator=(const graph_optimizer&) = delete;
+    //! optimize(loop_keyfrm, curr_keyfrm, non_corrected_Sim3s, pre_corrected_Sim3s, loop_connections) on the flattened pose graph
+    //! (see include/ovs_b200.h and INTEGRATION.md): sim3_cw[K*13] = S_iw {R row-major (9), t (3), s}, updated in place;
+    //! landmarks pos_w[L*3] corrected through their reference vertex (-1: unchanged); cam_poses_cw[K*12] = {R, t / s} (may be null).
+    void optimize(const int num_keyfrms, double* sim3_cw, const std::uint8_t* is_fixed, const int num_edges, const std::int32_t* edge_i,
+                  const std::int32_t* edge_j, const double* meas_Sji, const int num_landmarks, double* pos_w, const std::int32_t* ref_vertex,
+                  double* cam_poses_cw) const {
+        detail::check(ovs_graph_optimize_host(h_, num_keyfrms, sim3_cw, is_fixed, num_edges, edge_i, edge_j, meas_Sji, fix_scale_ ? 1 : 0,
+                                              static_cast<int>(num_iter_), num_landmarks, pos_w, ref_vertex, cam_poses_cw, nullptr));
     }
 private:
     const bool fix_scale_;

@@ -382,6 +382,31 @@ int ovs_transform_optimize_host(ovs_optimizer* h, const ovs_camera* cam_1, const
                                 int num_first_iter, int num_iter, double* sim3_12, uint8_t* inlier_out, int* num_inliers,
                                 ovs_ba_stats* stats);
 
+/* graph_optimizer::optimize(loop_keyfrm, curr_keyfrm, non_corrected_Sim3s, pre_corrected_Sim3s, loop_connections)
+ * (optimize/graph_optimizer.cc, loop closure) on plain arrays: one Sim3 vertex per keyframe, one relative Sim3 edge per keyframe
+ * pair, e = log(S_ji S_i S_j^-1) with identity information and no robust kernel, g2o's Levenberg with the user lambda 1e-16.
+ * The caller flattens the graph as the reference builds it (INTEGRATION.md):
+ *  sim3_cw[K*13]: S_iw as {R row-major (9), t (3), s > 0} -- the pre-corrected Sim3 where the keyframe has one, otherwise
+ *    {R, t, 1} of cam_pose_cw; overwritten with the optimised estimates;
+ *  fixed[K]: 1 for the loop keyframe (a free vertex without an edge is left out of the system and keeps its bits);
+ *  edge_i[E] / edge_j[E] / meas_ji[E*13]: vertex 0, vertex 1 and the measurement S_ji of each edge (i != j);
+ *  fix_scale: the constructor's fix_scale (stereo / RGB-D): update[6] = 0 inside the update, the system stays 7 per vertex;
+ *  num_iter: the reference's 50;
+ *  lm_pos_w[L*3] / lm_ref[L]: landmark positions, corrected in place as p <- S_wr^opt (S_rw^init p) through the reference
+ *    vertex r (the landmark's reference keyframe, or ref_keyfrm_id_in_loop_fusion_); lm_ref = -1 leaves a landmark's bits;
+ *  pose_cw_out[K*12] (may be NULL): cam_pose_cw = {R, t / s} of the optimised S_iw.
+ * stats: num_rounds (1), iterations, trials, lambda_init[0] (1e-16), last_lambda, last_chi2, final_chi2 (chi2 at the returned
+ * estimates, also when nothing is optimised; 0 for E == 0), device_us, solver_us, solver_launches, solver_trials,
+ * reduced_dim = 7 x free vertices.
+ * An index out of range, i == j, or a scale that is not positive and finite returns OVS_ERR_INVALID_ARG; more than 857 free
+ * vertices (7 x 857 = 5999 <= 6000, the dense solver's limit) returns OVS_ERR_UNSUPPORTED.  With no free vertex in the system
+ * (E == 0 included) nothing is optimised: the estimates come back unchanged and only the write-back runs.
+ * Like ovs_pose_optimize_host this call reuses the handle's device buffers: a local-BA problem prepared on the same handle is
+ * invalidated (ovs_local_ba_run / _fetch then fail with OVS_ERR_INVALID_ARG until it is prepared again). */
+int ovs_graph_optimize_host(ovs_optimizer* h, int K, double* sim3_cw, const uint8_t* fixed, int E, const int32_t* edge_i,
+                            const int32_t* edge_j, const double* meas_ji, int fix_scale, int num_iter, int L, double* lm_pos_w,
+                            const int32_t* lm_ref, double* pose_cw_out, ovs_ba_stats* stats);
+
 /* local_bundle_adjuster::optimize(curr_keyfrm, force_stop_flag) (optimize/local_bundle_adjuster.cc) on
  * the graph the reference builds: K keyframe vertices (local keyframes free, "fixed" keyframes and
  * keyframe id 0 fixed), L landmark vertices (marginalised), M reprojection edges.

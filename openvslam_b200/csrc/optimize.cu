@@ -28,12 +28,17 @@
 //
 // Transform optimiser (loop closure, optimize::transform_optimizer): the same shape with one Sim3 vertex and a 7x7
 // system -- both rounds, the outlier cut, the early exit and the write-back are ONE kernel, k_sim3_optimize.
+//
+// Pose graph (loop closure, optimize::graph_optimizer): one Sim3 vertex per keyframe, a dense 7 n_free system assembled per trial
+// batch (k_pg_*) and factorised by the local BA's solver, under the same device-side Levenberg controller (LmCtl, k_ba_reduce,
+// lm_round); see the section at the end of this file.
 #include <algorithm>
 #include <cfloat>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <new>
 #include <sched.h>
 #include <time.h>
@@ -1447,6 +1452,33 @@ __global__ void k_lm_round_end(LmCtl* ctl, const volatile int* stop_word, volati
     mirror_state(c, mirror);
 }
 
+// Start of a Levenberg iteration (one thread): the damping values and ring slots of its first trial batch.  lambda_init is
+// g2o's computeLambdaInit, used on the first iteration of a round.
+__device__ void lm_plan_iteration(LmCtl* ctl, double lambda_init, const volatile int* stop_word, int* fail, volatile int* mirror) {
+    LmCtl c = *ctl;
+    if (c.active && stop_word && *stop_word != 0) { c.active = 0; c.stopped = 1; }
+    if (!c.active) {
+        c.nbatch = 0;
+    } else {
+        if (c.it == 0) {
+            c.lambda = lambda_init;
+            c.ni = 2;
+            if (c.num_rounds < 8) c.lambda_init[c.num_rounds] = c.lambda;
+        }
+        c.qmax = 0; c.rho = 0;
+        const int nn = min(max(c.spec_width, 1), kSpec);
+        double l = c.lambda, n2 = c.ni;
+#pragma unroll
+        for (int k = 0; k < kSpec; ++k)
+            if (k < nn) { c.lam[k] = l; c.buf[k] = (c.cur + 1 + k) % (kSpec + 1); l *= n2; c.ni_after[k] = n2; n2 *= 2; }
+        c.nbatch = nn;
+    }
+    *ctl = c;
+#pragma unroll
+    for (int k = 0; k < kSpec; ++k) fail[k] = 0;
+    mirror_state(c, mirror);
+}
+
 __global__ void __launch_bounds__(1024) k_ba_pose_final_plan(LmCtl* ctl, int nfree, const int* __restrict__ kf_chunk_begin, const double* __restrict__ ppart,
                                                               double* __restrict__ Hpp, double* __restrict__ bp, double* maxdiag, int* fail,
                                                               const volatile int* stop_word, volatile int* mirror) {
@@ -1476,29 +1508,8 @@ __global__ void __launch_bounds__(1024) k_ba_pose_final_plan(LmCtl* ctl, int nfr
     if (halted) return;             // halted: the parked batch and the Hessian of the undecided iteration must survive
     for (int w = 0; w < 32; ++w) md = fmax(md, smax[w]);
     md = fmax(md, maxdiag[0]);      // the landmark blocks' share (k_ba_landmark_accum)
-    LmCtl c = *ctl;
-    if (c.active && stop_word && *stop_word != 0) { c.active = 0; c.stopped = 1; }
-    if (!c.active) {
-        c.nbatch = 0;
-    } else {
-        if (c.it == 0) {
-            c.lambda = 1e-5 * md;
-            c.ni = 2;
-            if (c.num_rounds < 8) c.lambda_init[c.num_rounds] = c.lambda;
-        }
-        c.qmax = 0; c.rho = 0;
-        const int nn = min(max(c.spec_width, 1), kSpec);
-        double l = c.lambda, n2 = c.ni;
-#pragma unroll
-        for (int k = 0; k < kSpec; ++k)
-            if (k < nn) { c.lam[k] = l; c.buf[k] = (c.cur + 1 + k) % (kSpec + 1); l *= n2; c.ni_after[k] = n2; n2 *= 2; }
-        c.nbatch = nn;
-    }
-    *ctl = c;
     maxdiag[0] = 0; maxdiag[1] = 0;
-#pragma unroll
-    for (int k = 0; k < kSpec; ++k) fail[k] = 0;
-    mirror_state(c, mirror);
+    lm_plan_iteration(ctl, 1e-5 * md, stop_word, fail, mirror);
 }
 
 // Outlier classification from the stored edge errors (edge->chi2()) and depth_is_positive().
@@ -2625,6 +2636,24 @@ struct ovs_ba_plan {
 
 namespace {
 
+// The dense FP64 solver of one trial batch: kSpec systems (n + 1) x n (lower triangle + rhs row, S_stride apart), factorised in
+// place, solutions to x (n apart).  The cluster kernel up to the shared-memory panel limit, the multi-launch path above it.
+struct DenseSolve {
+    double* S; size_t S_stride; int n; double* x; double* invL; size_t invL_stride; int* fail; long long* clk;
+    int chol_big, chol_dbuf; size_t chol_smem;
+};
+
+// chol_big / chol_dbuf / chol_smem for an n x n system
+void dense_solve_config(int n, DenseSolve& ds) {
+    // forward phase: the panel; backward phase: one or (if it fits) two (inverse block, row block) buffers
+    const size_t fixed = chol_fixed_doubles(n), panel = chol_panel_doubles(n), back = chol_back_doubles(n) - 32 * 33;
+    const size_t one = (fixed + std::max(panel, back)) * sizeof(double);
+    const size_t two = (fixed + std::max(panel, back + chol_back_doubles(n))) * sizeof(double);
+    ds.chol_big = one > (size_t)kCholMaxDynSmem ? 1 : 0;   // panel does not fit: multi-launch fallback (k_chol_big_*)
+    ds.chol_dbuf = two <= (size_t)kCholMaxDynSmem ? 1 : 0;
+    ds.chol_smem = ds.chol_big ? 0 : (ds.chol_dbuf ? two : one);
+}
+
 struct BaInputs {   // all host pointers, or all device pointers (obs_x_right may be null)
     const double* poses; const uint8_t* fixed; const double* points; const int32_t* obs_kf; const int32_t* obs_lm;
     const float* obs_xy; const float* obs_x_right; const float* inv_sigma_sq;
@@ -2807,13 +2836,9 @@ int prepare_impl(ovs_optimizer* h, const ovs_camera* cam, int setup_is_mono, int
     pl.K = K; pl.L = L; pl.M = M; pl.nfree = nfree; pl.n = n; pl.npairs = npairs; pl.nb_obs = nb_obs; pl.nb_upd = nb_upd;
     pl.npair_entries = npair_entries;
     {
-        // forward phase: the panel; backward phase: one or (if it fits) two (inverse block, row block) buffers
-        const size_t fixed = chol_fixed_doubles(n), panel = chol_panel_doubles(n), back = chol_back_doubles(n) - 32 * 33;
-        const size_t one = (fixed + std::max(panel, back)) * sizeof(double);
-        const size_t two = (fixed + std::max(panel, back + chol_back_doubles(n))) * sizeof(double);
-        pl.chol_big = one > (size_t)kCholMaxDynSmem ? 1 : 0;   // panel does not fit: multi-launch fallback (k_chol_big_*)
-        pl.chol_dbuf = two <= (size_t)kCholMaxDynSmem ? 1 : 0;
-        pl.chol_smem = pl.chol_big ? 0 : (pl.chol_dbuf ? two : one);
+        DenseSolve ds{};
+        dense_solve_config(n, ds);
+        pl.chol_big = ds.chol_big; pl.chol_dbuf = ds.chol_dbuf; pl.chol_smem = ds.chol_smem;
     }
     pl.hposes = hposes; pl.hpoints = hpoints; pl.hout = hout;
     pl.dposes_in = dposes_in; pl.dpoints_in = dpoints_in;
@@ -2869,6 +2894,136 @@ int wait_for_run(ovs_optimizer* h, cudaEvent_t done, const volatile uint8_t* for
         if (*force_stop_flag) *(volatile int*)(h->h_mirror + 2) = 1;
         if (blocking) { struct timespec ts = {0, 50000}; nanosleep(&ts, nullptr); } else sched_yield();
     }
+    return OVS_OK;
+}
+
+int launch_dense_solve(ovs_optimizer* h, cudaStream_t st, LmCtl* ctl, const DenseSolve& ds) {
+    const int n = ds.n;
+    if (!ds.chol_big) {
+        cudaLaunchConfig_t cfg = {};
+        cfg.gridDim = dim3((unsigned)(h->chol_cluster * kSpec));
+        cfg.blockDim = dim3(kCholThreads);
+        cfg.dynamicSmemBytes = ds.chol_smem;
+        cfg.stream = st;
+        cudaLaunchAttribute at[1];
+        at[0].id = cudaLaunchAttributeClusterDimension;
+        at[0].val.clusterDim.x = (unsigned)h->chol_cluster; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+        cfg.attrs = at; cfg.numAttrs = 1;
+        OVS_CUDA_CHECK(cudaLaunchKernelEx(&cfg, k_ba_cholesky_solve, (const LmCtl*)ctl, ds.S, ds.S_stride, n, ds.x, ds.invL, ds.invL_stride, ds.fail, ds.clk, ds.chol_dbuf));
+        ovs::count_launch();
+    } else {
+        for (int kb = 0; kb < n; kb += kNB) {
+            const int nb = std::min(kNB, n - kb), rem = n - kb - nb, prow = rem + 1;
+            k_chol_big_diag<<<dim3(1, kSpec), 64, 0, st>>>(ctl, ds.S, ds.S_stride, n, kb, nb, ds.invL, ds.invL_stride, ds.fail);
+            OVS_LAUNCH_CHECK();
+            k_chol_big_panel<<<dim3((prow + 127) / 128, kSpec), 128, 0, st>>>(ctl, ds.S, ds.S_stride, n, kb, nb, ds.invL, ds.invL_stride);
+            OVS_LAUNCH_CHECK();
+            if (rem > 0) {
+                int tiles = 0;
+                for (int mi = 0; mi < (prow + 15) / 16; ++mi) tiles += std::min((rem + 31) / 32, (16 * mi + 15) / 32 + 1);
+                k_chol_big_trailing<<<dim3((tiles + 3) / 4, kSpec), 128, 0, st>>>(ctl, ds.S, ds.S_stride, n, kb, nb);
+                OVS_LAUNCH_CHECK();
+            }
+        }
+        const size_t bsm = (size_t)(((n + 31) / 32) * 32 + 32 * 33 + 32) * sizeof(double);
+        k_chol_big_backsolve<<<kSpec, 512, bsm, st>>>(ctl, ds.S, ds.S_stride, n, ds.invL, ds.invL_stride, ds.x, ds.fail);
+        OVS_LAUNCH_CHECK();
+    }
+    return OVS_OK;
+}
+
+// The host side of one SparseOptimizer::optimize(iterations) call of the device-side Levenberg loop (LmCtl, k_ba_reduce):
+// per iteration a static launch sequence (iteration_head: linearise, plan, the first trial batch), enqueued for all iterations
+// at once (or replayed as a CUDA graph), one wait per round, and the rare path where a whole batch was rejected and the
+// device halted.  The bundle adjusters (run_impl) and the pose graph (ovs_graph_optimize_host) differ only in the callbacks.
+struct LmDriver {
+    ovs_optimizer* h = nullptr; cudaStream_t st = nullptr; LmCtl* ctl = nullptr;
+    const volatile int* stop_word = nullptr; double* maxdiag = nullptr; volatile int* mirror = nullptr; volatile int* hm = nullptr;
+    bool host_sync = false, use_graph = false;
+    std::function<int()> errors_at_current;                       // currentChi at the start of the round
+    std::function<int(bool in_graph, bool halt_if_undecided)> iteration_head;
+    std::function<int(bool in_graph, bool halt_if_undecided, int next_width_cap)> trial_batch;
+    std::function<int()> wait_device;                             // waits for everything enqueued so far
+};
+
+int lm_round(LmDriver& D, int iterations, int use_huber) {
+    ovs_optimizer* const h = D.h;
+    const cudaStream_t st = D.st;
+    LmCtl* const ctl = D.ctl;
+    volatile int* const hm = D.hm;
+    // the remaining trial batches of an iteration whose first batch was rejected entirely: enqueue one, look, repeat
+    auto finish_iteration = [&]() -> int {
+        for (;;) {
+            int rc = D.wait_device();
+            if (rc != OVS_OK) return rc;
+            if (hm[0] == 0) return OVS_OK;       // decided (or the round is over)
+            rc = D.trial_batch(false, false, 0);
+            if (rc != OVS_OK) return rc;
+        }
+    };
+    k_lm_round_begin<<<1, 1, 0, st>>>(ctl, iterations, use_huber, D.stop_word, D.maxdiag, D.mirror);
+    OVS_LAUNCH_CHECK();
+    if (iterations > 0) {
+        const int rc = D.errors_at_current();
+        if (rc != OVS_OK) return rc;
+    }
+    bool captured = false;
+    int it0 = 0;
+    while (it0 < iterations) {
+        if (D.host_sync) {
+            // one iteration at a time, the host deciding what to launch next
+            int rc = D.iteration_head(false, false);
+            if (rc != OVS_OK) return rc;
+            rc = finish_iteration();
+            if (rc != OVS_OK) return rc;
+            if (hm[1] == 0) break;            // ok == false, stopped, or the budget is used up
+            it0 = hm[4];
+            continue;
+        }
+        // optimistic: all remaining iterations, one batch each, no host round trip
+        for (int it = it0; it < iterations; ++it) {
+            if (D.use_graph) {
+                if (!captured) {
+                    // the iteration's launch sequence does not depend on the iteration: capture it once per round
+                    // (grids are those of the prepared problem), update-or-instantiate, then replay
+                    OVS_CUDA_CHECK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+                    const int rc_body = D.iteration_head(true, true);
+                    cudaGraph_t g = nullptr;
+                    const cudaError_t ce = cudaStreamEndCapture(st, &g);
+                    if (rc_body != OVS_OK) { if (g) cudaGraphDestroy(g); return rc_body; }
+                    OVS_CUDA_CHECK(ce);
+                    if (h->gx_iter) {
+                        cudaGraphExecUpdateResultInfo info;
+                        if (cudaGraphExecUpdate(h->gx_iter, g, &info) != cudaSuccess) { cudaGetLastError(); cudaGraphExecDestroy(h->gx_iter); h->gx_iter = nullptr; }
+                    }
+                    if (!h->gx_iter) {
+                        const cudaError_t ie = cudaGraphInstantiate(&h->gx_iter, g, 0);
+                        if (ie != cudaSuccess) { cudaGraphDestroy(g); OVS_CUDA_CHECK(ie); }
+                    }
+                    cudaGraphDestroy(g);
+                    captured = true;
+                }
+                OVS_CUDA_CHECK(cudaGraphLaunch(h->gx_iter, st));
+            } else {
+                const int rc = D.iteration_head(false, true);
+                if (rc != OVS_OK) return rc;
+            }
+        }
+        int rc = D.wait_device();
+        if (rc != OVS_OK) return rc;
+        if (hm[3] == 0) break;                // every iteration was decided by its first batch: the round is complete
+        // rare path: an iteration had its whole first batch rejected and the device halted there
+        k_lm_resume<<<1, 1, 0, st>>>(ctl, D.mirror);
+        OVS_LAUNCH_CHECK();
+        rc = D.trial_batch(false, false, 0);
+        if (rc != OVS_OK) return rc;
+        rc = finish_iteration();
+        if (rc != OVS_OK) return rc;
+        if (hm[1] == 0) break;
+        it0 = hm[4];
+    }
+    k_lm_round_end<<<1, 1, 0, st>>>(ctl, D.stop_word, D.mirror);
+    OVS_LAUNCH_CHECK();
     return OVS_OK;
 }
 
@@ -2948,36 +3103,9 @@ int run_impl(ovs_optimizer* h, int rounds, int huber_first, int num_first_iter, 
         k_ba_schur_final<<<dim3(npairs, kSpec), 64, 0, st>>>(n, ctl, pl.dpair_chunk_begin, pl.dpab, pl.dspart, pl.spart_stride, pl.dHpp, pl.dbp, pl.dS, pl.S_stride);
         OVS_LAUNCH_CHECK();
         if (ev) OVS_CUDA_CHECK(cudaEventRecord(h->solver_ev[4 * slot + 1], st));     // end of the Schur complement = start of the solver
-        if (!pl.chol_big) {
-            cudaLaunchConfig_t cfg = {};
-            cfg.gridDim = dim3((unsigned)(h->chol_cluster * kSpec));
-            cfg.blockDim = dim3(kCholThreads);
-            cfg.dynamicSmemBytes = pl.chol_smem;
-            cfg.stream = st;
-            cudaLaunchAttribute at[1];
-            at[0].id = cudaLaunchAttributeClusterDimension;
-            at[0].val.clusterDim.x = (unsigned)h->chol_cluster; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-            cfg.attrs = at; cfg.numAttrs = 1;
-            OVS_CUDA_CHECK(cudaLaunchKernelEx(&cfg, k_ba_cholesky_solve, (const LmCtl*)ctl, pl.dS, pl.S_stride, n, pl.dx, pl.dinvL, pl.invL_stride, pl.dfail, pl.dclk, pl.chol_dbuf));
-            ovs::count_launch();
-        } else {
-            for (int kb = 0; kb < n; kb += kNB) {
-                const int nb = std::min(kNB, n - kb), rem = n - kb - nb, prow = rem + 1;
-                k_chol_big_diag<<<dim3(1, kSpec), 64, 0, st>>>(ctl, pl.dS, pl.S_stride, n, kb, nb, pl.dinvL, pl.invL_stride, pl.dfail);
-                OVS_LAUNCH_CHECK();
-                k_chol_big_panel<<<dim3((prow + 127) / 128, kSpec), 128, 0, st>>>(ctl, pl.dS, pl.S_stride, n, kb, nb, pl.dinvL, pl.invL_stride);
-                OVS_LAUNCH_CHECK();
-                if (rem > 0) {
-                    int tiles = 0;
-                    for (int mi = 0; mi < (prow + 15) / 16; ++mi) tiles += std::min((rem + 31) / 32, (16 * mi + 15) / 32 + 1);
-                    k_chol_big_trailing<<<dim3((tiles + 3) / 4, kSpec), 128, 0, st>>>(ctl, pl.dS, pl.S_stride, n, kb, nb);
-                    OVS_LAUNCH_CHECK();
-                }
-            }
-            const size_t bsm = (size_t)(((n + 31) / 32) * 32 + 32 * 33 + 32) * sizeof(double);
-            k_chol_big_backsolve<<<kSpec, 512, bsm, st>>>(ctl, pl.dS, pl.S_stride, n, pl.dinvL, pl.invL_stride, pl.dx, pl.dfail);
-            OVS_LAUNCH_CHECK();
-        }
+        const DenseSolve ds{pl.dS, pl.S_stride, n, pl.dx, pl.dinvL, pl.invL_stride, pl.dfail, pl.dclk, pl.chol_big, pl.chol_dbuf, pl.chol_smem};
+        const int rc_solve = launch_dense_solve(h, st, ctl, ds);
+        if (rc_solve != OVS_OK) return rc_solve;
         if (ev) OVS_CUDA_CHECK(cudaEventRecord(h->solver_ev[4 * slot + 3], st));
         k_ba_update<<<nb_upd, 128, 0, st>>>(P, ctl, pl.dHpl, pl.dHll, pl.dbl, pl.dbp, pl.dx, pl.dposes_ring, pl.dpoints_ring, pl.dpscale, pl.dfail);
         OVS_LAUNCH_CHECK();
@@ -3009,87 +3137,22 @@ int run_impl(ovs_optimizer* h, int rounds, int huber_first, int num_first_iter, 
         return trial_batch(in_graph, halt_if_undecided, 0);
     };
 
-    // the remaining trial batches of an iteration whose first batch was rejected entirely: enqueue one, look, repeat
-    auto finish_iteration = [&]() -> int {
-        for (;;) {
-            int rc = wait_device();
-            if (rc != OVS_OK) return rc;
-            if (hm[0] == 0) return OVS_OK;       // decided (or the round is over)
-            rc = trial_batch(false, false, 0);
-            if (rc != OVS_OK) return rc;
-        }
-    };
-
-    // SparseOptimizer::optimize(iterations) with OptimizationAlgorithmLevenberg
-    auto lm_optimize = [&](int iterations, int use_huber) -> int {
-        k_lm_round_begin<<<1, 1, 0, st>>>(ctl, iterations, use_huber, stop_word, pl.dmaxdiag, mirror);
+    LmDriver drv;
+    drv.h = h; drv.st = st; drv.ctl = ctl; drv.stop_word = stop_word; drv.maxdiag = pl.dmaxdiag; drv.mirror = mirror; drv.hm = hm;
+    drv.host_sync = host_sync; drv.use_graph = use_graph;
+    drv.errors_at_current = [&]() -> int {
+        // computeActiveErrors + activeRobustChi2 at the current estimate (errors go to slot 0)
+        k_ba_errors<<<dim3(nb_obs, 1), 128, 0, st>>>(P, ctl, 1, pl.derr, pl.dpchi);
         OVS_LAUNCH_CHECK();
-        if (iterations > 0) {
-            // computeActiveErrors + activeRobustChi2 at the current estimate (errors go to slot 0)
-            k_ba_errors<<<dim3(nb_obs, 1), 128, 0, st>>>(P, ctl, 1, pl.derr, pl.dpchi);
-            OVS_LAUNCH_CHECK();
-            k_ba_reduce<<<1, kSpec * 256, 0, st>>>(ctl, 0, pl.dpchi, nb_obs, pl.dpscale, 0, pl.dfail, stop_word, -1, nullptr, nullptr, 0, 0);
-            OVS_LAUNCH_CHECK();
-        }
-        bool captured = false;
-        int it0 = 0;
-        while (it0 < iterations) {
-            if (host_sync) {
-                // one iteration at a time, the host deciding what to launch next
-                int rc = iteration_head(false, false);
-                if (rc != OVS_OK) return rc;
-                rc = finish_iteration();
-                if (rc != OVS_OK) return rc;
-                if (hm[1] == 0) break;            // ok == false, stopped, or the budget is used up
-                it0 = hm[4];
-                continue;
-            }
-            // optimistic: all remaining iterations, one batch each, no host round trip
-            for (int it = it0; it < iterations; ++it) {
-                if (use_graph) {
-                    if (!captured) {
-                        // the iteration's launch sequence does not depend on the iteration: capture it once per round
-                        // (grids are those of the prepared problem), update-or-instantiate, then replay
-                        OVS_CUDA_CHECK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-                        const int rc_body = iteration_head(true, true);
-                        cudaGraph_t g = nullptr;
-                        const cudaError_t ce = cudaStreamEndCapture(st, &g);
-                        if (rc_body != OVS_OK) { if (g) cudaGraphDestroy(g); return rc_body; }
-                        OVS_CUDA_CHECK(ce);
-                        if (h->gx_iter) {
-                            cudaGraphExecUpdateResultInfo info;
-                            if (cudaGraphExecUpdate(h->gx_iter, g, &info) != cudaSuccess) { cudaGetLastError(); cudaGraphExecDestroy(h->gx_iter); h->gx_iter = nullptr; }
-                        }
-                        if (!h->gx_iter) {
-                            const cudaError_t ie = cudaGraphInstantiate(&h->gx_iter, g, 0);
-                            if (ie != cudaSuccess) { cudaGraphDestroy(g); OVS_CUDA_CHECK(ie); }
-                        }
-                        cudaGraphDestroy(g);
-                        captured = true;
-                    }
-                    OVS_CUDA_CHECK(cudaGraphLaunch(h->gx_iter, st));
-                } else {
-                    const int rc = iteration_head(false, true);
-                    if (rc != OVS_OK) return rc;
-                }
-            }
-            int rc = wait_device();
-            if (rc != OVS_OK) return rc;
-            if (hm[3] == 0) break;                // every iteration was decided by its first batch: the round is complete
-            // rare path: an iteration had its whole first batch rejected and the device halted there
-            k_lm_resume<<<1, 1, 0, st>>>(ctl, mirror);
-            OVS_LAUNCH_CHECK();
-            rc = trial_batch(false, false, 0);
-            if (rc != OVS_OK) return rc;
-            rc = finish_iteration();
-            if (rc != OVS_OK) return rc;
-            if (hm[1] == 0) break;
-            it0 = hm[4];
-        }
-        k_lm_round_end<<<1, 1, 0, st>>>(ctl, stop_word, mirror);
+        k_ba_reduce<<<1, kSpec * 256, 0, st>>>(ctl, 0, pl.dpchi, nb_obs, pl.dpscale, 0, pl.dfail, stop_word, -1, nullptr, nullptr, 0, 0);
         OVS_LAUNCH_CHECK();
         return OVS_OK;
     };
+    drv.iteration_head = iteration_head;
+    drv.trial_batch = trial_batch;
+    drv.wait_device = wait_device;
+    // SparseOptimizer::optimize(iterations) with OptimizationAlgorithmLevenberg
+    auto lm_optimize = [&](int iterations, int use_huber) -> int { return lm_round(drv, iterations, use_huber); };
 
     int rc = lm_optimize(num_first_iter, huber_first);
     if (rc != OVS_OK) return rc;
@@ -3340,3 +3403,469 @@ extern "C" void ovs_optimizer_destroy(ovs_optimizer* h) {
     delete h;
 }
 
+
+// ================================================================================ pose graph
+// optimize::graph_optimizer::optimize (loop closure): one Sim3 vertex per keyframe, relative Sim3 edges with identity
+// information, g2o's Levenberg with the user lambda 1e-16, then the write-back of the poses and the landmark correction.
+// Per Levenberg iteration (state in LmCtl, the same device-side controller as the bundle adjusters):
+//   k_pg_linearize   per edge: e = log(S_ji S_i S_j^-1), J_i, J_j (sim3_math.cuh) -> H_ii, H_ij, H_jj, b_i, b_j
+//   k_pg_plan        lambda_0 and the damping values of the first trial batch
+//  per trial batch (up to 4 damping values):
+//   k_pg_assemble    per block pair (r >= c) and trial: the whole lower triangle of H + lambda I and the rhs row, summed over the
+//                    pair's edge list (edges sorted by block pair once per call, stable) in a fixed order -- no atomics
+//   dense solver     the local BA's: k_ba_cholesky_solve (7 n_free <= 688) or k_chol_big_* above
+//   k_pg_update      per vertex: S <- exp(x) S into the candidate slots, LM scale terms
+//   k_pg_errors      per edge: chi2 at each candidate;  k_ba_reduce: the Levenberg decision
+// Finish: k_pg_finish writes the optimised Sim3s, pose_cw = {R, t / s} and the corrected landmarks.
+namespace {
+
+constexpr int kPgBlk = 161;   // per-edge linearisation: H_ii, H_ij, H_jj (7 x 7 row-major each), b_i, b_j
+
+struct PgDev {
+    int K, E, nfree, n, fix_scale;      // n: pitch of a trial's solution in x (the system's row pitch)
+    double* ring;                                       // (kSpec + 1) x K x 13: current estimate and candidates
+    const int* free_idx;                                // K: block of a free vertex, -1 for fixed and isolated vertices
+    const int* ei; const int* ej; const double* meas;   // E, E, E x 13 (S_ji)
+};
+
+__host__ __device__ __forceinline__ int pg_pair_id(int r, int c) { return r * (r + 1) / 2 + c; }   // block pair r >= c
+
+// Edge list entries by block pair: per edge up to three (edge << 2 | role) -- role 0: H_ii on (a, a), 1: H_jj on (b, b),
+// 2: H_ij on (a, b) with a > b, 3: H_ij' on (b, a) with b > a -- and the key `sentinel` for the slots an edge does not use.
+__global__ void __launch_bounds__(256) k_pg_emit(PgDev P, unsigned sentinel, unsigned* __restrict__ keys, unsigned long long* __restrict__ vals) {
+    const int e = blockIdx.x * 256 + threadIdx.x;
+    if (e >= P.E) return;
+    const int a = P.free_idx[P.ei[e]], b = P.free_idx[P.ej[e]];
+    const unsigned long long v = (unsigned long long)e << 2;
+    keys[3 * (size_t)e] = a >= 0 ? (unsigned)pg_pair_id(a, a) : sentinel;
+    vals[3 * (size_t)e] = v;
+    keys[3 * (size_t)e + 1] = b >= 0 ? (unsigned)pg_pair_id(b, b) : sentinel;
+    vals[3 * (size_t)e + 1] = v | 1;
+    unsigned k2 = sentinel;
+    unsigned long long v2 = v | 2;
+    if (a >= 0 && b >= 0) {
+        if (a > b) k2 = (unsigned)pg_pair_id(a, b);
+        else { k2 = (unsigned)pg_pair_id(b, a); v2 = v | 3; }
+    }
+    keys[3 * (size_t)e + 2] = k2;
+    vals[3 * (size_t)e + 2] = v2;
+}
+
+__device__ __forceinline__ void pg_load13(const double* src, double* dst) {
+#pragma unroll
+    for (int k = 0; k < 13; ++k) dst[k] = src[k];
+}
+
+// one thread per edge with at least one free vertex
+__global__ void __launch_bounds__(128) k_pg_linearize(PgDev P, const LmCtl* __restrict__ ctl, double* __restrict__ blk) {
+    if (!ctl->active) return;
+    const int e = blockIdx.x * 128 + threadIdx.x;
+    if (e >= P.E) return;
+    const int i = P.ei[e], j = P.ej[e];
+    if (P.free_idx[i] < 0 && P.free_idx[j] < 0) return;
+    const double* S = P.ring + (size_t)ctl->cur * 13 * P.K;
+    double Sji[13], Si[13], Sj[13], err[7], J[98];
+    pg_load13(P.meas + 13 * (size_t)e, Sji);
+    pg_load13(S + 13 * (size_t)i, Si);
+    pg_load13(S + 13 * (size_t)j, Sj);
+    ovs::graph_edge(Sji, Si, Sj, err, J);
+    double* o = blk + (size_t)kPgBlk * e;
+    for (int r = 0; r < 7; ++r)
+        for (int c = 0; c < 7; ++c) {
+            double hii = 0.0, hij = 0.0, hjj = 0.0;
+            for (int k = 0; k < 7; ++k) {
+                hii += J[14 * k + r] * J[14 * k + c];
+                hij += J[14 * k + r] * J[14 * k + 7 + c];
+                hjj += J[14 * k + 7 + r] * J[14 * k + 7 + c];
+            }
+            o[7 * r + c] = hii; o[49 + 7 * r + c] = hij; o[98 + 7 * r + c] = hjj;
+        }
+    for (int r = 0; r < 7; ++r) {
+        double gi = 0.0, gj = 0.0;
+        for (int k = 0; k < 7; ++k) { gi += J[14 * k + r] * err[k]; gj += J[14 * k + 7 + r] * err[k]; }
+        o[147 + r] = -gi; o[154 + r] = -gj;      // b = -J' e
+    }
+}
+
+// One block per block pair (r >= c) and trial of the batch: element (7r + ri, 7c + ci) of H + lambda I, and on diagonal pairs
+// the rhs row (row n).  Every element of the lower triangle is rewritten, zero blocks included: the factorisation works in
+// place.  The pair's entries are summed in their sorted (edge) order.
+// n is the system's row pitch: 7 x free vertices, plus one decoupled row (identity, rhs 0, solution 0) when that is odd, because
+// the cluster Cholesky loads its rows 16 bytes at a time.  Block pid == npairs writes that row.
+__global__ void __launch_bounds__(64) k_pg_assemble(int n, int npairs, const LmCtl* __restrict__ ctl, const int* __restrict__ seg_begin,
+                                                    const int* __restrict__ seg_end, const unsigned long long* __restrict__ ent,
+                                                    const double* __restrict__ blk, double* __restrict__ S, size_t S_stride,
+                                                    double* __restrict__ bvec) {
+    const int bt = blockIdx.y;
+    if (bt >= ctl->nbatch) return;
+    const double lambda = ctl->lam[bt];
+    const int pid = blockIdx.x, t = threadIdx.x;
+    if (pid >= npairs) {
+        S += (size_t)bt * S_stride;
+        for (int c = t; c < n; c += 64) S[(size_t)(n - 1) * n + c] = c == n - 1 ? 1.0 : 0.0;
+        if (t == 0) S[(size_t)n * n + n - 1] = 0.0;
+        return;
+    }
+    int r = (int)((sqrt(8.0 * pid + 1.0) - 1.0) * 0.5);
+    while (pg_pair_id(r, 0) > pid) --r;
+    while (pg_pair_id(r + 1, 0) <= pid) ++r;
+    const int c = pid - pg_pair_id(r, 0);
+    const bool diag = r == c;
+    if (t >= 56 || (t >= 49 && !diag)) return;
+    S += (size_t)bt * S_stride;
+    const int s0 = seg_begin[pid], s1 = seg_end[pid];
+    double v = 0.0;
+    if (t < 49) {
+        const int ri = t / 7, ci = t - 7 * ri;
+        for (int s = s0; s < s1; ++s) {
+            const unsigned long long x = ent[s];
+            const double* o = blk + (size_t)kPgBlk * (size_t)(x >> 2);
+            const int role = (int)(x & 3);
+            v += role == 0 ? o[t] : role == 1 ? o[98 + t] : role == 2 ? o[49 + t] : o[49 + 7 * ci + ri];
+        }
+        if (diag && ri == ci) v += lambda;
+        S[(size_t)(7 * r + ri) * n + 7 * c + ci] = v;
+    } else {
+        const int k = t - 49;
+        for (int s = s0; s < s1; ++s) {
+            const unsigned long long x = ent[s];
+            const double* o = blk + (size_t)kPgBlk * (size_t)(x >> 2);
+            v += (x & 3) == 0 ? o[147 + k] : o[154 + k];
+        }
+        S[(size_t)n * n + 7 * r + k] = v;
+        if (bt == 0) bvec[7 * r + k] = v;
+    }
+}
+
+// g2o's setUserLambdaInit(1e-16): the first iteration's damping is the user lambda, not 1e-5 max diag(H)
+__global__ void k_pg_plan(LmCtl* ctl, int* fail, volatile int* mirror) {
+    if (ctl->need_more) return;     // halted: the parked batch of the undecided iteration must survive
+    lm_plan_iteration(ctl, 1e-16, nullptr, fail, mirror);
+}
+
+// one thread per vertex: the candidate of every trial of the batch (free vertices S <- exp(x) S, the others copied) and the
+// LM scale terms x (lambda x + b) over all seven components, one partial per block and trial
+__global__ void __launch_bounds__(128) k_pg_update(PgDev P, const LmCtl* __restrict__ ctl, const double* __restrict__ x,
+                                                   const double* __restrict__ bvec, double* __restrict__ partial_scale) {
+    __shared__ double sm[36];
+    const int nbatch = ctl->nbatch;
+    if (nbatch == 0) return;
+    const int k = blockIdx.x * 128 + threadIdx.x;
+    double sc[kSpec];
+#pragma unroll
+    for (int bt = 0; bt < kSpec; ++bt) sc[bt] = 0.0;
+    if (k < P.K) {
+        const int fi = P.free_idx[k];
+        double S[13];
+        pg_load13(P.ring + (size_t)ctl->cur * 13 * P.K + 13 * (size_t)k, S);
+        for (int bt = 0; bt < nbatch; ++bt) {
+            const double lambda = ctl->lam[bt];
+            double out[13];
+            if (fi >= 0) {
+                double u[7];
+                for (int q = 0; q < 7; ++q) {
+                    u[q] = x[(size_t)bt * P.n + 7 * fi + q];
+                    sc[bt] += u[q] * (lambda * u[q] + bvec[7 * fi + q]);
+                }
+                ovs::sim3_oplus(S, u, P.fix_scale != 0, out);
+            } else {
+                for (int q = 0; q < 13; ++q) out[q] = S[q];
+            }
+            double* dst = P.ring + (size_t)ctl->buf[bt] * 13 * P.K + 13 * (size_t)k;
+            for (int q = 0; q < 13; ++q) dst[q] = out[q];
+        }
+    }
+#pragma unroll
+    for (int bt = 0; bt < kSpec; ++bt) {
+        if (bt < nbatch) {          // block-uniform
+            const double tot = block_sum(sc[bt], sm);
+            if (threadIdx.x == 0) partial_scale[(size_t)bt * gridDim.x + blockIdx.x] = tot;
+        }
+    }
+}
+
+// chi2 = e'e per edge (every edge, also those between fixed vertices), one partial per block; at_current: the current estimate
+__global__ void __launch_bounds__(128) k_pg_errors(PgDev P, const LmCtl* __restrict__ ctl, int at_current, double* __restrict__ partial_chi) {
+    __shared__ double sm[36];
+    int slot;
+    if (at_current) {
+        if (!ctl->active) return;
+        slot = ctl->cur;
+    } else {
+        if ((int)blockIdx.y >= ctl->nbatch) return;
+        slot = ctl->buf[blockIdx.y];
+    }
+    partial_chi += (size_t)blockIdx.y * gridDim.x;
+    const int e = blockIdx.x * 128 + threadIdx.x;
+    double c = 0.0;
+    if (e < P.E) {
+        const double* S = P.ring + (size_t)slot * 13 * P.K;
+        double Sji[13], Si[13], Sj[13], err[7];
+        pg_load13(P.meas + 13 * (size_t)e, Sji);
+        pg_load13(S + 13 * (size_t)P.ei[e], Si);
+        pg_load13(S + 13 * (size_t)P.ej[e], Sj);
+        ovs::graph_edge(Sji, Si, Sj, err, nullptr);
+        for (int k = 0; k < 7; ++k) c += err[k] * err[k];
+    }
+    const double tot = block_sum(c, sm);
+    if (threadIdx.x == 0) partial_chi[blockIdx.x] = tot;
+}
+
+// Write-back, one thread per vertex and per landmark: the optimised Sim3s, pose_cw = {R, t / s}, and
+// p <- S_wr^opt (S_rw^init p) for a landmark with reference vertex r (ref = -1: the landmark's bits stay).
+// ctl == null: no optimisation ran, the estimate is ring slot 0.
+__global__ void __launch_bounds__(128) k_pg_finish(PgDev P, const LmCtl* __restrict__ ctl, const double* __restrict__ sim3_init,
+                                                   double* __restrict__ sim3_out, double* __restrict__ pose_out, int L,
+                                                   const double* __restrict__ lm_in, const int* __restrict__ lm_ref, double* __restrict__ lm_out) {
+    const int t = blockIdx.x * 128 + threadIdx.x;
+    const double* cur = P.ring + (size_t)(ctl ? ctl->cur : 0) * 13 * P.K;
+    if (t < P.K) {
+        double S[13];
+        pg_load13(cur + 13 * (size_t)t, S);
+        for (int q = 0; q < 13; ++q) sim3_out[13 * (size_t)t + q] = S[q];
+        for (int q = 0; q < 9; ++q) pose_out[12 * (size_t)t + q] = S[q];
+        for (int q = 0; q < 3; ++q) pose_out[12 * (size_t)t + 9 + q] = S[9 + q] / S[12];
+    } else if (t < P.K + L) {
+        const int l = t - P.K, r = lm_ref[l];
+        const double p[3] = {lm_in[3 * (size_t)l], lm_in[3 * (size_t)l + 1], lm_in[3 * (size_t)l + 2]};
+        if (r < 0) {
+            for (int q = 0; q < 3; ++q) lm_out[3 * (size_t)l + q] = p[q];
+            return;
+        }
+        double S0[13], S1[13], Si[13], q0[3], q1[3], pc[3];
+        pg_load13(sim3_init + 13 * (size_t)r, S0);
+        pg_load13(cur + 13 * (size_t)r, S1);
+        ovs::sim3_inverse(S1, Si);
+        ovs::mat3_vec(S0, p, q0);
+        for (int q = 0; q < 3; ++q) pc[q] = S0[12] * q0[q] + S0[9 + q];      // S_rw^init p: camera frame of r
+        ovs::mat3_vec(Si, pc, q1);
+        for (int q = 0; q < 3; ++q) lm_out[3 * (size_t)l + q] = Si[12] * q1[q] + Si[9 + q];
+    }
+}
+
+}  // namespace
+
+extern "C" int ovs_graph_optimize_host(ovs_optimizer* h, int K, double* sim3_cw, const uint8_t* fixed, int E, const int32_t* edge_i,
+                                       const int32_t* edge_j, const double* meas_ji, int fix_scale, int num_iter, int L, double* lm_pos_w,
+                                       const int32_t* lm_ref, double* pose_cw_out, ovs_ba_stats* stats) {
+    OVS_REQUIRE(h && K >= 1 && E >= 0 && L >= 0 && num_iter >= 0, OVS_ERR_INVALID_ARG, "bad argument");
+    OVS_REQUIRE(sim3_cw && fixed && (E == 0 || (edge_i && edge_j && meas_ji)) && (L == 0 || (lm_pos_w && lm_ref)), OVS_ERR_INVALID_ARG,
+                "null argument");
+    auto scale_ok = [](double s) { return s > 0.0 && std::isfinite(s); };
+    for (int k = 0; k < K; ++k)
+        OVS_REQUIRE(scale_ok(sim3_cw[13 * (size_t)k + 12]), OVS_ERR_INVALID_ARG, "vertex %d: the Sim3 scale must be positive and finite", k);
+    for (int e = 0; e < E; ++e) {
+        const int i = edge_i[e], j = edge_j[e];
+        OVS_REQUIRE(i >= 0 && i < K && j >= 0 && j < K, OVS_ERR_INVALID_ARG, "edge %d references a vertex out of range", e);
+        OVS_REQUIRE(i != j, OVS_ERR_INVALID_ARG, "edge %d joins vertex %d to itself", e, i);
+        OVS_REQUIRE(scale_ok(meas_ji[13 * (size_t)e + 12]), OVS_ERR_INVALID_ARG, "edge %d: the Sim3 scale must be positive and finite", e);
+    }
+    for (int l = 0; l < L; ++l)
+        OVS_REQUIRE(lm_ref[l] >= -1 && lm_ref[l] < K, OVS_ERR_INVALID_ARG, "landmark %d references a vertex out of range", l);
+    if (stats) memset(stats, 0, sizeof(*stats));
+    // g2o optimises the vertices of its edges only: a free vertex without an edge is not part of the system
+    std::vector<int> free_idx((size_t)K, -1);
+    {
+        std::vector<uint8_t> used((size_t)K, 0);
+        for (int e = 0; e < E; ++e) { used[edge_i[e]] = 1; used[edge_j[e]] = 1; }
+        int f = 0;
+        for (int k = 0; k < K; ++k)
+            if (used[k] && !fixed[k]) free_idx[k] = f++;
+    }
+    const int nfree = K > 0 ? *std::max_element(free_idx.begin(), free_idx.end()) + 1 : 0;
+    const int n = 7 * nfree;
+    const int nsys = n + (n & 1);      // row pitch of the dense system: even (see k_pg_assemble)
+    OVS_REQUIRE(n <= kMaxReducedDimBig, OVS_ERR_UNSUPPORTED, "more than %d free vertices (dense 7n system)", kMaxReducedDimBig / 7);
+    const bool run_lm = nfree > 0 && num_iter > 0;
+    OVS_CUDA_CHECK(cudaSetDevice(h->device));
+    // carved from the arenas a prepared local-BA problem lives in: that problem is gone
+    invalidate_plan(h);
+    if (h->pending) { OVS_CUDA_CHECK(ovs::sync_stream(h->stream)); h->pending = false; }
+
+    const size_t sK = (size_t)K, sE = (size_t)E, sL = (size_t)L, nent = 3 * sE;
+    const int npairs = nfree * (nfree + 1) / 2;
+    const int nb_edge = (E + 127) / 128, nb_vert = (K + 127) / 128;
+    const int exec_cap = 1024;
+    DenseSolve ds{};
+    dense_solve_config(std::max(nsys, 1), ds);
+    ds.n = nsys;
+    ds.S_stride = ((size_t)(nsys + 1) * nsys + 31) / 32 * 32;
+    ds.invL_stride = (size_t)((nsys + kNB - 1) / kNB) * kNB * kNB;
+
+    double *hS, *hmeas, *hlm, *hS_out, *hpose, *hlm_out; int *hfree, *hei, *hej, *href, *hexec; LmCtl* hctl;
+    double *dS_in, *dmeas, *dlm, *dS_out, *dpose, *dlm_out, *dring, *dblk, *dbvec, *dpchi, *dpscale, *dmaxdiag;
+    int *dfree, *dei, *dej, *dref, *dsegb, *dsege, *dsort, *dfail, *dexec; LmCtl* dctl;
+    unsigned *dkeys, *dkeys2; unsigned long long *dvals, *dvals2;
+    size_t in_bytes = 0;
+    auto carve = [&](Arena& H, Arena& D) {
+        // inputs: the same carving order on both sides -> one contiguous upload
+        hS = H.take<double>(13 * sK); hfree = H.take<int>(sK); hei = H.take<int>(sE); hej = H.take<int>(sE); hmeas = H.take<double>(13 * sE);
+        hlm = H.take<double>(3 * sL); href = H.take<int>(sL);
+        in_bytes = H.off;
+        hS_out = H.take<double>(13 * sK); hpose = H.take<double>(12 * sK); hlm_out = H.take<double>(3 * sL);
+        hctl = H.take<LmCtl>(1); hexec = H.take<int>(exec_cap);
+        dS_in = D.take<double>(13 * sK); dfree = D.take<int>(sK); dei = D.take<int>(sE); dej = D.take<int>(sE); dmeas = D.take<double>(13 * sE);
+        dlm = D.take<double>(3 * sL); dref = D.take<int>(sL);
+        dS_out = D.take<double>(13 * sK); dpose = D.take<double>(12 * sK); dlm_out = D.take<double>(3 * sL);
+        dctl = D.take<LmCtl>(1); dexec = D.take<int>(exec_cap);
+        dring = D.take<double>((kSpec + 1) * 13 * sK);
+        dblk = D.take<double>(kPgBlk * sE);
+        dkeys = D.take<unsigned>(nent); dkeys2 = D.take<unsigned>(nent);
+        dvals = D.take<unsigned long long>(nent); dvals2 = D.take<unsigned long long>(nent);
+        dsort = D.take<int>(sort_scratch_ints((long long)std::max<size_t>(nent, 1)));
+        dsegb = D.take<int>((size_t)npairs + 1); dsege = D.take<int>((size_t)npairs + 1);
+        dbvec = D.take<double>((size_t)std::max(n, 1));
+        dpchi = D.take<double>(kSpec * (size_t)std::max(nb_edge, 1)); dpscale = D.take<double>(kSpec * (size_t)nb_vert);
+        dfail = D.take<int>(kSpec); dmaxdiag = D.take<double>(2);
+    };
+    {
+        Arena H0{nullptr, 0, 0}, D0{nullptr, 0, 0};
+        carve(H0, D0);
+        int rc = ensure_arenas(h, D0.off + 256, H0.off + 256);
+        if (rc != OVS_OK) return rc;
+        if (run_lm) {
+            Arena W0{nullptr, 0, 0};
+            W0.take<double>(kSpec * ds.S_stride); W0.take<double>(kSpec * (size_t)nsys); W0.take<double>(kSpec * ds.invL_stride);
+            rc = ensure_work(h, W0.off + 256);
+            if (rc != OVS_OK) return rc;
+        }
+    }
+    Arena H{h->h_arena, 0, h->h_cap}, D{h->d_arena, 0, h->d_cap};
+    carve(H, D);
+    if (run_lm) {
+        Arena W{h->d_work, 0, h->w_cap};
+        ds.S = W.take<double>(kSpec * ds.S_stride); ds.x = W.take<double>(kSpec * (size_t)nsys); ds.invL = W.take<double>(kSpec * ds.invL_stride);
+        ds.fail = dfail; ds.clk = nullptr;
+    }
+    memcpy(hS, sim3_cw, 104 * sK);
+    memcpy(hfree, free_idx.data(), 4 * sK);
+    if (E) { memcpy(hei, edge_i, 4 * sE); memcpy(hej, edge_j, 4 * sE); memcpy(hmeas, meas_ji, 104 * sE); }
+    if (L) { memcpy(hlm, lm_pos_w, 24 * sL); memcpy(href, lm_ref, 4 * sL); }
+
+    cudaStream_t st = h->stream;
+    h->pending = true;
+    h->h_mirror[0] = 0; h->h_mirror[1] = 0; h->h_mirror[2] = 0;
+    volatile int* const mirror = (volatile int*)h->d_mirror;
+    OVS_CUDA_CHECK(cudaEventRecord(h->ev[0], st));
+    OVS_CUDA_CHECK(cudaMemcpyAsync(h->d_arena, h->h_arena, in_bytes, cudaMemcpyHostToDevice, st));
+    OVS_CUDA_CHECK(cudaMemcpyAsync(dring, dS_in, 104 * sK, cudaMemcpyDeviceToDevice, st));
+    PgDev P;
+    P.K = K; P.E = E; P.nfree = nfree; P.n = nsys; P.fix_scale = fix_scale ? 1 : 0;
+    P.ring = dring; P.free_idx = dfree; P.ei = dei; P.ej = dej; P.meas = dmeas;
+    int solver_slots = 0;
+    const bool time_solver = stats != nullptr;
+    if (run_lm) {
+        // the edge lists of the block pairs: (pair id, edge << 2 | role), stable sort by pair id, segments
+        const unsigned sentinel = (unsigned)npairs;
+        k_pg_emit<<<(E + 255) / 256, 256, 0, st>>>(P, sentinel, dkeys, dvals);
+        OVS_LAUNCH_CHECK();
+        int end_bit = 1;
+        while ((1u << end_bit) <= sentinel) ++end_bit;
+        unsigned* ksorted = nullptr; unsigned long long* vsorted = nullptr;
+        int rc = sort_pairs(st, dkeys, dkeys2, dvals, dvals2, (int)nent, end_bit, dsort, &ksorted, &vsorted);
+        if (rc != OVS_OK) return rc;
+        OVS_CUDA_CHECK(cudaMemsetAsync(dsegb, 0, 4 * ((size_t)npairs + 1), st));
+        OVS_CUDA_CHECK(cudaMemsetAsync(dsege, 0, 4 * ((size_t)npairs + 1), st));
+        k_ba_segments<<<(int)((nent + 255) / 256), 256, 0, st>>>(ksorted, (int)nent, dsegb, dsege);
+        OVS_LAUNCH_CHECK();
+        const int sw = std::min(std::max(h->spec_width, 1), kSpec);
+        k_lm_init<<<1, 1, 0, st>>>(dctl, sw, dfail, mirror);
+        OVS_LAUNCH_CHECK();
+
+        LmDriver drv;
+        drv.h = h; drv.st = st; drv.ctl = dctl; drv.stop_word = nullptr; drv.maxdiag = dmaxdiag; drv.mirror = mirror;
+        drv.hm = (volatile int*)h->h_mirror;
+        drv.host_sync = h->lm_host_sync >= 0 ? h->lm_host_sync != 0 : ds.chol_big != 0;   // as the local BA: skip the ~100-launch batches
+        drv.use_graph = false;
+        drv.errors_at_current = [&]() -> int {
+            k_pg_errors<<<dim3(nb_edge, 1), 128, 0, st>>>(P, dctl, 1, dpchi);
+            OVS_LAUNCH_CHECK();
+            k_ba_reduce<<<1, kSpec * 256, 0, st>>>(dctl, 0, dpchi, nb_edge, dpscale, 0, dfail, nullptr, -1, nullptr, nullptr, 0, 0);
+            OVS_LAUNCH_CHECK();
+            return OVS_OK;
+        };
+        drv.trial_batch = [&](bool in_graph, bool halt_if_undecided, int next_width_cap) -> int {
+            const int slot = solver_slots;
+            const bool ev = time_solver && !in_graph && slot < exec_cap;
+            if (ev) {
+                while (h->solver_ev.size() < 4 * (size_t)(slot + 1)) {
+                    cudaEvent_t e0;
+                    OVS_CUDA_CHECK(cudaEventCreateWithFlags(&e0, cudaEventDefault));
+                    h->solver_ev.push_back(e0);
+                }
+            }
+            k_pg_assemble<<<dim3(npairs + (nsys - n), kSpec), 64, 0, st>>>(nsys, npairs, dctl, dsegb, dsege, vsorted, dblk, ds.S, ds.S_stride, dbvec);
+            OVS_LAUNCH_CHECK();
+            if (ev) OVS_CUDA_CHECK(cudaEventRecord(h->solver_ev[4 * slot + 1], st));
+            const int rc_solve = launch_dense_solve(h, st, dctl, ds);
+            if (rc_solve != OVS_OK) return rc_solve;
+            if (ev) OVS_CUDA_CHECK(cudaEventRecord(h->solver_ev[4 * slot + 3], st));
+            k_pg_update<<<nb_vert, 128, 0, st>>>(P, dctl, ds.x, dbvec, dpscale);
+            OVS_LAUNCH_CHECK();
+            k_pg_errors<<<dim3(nb_edge, kSpec), 128, 0, st>>>(P, dctl, 0, dpchi);
+            OVS_LAUNCH_CHECK();
+            k_ba_reduce<<<1, kSpec * 256, 0, st>>>(dctl, 1, dpchi, nb_edge, dpscale, nb_vert, dfail, nullptr, ev ? slot : -1, dexec, mirror,
+                                                   halt_if_undecided ? 1 : 0, next_width_cap);
+            OVS_LAUNCH_CHECK();
+            if (!in_graph) ++solver_slots;
+            return OVS_OK;
+        };
+        drv.iteration_head = [&](bool in_graph, bool halt_if_undecided) -> int {
+            k_pg_linearize<<<nb_edge, 128, 0, st>>>(P, dctl, dblk);
+            OVS_LAUNCH_CHECK();
+            k_pg_plan<<<1, 1, 0, st>>>(dctl, dfail, mirror);
+            OVS_LAUNCH_CHECK();
+            return drv.trial_batch(in_graph, halt_if_undecided, 0);
+        };
+        drv.wait_device = [&]() -> int { OVS_CUDA_CHECK(ovs::sync_stream(st)); return OVS_OK; };
+        rc = lm_round(drv, num_iter, 0);
+        if (rc != OVS_OK) return rc;
+        OVS_CUDA_CHECK(cudaMemcpyAsync(hctl, dctl, sizeof(LmCtl), cudaMemcpyDeviceToHost, st));
+        const int nslots = std::min(solver_slots, exec_cap);
+        if (time_solver && nslots > 0) OVS_CUDA_CHECK(cudaMemcpyAsync(hexec, dexec, sizeof(int) * (size_t)nslots, cudaMemcpyDeviceToHost, st));
+    } else if (E > 0 && stats) {
+        // nothing to optimise (no free vertex, or num_iter == 0): chi2 at the returned estimates, for the statistics
+        k_lm_init<<<1, 1, 0, st>>>(dctl, 1, dfail, mirror);
+        OVS_LAUNCH_CHECK();
+        k_lm_round_begin<<<1, 1, 0, st>>>(dctl, 1, 0, nullptr, dmaxdiag, mirror);   // active, so that the errors are evaluated
+        OVS_LAUNCH_CHECK();
+        k_pg_errors<<<dim3(nb_edge, 1), 128, 0, st>>>(P, dctl, 1, dpchi);
+        OVS_LAUNCH_CHECK();
+        k_ba_reduce<<<1, kSpec * 256, 0, st>>>(dctl, 0, dpchi, nb_edge, dpscale, 0, dfail, nullptr, -1, nullptr, nullptr, 0, 0);
+        OVS_LAUNCH_CHECK();
+        OVS_CUDA_CHECK(cudaMemcpyAsync(hctl, dctl, sizeof(LmCtl), cudaMemcpyDeviceToHost, st));
+    }
+    k_pg_finish<<<(unsigned)((sK + sL + 127) / 128), 128, 0, st>>>(P, run_lm ? dctl : nullptr, dS_in, dS_out, dpose, L, dlm, dref, dlm_out);
+    OVS_LAUNCH_CHECK();
+    OVS_CUDA_CHECK(cudaEventRecord(h->ev[1], st));
+    OVS_CUDA_CHECK(cudaMemcpyAsync(hS_out, dS_out, 104 * sK, cudaMemcpyDeviceToHost, st));
+    OVS_CUDA_CHECK(cudaMemcpyAsync(hpose, dpose, 96 * sK, cudaMemcpyDeviceToHost, st));
+    if (L) OVS_CUDA_CHECK(cudaMemcpyAsync(hlm_out, dlm_out, 24 * sL, cudaMemcpyDeviceToHost, st));
+    OVS_CUDA_CHECK(ovs::sync_stream(st));
+    h->pending = false;
+    memcpy(sim3_cw, hS_out, 104 * sK);
+    if (pose_cw_out) memcpy(pose_cw_out, hpose, 96 * sK);
+    if (L) memcpy(lm_pos_w, hlm_out, 24 * sL);
+    if (stats) {
+        if (run_lm) {
+            const LmCtl& c = *hctl;
+            stats->num_rounds = c.num_rounds; stats->num_iterations = c.num_iterations; stats->num_trials = c.num_trials;
+            stats->round_iterations[0] = c.round_iterations[0]; stats->lambda_init[0] = c.lambda_init[0];
+            stats->last_lambda = c.last_lambda; stats->last_chi2 = c.last_chi2; stats->final_chi2 = c.last_chi2;
+            stats->solver_launches = c.batches; stats->solver_trials = c.solver_trials;
+            float sum = 0;
+            const int nslots = std::min(solver_slots, exec_cap);
+            for (int i = 0; i < nslots; ++i)
+                if (hexec[i] > 0) { float m = 0; cudaEventElapsedTime(&m, h->solver_ev[4 * i + 1], h->solver_ev[4 * i + 3]); sum += m; }
+            stats->solver_us = sum * 1000.f;
+        } else {
+            // one optimize() call with no iteration; chi2 of an empty graph is 0
+            stats->num_rounds = 1;
+            stats->final_chi2 = stats->last_chi2 = E > 0 ? hctl->currentChi : 0.0;
+        }
+        stats->reduced_dim = n;
+        float ms = 0; cudaEventElapsedTime(&ms, h->ev[0], h->ev[1]);
+        stats->device_us = ms * 1000.f;
+    }
+    return OVS_OK;
+}

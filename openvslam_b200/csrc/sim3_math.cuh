@@ -168,4 +168,202 @@ OVS_BA_HD bool solve7(const double* Hs, double lambda, const double* b, double* 
     return true;
 }
 
+// ------------------------------------------------------------------ pose graph (optimize::graph_optimizer, loop closure)
+// One Sim3 vertex per keyframe (S_iw, camera from world), one relative edge per keyframe pair with the measurement S_ji:
+//   e = log(S_ji S_i S_j^-1),  identity information.
+// Jacobians with respect to the left updates S <- exp(d) S of both vertices, analytic:
+//   J_i = J_l^-1(e) Ad(S_ji),  J_j = -J_l^-1(e) Ad(E),  E = S_ji S_i S_j^-1,  J_l(xi) = phi(ad xi),  phi(x) = (e^x - 1) / x.
+
+// S^-1 = {R', -R' t / s, 1 / s}
+OVS_BA_HD void sim3_inverse(const double* S, double* out) {
+    const double is = 1.0 / S[12];
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) out[3 * i + j] = S[3 * j + i];
+    for (int k = 0; k < 3; ++k) out[9 + k] = -(S[k] * S[9] + S[3 + k] * S[10] + S[6 + k] * S[11]) * is;
+    out[12] = is;
+}
+
+// A B = {R_a R_b, s_a R_a t_b + t_a, s_a s_b}  (out must not alias A or B)
+OVS_BA_HD void sim3_compose(const double* A, const double* B, double* out) {
+    double q[3];
+    mat3_mat3(A, B, out);
+    mat3_vec(A, B + 9, q);
+    for (int k = 0; k < 3; ++k) out[9 + k] = A[12] * q[k] + A[9 + k];
+    out[12] = A[12] * B[12];
+}
+
+// The exact inverse of sim3_exp: sigma = log s; omega from R with the angle atan2(|vee(R - R')| / 2, (tr R - 1) / 2) (accurate
+// near 0 and near pi; near pi the axis comes from the symmetric part of R); upsilon = W^-1 t with W read from sim3_exp itself
+// (its t for upsilon = e_k is W's column k), so that every branch of the exponential is inverted exactly.
+OVS_BA_HD void sim3_log(const double* S, double* xi) {
+    const double* R = S;
+    const double v[3] = {R[7] - R[5], R[2] - R[6], R[3] - R[1]};
+    const double sn = 0.5 * sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
+    const double c = 0.5 * (R[0] + R[4] + R[8] - 1.0);
+    const double theta = atan2(sn, c);
+    if (c > -0.5) {
+        // theta < 2 pi / 3: theta / (2 sin theta) is well conditioned
+        // below 1e-5 sim3_exp takes R = I + O + O^2 / 2, whose vee(R - R') / 2 is omega itself
+        const double f = theta < 1e-5 ? 0.5 : 0.5 * theta / sn;
+        for (int k = 0; k < 3; ++k) xi[k] = f * v[k];
+    } else {
+        // (R + R') / 2 - cos(theta) I = (1 - cos theta) a a'; the axis from its largest diagonal entry, the sign from vee(R - R')
+        const double oc = 1.0 - c;
+        const double B[9] = {R[0] - c, 0.5 * (R[1] + R[3]), 0.5 * (R[2] + R[6]),
+                             0.5 * (R[3] + R[1]), R[4] - c, 0.5 * (R[5] + R[7]),
+                             0.5 * (R[6] + R[2]), 0.5 * (R[7] + R[5]), R[8] - c};
+        int k = 0;
+        if (B[4] > B[0]) k = 1;
+        if (B[8] > B[4 * k]) k = 2;
+        const double ak = sqrt(B[4 * k] / oc);
+        double a[3];
+        for (int m = 0; m < 3; ++m) a[m] = (m == k) ? ak : B[3 * k + m] / (oc * ak);
+        const double sg = (a[0] * v[0] + a[1] * v[1] + a[2] * v[2]) < 0.0 ? -1.0 : 1.0;
+        for (int m = 0; m < 3; ++m) xi[m] = sg * theta * a[m];
+    }
+    xi[6] = log(S[12]);
+    double W[9];
+    for (int col = 0; col < 3; ++col) {
+        double u[7] = {xi[0], xi[1], xi[2], 0.0, 0.0, 0.0, xi[6]}, E[13];
+        u[3 + col] = 1.0;
+        sim3_exp(u, E);
+        for (int r = 0; r < 3; ++r) W[3 * r + col] = E[9 + r];
+    }
+    // upsilon = W^-1 t by the adjugate
+    const double c00 = W[4] * W[8] - W[5] * W[7], c01 = W[5] * W[6] - W[3] * W[8], c02 = W[3] * W[7] - W[4] * W[6];
+    const double c10 = W[2] * W[7] - W[1] * W[8], c11 = W[0] * W[8] - W[2] * W[6], c12 = W[1] * W[6] - W[0] * W[7];
+    const double c20 = W[1] * W[5] - W[2] * W[4], c21 = W[2] * W[3] - W[0] * W[5], c22 = W[0] * W[4] - W[1] * W[3];
+    const double id = 1.0 / (W[0] * c00 + W[1] * c01 + W[2] * c02);
+    const double* t = S + 9;
+    xi[3] = (c00 * t[0] + c10 * t[1] + c20 * t[2]) * id;
+    xi[4] = (c01 * t[0] + c11 * t[1] + c21 * t[2]) * id;
+    xi[5] = (c02 * t[0] + c12 * t[1] + c22 * t[2]) * id;
+}
+
+// Ad(S) (7 x 7 row-major) in the update order (omega, upsilon, sigma): exp(Ad(S) d) = S exp(d) S^-1
+//   [[R, 0, 0], [[t]x R, s R, -t], [0, 0, 1]]
+OVS_BA_HD void sim3_adjoint(const double* S, double* Ad) {
+    for (int k = 0; k < 49; ++k) Ad[k] = 0.0;
+    const double* t = S + 9;
+    const double T[9] = {0, -t[2], t[1], t[2], 0, -t[0], -t[1], t[0], 0};
+    double TR[9];
+    mat3_mat3(T, S, TR);
+    for (int i = 0; i < 3; ++i) {
+        for (int j = 0; j < 3; ++j) {
+            Ad[7 * i + j] = S[3 * i + j];
+            Ad[7 * (3 + i) + j] = TR[3 * i + j];
+            Ad[7 * (3 + i) + 3 + j] = S[12] * S[3 * i + j];
+        }
+        Ad[7 * (3 + i) + 6] = -t[i];
+    }
+    Ad[48] = 1.0;
+}
+
+// ad(xi) = [[[w]x, 0, 0], [[u]x, sigma I + [w]x, -u], [0, 0, 0]]
+OVS_BA_HD void sim3_ad(const double* xi, double* ad) {
+    for (int k = 0; k < 49; ++k) ad[k] = 0.0;
+    const double W[9] = {0, -xi[2], xi[1], xi[2], 0, -xi[0], -xi[1], xi[0], 0};
+    const double U[9] = {0, -xi[5], xi[4], xi[5], 0, -xi[3], -xi[4], xi[3], 0};
+    for (int i = 0; i < 3; ++i) {
+        for (int j = 0; j < 3; ++j) {
+            ad[7 * i + j] = W[3 * i + j];
+            ad[7 * (3 + i) + j] = U[3 * i + j];
+            ad[7 * (3 + i) + 3 + j] = W[3 * i + j] + (i == j ? xi[6] : 0.0);
+        }
+        ad[7 * (3 + i) + 6] = -xi[3 + i];
+    }
+}
+
+// C = A B, 7 x 7 row-major (C must not alias A or B)
+OVS_BA_HD void mat7_mul(const double* A, const double* B, double* C) {
+    for (int i = 0; i < 7; ++i)
+        for (int j = 0; j < 7; ++j) {
+            double s = 0.0;
+            for (int k = 0; k < 7; ++k) s += A[7 * i + k] * B[7 * k + j];
+            C[7 * i + j] = s;
+        }
+}
+
+// phi(A) = sum_k A^k / (k + 1)! of a 7 x 7 matrix by scaling and squaring: A is halved until its infinity norm is <= 1/2,
+// a degree-12 Taylor core (Horner) gives phi there, and phi(2X) = phi(X) (2 I + X phi(X)) / 2 undoes the halving.
+OVS_BA_HD void sim3_phi7(const double* A, double* F) {
+    double nrm = 0.0;
+    for (int i = 0; i < 7; ++i) {
+        double r = 0.0;
+        for (int j = 0; j < 7; ++j) r += fabs(A[7 * i + j]);
+        nrm = fmax(nrm, r);
+    }
+    int sq = 0;
+    double scale = 1.0;
+    while (nrm * scale > 0.5 && sq < 64) { scale *= 0.5; ++sq; }
+    double X[49], T[49];
+    for (int k = 0; k < 49; ++k) X[k] = A[k] * scale;
+    // Horner: F = I / 13!, then F = I / (k + 1)! + X F for k = 11 .. 0
+    double inv_fact[13];
+    inv_fact[0] = 1.0;
+    for (int k = 1; k < 13; ++k) inv_fact[k] = inv_fact[k - 1] / (double)(k + 1);   // inv_fact[k] = 1 / (k + 1)!
+    for (int k = 0; k < 49; ++k) F[k] = (k % 8 == 0) ? inv_fact[12] : 0.0;
+    for (int k = 11; k >= 0; --k) {
+        mat7_mul(X, F, T);
+        for (int m = 0; m < 49; ++m) F[m] = T[m] + ((m % 8 == 0) ? inv_fact[k] : 0.0);
+    }
+    for (int s = 0; s < sq; ++s) {
+        mat7_mul(X, F, T);                                             // X phi(X)
+        for (int m = 0; m < 49; ++m) T[m] = 0.5 * T[m] + ((m % 8 == 0) ? 1.0 : 0.0);   // I + X phi(X) / 2
+        double Fn[49];
+        mat7_mul(F, T, Fn);
+        for (int m = 0; m < 49; ++m) { F[m] = Fn[m]; X[m] = 2.0 * X[m]; }
+    }
+}
+
+// X = M^-1 B for a 7 x 7 M and a 7 x nrhs B (row-major, pitch nrhs) by Gaussian elimination with partial pivoting.
+// M and B are overwritten.  Returns false for a singular M.
+OVS_BA_HD bool solve7_general(double* M, double* B, int nrhs) {
+    for (int c = 0; c < 7; ++c) {
+        int p = c;
+        for (int r = c + 1; r < 7; ++r)
+            if (fabs(M[7 * r + c]) > fabs(M[7 * p + c])) p = r;
+        if (!(fabs(M[7 * p + c]) > 0.0)) return false;
+        if (p != c) {
+            for (int k = 0; k < 7; ++k) { const double tmp = M[7 * c + k]; M[7 * c + k] = M[7 * p + k]; M[7 * p + k] = tmp; }
+            for (int k = 0; k < nrhs; ++k) { const double tmp = B[nrhs * c + k]; B[nrhs * c + k] = B[nrhs * p + k]; B[nrhs * p + k] = tmp; }
+        }
+        const double ip = 1.0 / M[8 * c];
+        for (int r = c + 1; r < 7; ++r) {
+            const double f = M[7 * r + c] * ip;
+            if (f == 0.0) continue;
+            for (int k = c; k < 7; ++k) M[7 * r + k] -= f * M[7 * c + k];
+            for (int k = 0; k < nrhs; ++k) B[nrhs * r + k] -= f * B[nrhs * c + k];
+        }
+    }
+    for (int c = 6; c >= 0; --c) {
+        const double ip = 1.0 / M[8 * c];
+        for (int k = 0; k < nrhs; ++k) {
+            double s = B[nrhs * c + k];
+            for (int m = c + 1; m < 7; ++m) s -= M[7 * c + m] * B[nrhs * m + k];
+            B[nrhs * c + k] = s * ip;
+        }
+    }
+    return true;
+}
+
+// The relative Sim3 edge: e = log(S_ji S_i S_j^-1) (7) and, when J is not null, J = [J_i | J_j] (7 x 14 row-major).
+OVS_BA_HD void graph_edge(const double* S_ji, const double* S_i, const double* S_j, double* e, double* J) {
+    double Sji_i[13], Sj_inv[13], E[13];
+    sim3_compose(S_ji, S_i, Sji_i);
+    sim3_inverse(S_j, Sj_inv);
+    sim3_compose(Sji_i, Sj_inv, E);
+    sim3_log(E, e);
+    if (!J) return;
+    double Jl[49], ad[49], Ad1[49], Ad2[49];
+    sim3_ad(e, ad);
+    sim3_phi7(ad, Jl);
+    sim3_adjoint(S_ji, Ad1);
+    sim3_adjoint(E, Ad2);
+    for (int r = 0; r < 7; ++r)
+        for (int k = 0; k < 7; ++k) { J[14 * r + k] = Ad1[7 * r + k]; J[14 * r + 7 + k] = -Ad2[7 * r + k]; }
+    if (!solve7_general(Jl, J, 14))
+        for (int k = 0; k < 98; ++k) J[k] = 0.0;   // J_l is singular only at |omega| = 2 pi k: not reached by log's output
+}
+
 }  // namespace ovs

@@ -191,6 +191,40 @@ class transform_optimizer(_optimizer_handle):
         return ninl.value, S, flags[:n].astype(bool), _stats(st)
 
 
+class graph_optimizer(_optimizer_handle):
+    """openvslam::optimize::graph_optimizer(fix_scale, num_iter = 50): the loop-closure pose graph over Sim3 vertices."""
+
+    def __init__(self, fix_scale, num_iter=50, device=0):
+        super().__init__(device)
+        self.fix_scale_ = bool(fix_scale)
+        self.num_iter_ = int(num_iter)
+
+    def optimize(self, sim3_cw, fixed, edge_i, edge_j, meas_ji, lm_pos_w=None, lm_ref=None):
+        """sim3_cw[K, 13] = S_iw {R row-major (9), t (3), s}; edges (i, j) with measurements S_ji[E, 13]; landmarks corrected through
+        their reference vertex lm_ref (-1: unchanged).  See include/ovs_b200.h.
+        -> (sim3_cw[K, 13], pose_cw[K, 12], lm_pos_w[L, 3], stats)."""
+        S = np.array(sim3_cw, np.float64).reshape(-1, 13).copy()
+        K = len(S)
+        fixed, pf = _p(np.asarray(fixed).reshape(-1), np.uint8)
+        ei, pi = _p(np.asarray(edge_i).reshape(-1), np.int32); ej, pj = _p(np.asarray(edge_j).reshape(-1), np.int32)
+        meas, pm = _p(np.asarray(meas_ji, np.float64).reshape(-1, 13), np.float64)
+        E = len(ei)
+        if not (len(fixed) == K and len(ej) == E and len(meas) == E):
+            raise ValueError("graph_optimizer: fixed needs K rows, edge_j and meas_ji need E rows")
+        lm = np.zeros((0, 3)) if lm_pos_w is None else np.array(lm_pos_w, np.float64).reshape(-1, 3).copy()
+        L = len(lm)
+        ref, pr = _p(np.full(L, -1, np.int32) if lm_ref is None else np.asarray(lm_ref).reshape(-1), np.int32)
+        if len(ref) != L:
+            raise ValueError("graph_optimizer: lm_ref needs one entry per landmark")
+        pose = np.zeros((K, 12))
+        st = BaStats()
+        _lib.check(_lib.lib().ovs_graph_optimize_host(self._h, K, S.ctypes.data_as(C.c_void_p), pf, E, pi if E else None, pj if E else None,
+                                                      pm if E else None, int(self.fix_scale_), self.num_iter_, L,
+                                                      lm.ctypes.data_as(C.c_void_p) if L else None, pr if L else None,
+                                                      pose.ctypes.data_as(C.c_void_p), C.byref(st)))
+        return S, pose, lm, _stats(st)
+
+
 class prepared_local_ba(_optimizer_handle):
     """A local-BA problem kept resident on the device: prepare once, run many times (bench.py's
     device-resident leg), fetch the result of the last run."""
