@@ -6,6 +6,8 @@
 //   match::projection::match_frame_and_landmarks(data::frame&, const std::vector<data::landmark*>&, float)      (match/projection.h)
 //   optimize::pose_optimizer::optimize(data::frame&)                                                             (optimize/pose_optimizer.h)
 //   optimize::local_bundle_adjuster::optimize(data::keyframe*, bool* const)                                      (optimize/local_bundle_adjuster.h)
+//   solve::sim3_solver(data::keyframe*, data::keyframe*, const std::vector<data::landmark*>&, bool, unsigned),
+//     find_via_ransac(unsigned), solution_is_valid(), get_best_{rotation,translation,scale}_12()                 (solve/sim3_solver.h)
 //
 // Include it INSTEAD of openvslam_b200.hpp in a translation unit that can see the reference's headers (here: the stand-ins
 // under tests/cpp/standin, which declare the members used below with the names recalled in SURVEY.md section 2 / 8b;
@@ -257,6 +259,65 @@ inline void optimize::local_bundle_adjuster::optimize(data::keyframe* curr_keyfr
             lms[static_cast<std::size_t>(l)]->update_normal_and_depth();
         }
     }
+}
+
+// ------------------------------------------------------------------------------------------------ solve::sim3_solver
+// The reference's constructor keeps, in keyframe 1's keypoint order, the pairs whose two landmarks exist and are not to be erased
+// and whose lm_2 is observed in keyframe 2; each side contributes its landmark's world position and level_sigma_sq_ at the octave
+// of its keypoint.  The sampler seed is (keyfrm_1->id_ << 32) | keyfrm_2->id_, so a candidate always gives the same solution.
+namespace adapters {
+//! level_sigma_sq_[octave] of a keyframe, formed as orb_params::calc_level_sigma_sq defines it: the float square of the level's
+//! scale factor (the same bits; ovs_extractor_scale_factors computes it the same way).  Only scale_factors_ is read, so the
+//! adapter needs no member beyond those the other adapters use.
+inline float level_sigma_sq(const data::keyframe* keyfrm, const int octave) {
+    const float s = keyfrm->scale_factors_.at(static_cast<std::size_t>(octave));
+    return s * s;
+}
+}  // namespace adapters
+
+inline solve::sim3_solver::sim3_solver(data::keyframe* keyfrm_1, data::keyframe* keyfrm_2, const std::vector<data::landmark*>& matched_lms_in_keyfrm_2,
+                                       const bool fix_scale, const unsigned int min_num_inliers)
+    : sim3_solver(fix_scale, min_num_inliers) {
+    const auto keyfrm_1_lms = keyfrm_1->get_landmarks();
+    for (std::size_t idx1 = 0; idx1 < keyfrm_1_lms.size() && idx1 < matched_lms_in_keyfrm_2.size(); ++idx1) {
+        data::landmark* lm_1 = keyfrm_1_lms[idx1];
+        data::landmark* lm_2 = matched_lms_in_keyfrm_2[idx1];
+        if (!lm_1 || !lm_2) continue;
+        if (lm_1->will_be_erased() || lm_2->will_be_erased()) continue;
+        const int idx2 = lm_2->get_index_in_keyframe(keyfrm_2);
+        if (idx2 < 0) continue;
+        const Vec3_t p1 = lm_1->get_pos_in_world(), p2 = lm_2->get_pos_in_world();
+        for (int k = 0; k < 3; ++k) { own_pos_w_1_.push_back(p1(k)); own_pos_w_2_.push_back(p2(k)); }
+        own_sigma_sq_1_.push_back(adapters::level_sigma_sq(keyfrm_1, keyfrm_1->undist_keypts_.at(idx1).octave));
+        own_sigma_sq_2_.push_back(adapters::level_sigma_sq(keyfrm_2, keyfrm_2->undist_keypts_.at(static_cast<std::size_t>(idx2)).octave));
+    }
+    own_poses_.resize(24);
+    adapters::to_Rt(keyfrm_1->get_cam_pose(), own_poses_.data());
+    adapters::to_Rt(keyfrm_2->get_cam_pose(), own_poses_.data() + 12);
+    own_.camera_1 = adapters::to_camera(keyfrm_1->camera_);
+    own_.camera_2 = adapters::to_camera(keyfrm_2->camera_);
+    own_.cam_pose_1w = own_poses_.data(); own_.cam_pose_2w = own_poses_.data() + 12;
+    own_.num_pairs = static_cast<int>(own_sigma_sq_1_.size());
+    own_.pos_w_1 = own_pos_w_1_.data(); own_.level_sigma_sq_1 = own_sigma_sq_1_.data();
+    own_.pos_w_2 = own_pos_w_2_.data(); own_.level_sigma_sq_2 = own_sigma_sq_2_.data();
+    own_.seed = (static_cast<std::uint64_t>(keyfrm_1->id_) << 32) | static_cast<std::uint64_t>(keyfrm_2->id_);
+}
+
+inline void solve::sim3_solver::find_via_ransac(const unsigned int max_num_iter) {
+    best_ = find_via_ransac(std::vector<problem_view>{own_}, max_num_iter).front();
+}
+
+inline Mat33_t solve::sim3_solver::get_best_rotation_12() const {
+    Mat33_t R;
+    for (int r = 0; r < 3; ++r)
+        for (int c = 0; c < 3; ++c) R(r, c) = best_.sim3_12[3 * r + c];
+    return R;
+}
+
+inline Vec3_t solve::sim3_solver::get_best_translation_12() const {
+    Vec3_t t;
+    for (int k = 0; k < 3; ++k) t(k) = best_.sim3_12[9 + k];
+    return t;
 }
 
 }  // namespace openvslam

@@ -4,6 +4,7 @@
 //   openvslam::feature::orb_params / orb_extractor        (src/openvslam/feature/orb_params.h, orb_extractor.h)
 //   openvslam::match::robust / projection / area / stereo (src/openvslam/match/*.h)
 //   openvslam::optimize::pose_optimizer / local_bundle_adjuster / transform_optimizer / graph_optimizer (src/openvslam/optimize/*.h)
+//   openvslam::solve::sim3_solver                         (src/openvslam/solve/sim3_solver.h)
 // [file names as recalled in SURVEY.md 8(a); /root/reference holds no source, so no line numbers].
 //
 // The reference's methods take cv::Mat / cv::KeyPoint / Eigen / data::frame / data::keyframe.  None of
@@ -509,4 +510,96 @@ private:
 };
 
 }  // namespace optimize
+
+namespace solve {
+
+//! solve::sim3_solver (loop detection): RANSAC over Horn's closed-form Sim3 on three landmark pairs.  The reference builds one
+//! solver per loop candidate; here find_via_ransac(problems, max_num_iter) solves a whole batch of candidates in one call, and
+//! the reference's per-candidate constructor / find_via_ransac(max_num_iter) / getters are in adapters.hpp.
+class sim3_solver {
+public:
+    //! One loop candidate on array views (see include/ovs_b200.h, ovs_sim3_solve_ransac_host).
+    struct problem_view {
+        ovs_camera camera_1{}, camera_2{};
+        const double* cam_pose_1w = nullptr; const double* cam_pose_2w = nullptr;   // {R row-major (9), t (3)}
+        int num_pairs = 0;
+        const double* pos_w_1 = nullptr; const float* level_sigma_sq_1 = nullptr;
+        const double* pos_w_2 = nullptr; const float* level_sigma_sq_2 = nullptr;
+        std::uint64_t seed = 0;
+    };
+    struct solution {
+        bool valid = false;
+        double sim3_12[13] = {1, 0, 0, 0, 1, 0, 0, 0, 1, 0, 0, 0, 1};   // {R row-major (9), t (3), s}
+        unsigned int num_inliers = 0;
+        int best_iter = -1;
+        std::vector<std::uint8_t> is_inlier;
+    };
+
+    explicit sim3_solver(const bool fix_scale, const unsigned int min_num_inliers = 20, const int device = 0)
+        : fix_scale_(fix_scale), min_num_inliers_(min_num_inliers) { detail::check(ovs_optimizer_create(device, &h_)); }
+    ~sim3_solver() { ovs_optimizer_destroy(h_); }
+    sim3_solver(const sim3_solver&) = delete;
+    sim3_solver& operator=(const sim3_solver&) = delete;
+
+    //! find_via_ransac(max_num_iter) for every problem, one GPU call
+    std::vector<solution> find_via_ransac(const std::vector<problem_view>& problems, const unsigned int max_num_iter = 200) const {
+        const int B = static_cast<int>(problems.size());
+        std::vector<std::int32_t> off(static_cast<std::size_t>(B) + 1, 0);
+        for (int b = 0; b < B; ++b) off[b + 1] = off[b] + problems[b].num_pairs;
+        const std::size_t N = static_cast<std::size_t>(off[B]);
+        std::vector<ovs_camera> c1(B), c2(B);
+        std::vector<double> p1(12 * static_cast<std::size_t>(B)), p2(12 * static_cast<std::size_t>(B)), w1(3 * N), w2(3 * N);
+        std::vector<float> s1(N), s2(N);
+        std::vector<std::uint64_t> seeds(B);
+        for (int b = 0; b < B; ++b) {
+            const problem_view& p = problems[b];
+            c1[b] = p.camera_1; c2[b] = p.camera_2; seeds[b] = p.seed;
+            std::memcpy(&p1[12 * b], p.cam_pose_1w, 96); std::memcpy(&p2[12 * b], p.cam_pose_2w, 96);
+            const std::size_t o = static_cast<std::size_t>(off[b]), n = static_cast<std::size_t>(p.num_pairs);
+            if (n == 0) continue;
+            std::memcpy(&w1[3 * o], p.pos_w_1, 24 * n); std::memcpy(&w2[3 * o], p.pos_w_2, 24 * n);
+            std::memcpy(&s1[o], p.level_sigma_sq_1, 4 * n); std::memcpy(&s2[o], p.level_sigma_sq_2, 4 * n);
+        }
+        std::vector<double> S(13 * static_cast<std::size_t>(std::max(B, 1)));
+        std::vector<std::uint8_t> valid(std::max(B, 1)), flags(std::max<std::size_t>(N, 1));
+        std::vector<std::int32_t> num(std::max(B, 1)), best(std::max(B, 1));
+        detail::check(ovs_sim3_solve_ransac_host(h_, B, off.data(), c1.data(), p1.data(), c2.data(), p2.data(), w1.data(), s1.data(), w2.data(),
+                                                 s2.data(), fix_scale_ ? 1 : 0, static_cast<int>(min_num_inliers_), static_cast<int>(max_num_iter),
+                                                 seeds.data(), S.data(), valid.data(), num.data(), best.data(), flags.data()));
+        std::vector<solution> out(B);
+        for (int b = 0; b < B; ++b) {
+            out[b].valid = valid[b] != 0;
+            std::memcpy(out[b].sim3_12, &S[13 * static_cast<std::size_t>(b)], 13 * sizeof(double));
+            out[b].num_inliers = static_cast<unsigned int>(num[b]);
+            out[b].best_iter = best[b];
+            out[b].is_inlier.assign(flags.begin() + off[b], flags.begin() + off[b + 1]);
+        }
+        return out;
+    }
+
+#ifdef OVS_B200_WITH_REFERENCE_TYPES
+    //! The reference's signatures (solve/sim3_solver.h); bodies in adapters.hpp.  The sampler is seeded with
+    //! (keyfrm_1->id_ << 32) | keyfrm_2->id_.
+    sim3_solver(data::keyframe* keyfrm_1, data::keyframe* keyfrm_2, const std::vector<data::landmark*>& matched_lms_in_keyfrm_2,
+                const bool fix_scale, const unsigned int min_num_inliers = 20);
+    void find_via_ransac(const unsigned int max_num_iter);
+    bool solution_is_valid() const { return best_.valid; }
+    Mat33_t get_best_rotation_12() const;
+    Vec3_t get_best_translation_12() const;
+    float get_best_scale_12() const { return static_cast<float>(best_.sim3_12[12]); }
+#endif
+    //! the last find_via_ransac(max_num_iter) of a solver built with the reference's constructor
+    const solution& best_solution() const { return best_; }
+
+private:
+    const bool fix_scale_;
+    const unsigned int min_num_inliers_;
+    ovs_optimizer* h_ = nullptr;
+    problem_view own_{};                                   // the reference constructor's flattened candidate
+    std::vector<double> own_pos_w_1_, own_pos_w_2_, own_poses_;
+    std::vector<float> own_sigma_sq_1_, own_sigma_sq_2_;
+    solution best_{};
+};
+
+}  // namespace solve
 }  // namespace openvslam

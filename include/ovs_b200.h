@@ -382,6 +382,29 @@ int ovs_transform_optimize_host(ovs_optimizer* h, const ovs_camera* cam_1, const
                                 int num_first_iter, int num_iter, double* sim3_12, uint8_t* inlier_out, int* num_inliers,
                                 ovs_ba_stats* stats);
 
+/* solve::sim3_solver(keyfrm_1, keyfrm_2, matched_lms_in_keyfrm_2, fix_scale, min_num_inliers).find_via_ransac(max_num_iter)
+ * (solve/sim3_solver.cc, loop detection) for B independent problems (loop candidates) in one call.  Problem b owns the pairs
+ * pair_offsets[b] .. pair_offsets[b + 1] - 1 (pair_offsets[0] = 0, non-decreasing); the caller keeps the pairs the reference keeps
+ * (both landmarks valid and not to be erased, lm_2 observed in keyframe 2), in keyframe 1's keypoint order:
+ *  cam_1[b] / cam_2[b]: keyfrm_x->camera_;  pose_1w / pose_2w [B*12]: keyfrm_x->get_cam_pose() as {R row-major, t};
+ *  pos_w_1[n*3]: lm_1->get_pos_in_world();  sigma_sq_1[n]: keyfrm_1->level_sigma_sq_[octave of lm_1's keypoint];
+ *  pos_w_2 / sigma_sq_2: the same for lm_2 = matched_lms_in_keyfrm_2[idx_1] and its keypoint in keyframe 2;
+ *  fix_scale, min_num_inliers (the reference passes 20), max_num_iter (200): as in the reference;
+ *  seeds[B]: the sampler's seed per problem (a problem gives the same result alone or inside a batch).
+ * Per problem: sim3_12[b*13] = the best S_12 {R row-major (9), t (3), s} (identity when no hypothesis has an inlier);
+ * valid[b] = solution_is_valid(); num_inliers[b] = the best count; best_iter[b] = the hypothesis it came from (-1: none);
+ * inlier_out[n] = the best hypothesis's inlier flags.  With fewer than 3 or fewer than min_num_inliers pairs no hypothesis runs
+ * and the problem is invalid.  The sampler, Horn's solution, the inlier test and the conventions fixed here are described in
+ * DESIGN.md section 5.  B > 65535, invalid offsets, camera models, sigma_sq that is not positive and finite, or negative counts return
+ * OVS_ERR_INVALID_ARG; B == 0 or no pair at all returns without a launch.  Otherwise the call is two launches, one copy each
+ * way and one wait.  Like ovs_pose_optimize_host this call reuses the handle's device buffers: a local-BA problem prepared on
+ * the same handle is invalidated (ovs_local_ba_run / _fetch then fail with OVS_ERR_INVALID_ARG until it is prepared again). */
+int ovs_sim3_solve_ransac_host(ovs_optimizer* h, int B, const int32_t* pair_offsets, const ovs_camera* cam_1, const double* pose_1w,
+                               const ovs_camera* cam_2, const double* pose_2w, const double* pos_w_1, const float* sigma_sq_1,
+                               const double* pos_w_2, const float* sigma_sq_2, int fix_scale, int min_num_inliers, int max_num_iter,
+                               const uint64_t* seeds, double* sim3_12, uint8_t* valid, int32_t* num_inliers, int32_t* best_iter,
+                               uint8_t* inlier_out);
+
 /* graph_optimizer::optimize(loop_keyfrm, curr_keyfrm, non_corrected_Sim3s, pre_corrected_Sim3s, loop_connections)
  * (optimize/graph_optimizer.cc, loop closure) on plain arrays: one Sim3 vertex per keyframe, one relative Sim3 edge per keyframe
  * pair, e = log(S_ji S_i S_j^-1) with identity information and no robust kernel, g2o's Levenberg with the user lambda 1e-16.

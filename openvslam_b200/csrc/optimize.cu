@@ -2600,6 +2600,219 @@ extern "C" int ovs_transform_optimize_host(ovs_optimizer* h, const ovs_camera* c
     return OVS_OK;
 }
 
+// ----------------------------------------------------------------------- Sim3 RANSAC solver
+namespace {
+
+constexpr int kRansacWarps = 4;                      // hypotheses per CTA, one warp each
+constexpr int kRansacThreads = 32 * kRansacWarps;
+constexpr int kRansacPrepThreads = 256;
+
+struct RansacArgs {
+    int B, N, fix_scale, min_num_inliers, max_num_iter;
+    const int* off;                                  // B + 1 pair offsets
+    const CameraD* cam1; const CameraD* cam2;        // B each
+    const double* pose1; const double* pose2;        // B x 12, {R row-major, t}
+    const double* pw1; const float* sig1; const double* pw2; const float* sig2;   // per pair
+    const uint64_t* seed;                            // B
+    unsigned long long* key;                         // B, zero on entry: max over hypotheses of (count << 32) | ~k
+    unsigned* done;                                  // B, zero on entry: CTAs of the problem that have finished scoring
+    double* pc1; double* pc2; double* rp1; double* rp2; float* bd1; float* bd2;   // per pair, written by k_sim3_ransac_prep
+    double* sim3; int* num_inliers; int* best_iter; uint8_t* valid; uint8_t* inlier;  // out
+};
+
+// One thread per pair: the points in their keyframes' camera frames, their own reprojections and the two bounds
+// (ransac_bound: -1 where the own reprojection does not exist).
+__global__ void __launch_bounds__(kRansacPrepThreads) k_sim3_ransac_prep(RansacArgs A) {
+    const int g = blockIdx.x * kRansacPrepThreads + threadIdx.x;
+    if (g >= A.N) return;
+    int lo = 0, hi = A.B;                            // the largest b with off[b] <= g (empty problems precede it)
+    while (hi - lo > 1) {
+        const int mid = (lo + hi) >> 1;
+        if (A.off[mid] <= g) lo = mid; else hi = mid;
+    }
+    const int b = lo;
+    const double I[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1}, zero[3] = {0, 0, 0};
+#pragma unroll 1
+    for (int side = 0; side < 2; ++side) {
+        const double* pose = (side == 0 ? A.pose1 : A.pose2) + 12 * (size_t)b;
+        const double* pwp = (side == 0 ? A.pw1 : A.pw2) + 3 * (size_t)g;
+        const double pw[3] = {pwp[0], pwp[1], pwp[2]};
+        double pc[3], uv[2] = {0.0, 0.0};
+        ovs::mat3_vec(pose, pw, pc);
+        pc[0] += pose[9]; pc[1] += pose[10]; pc[2] += pose[11];
+        const bool ok = ovs::ransac_reproject(side == 0 ? A.cam1[b] : A.cam2[b], I, zero, pc, uv);
+        double* pco = (side == 0 ? A.pc1 : A.pc2) + 3 * (size_t)g;
+        double* rpo = (side == 0 ? A.rp1 : A.rp2) + 2 * (size_t)g;
+        pco[0] = pc[0]; pco[1] = pc[1]; pco[2] = pc[2];
+        rpo[0] = ok ? uv[0] : 0.0; rpo[1] = ok ? uv[1] : 0.0;
+        (side == 0 ? A.bd1 : A.bd2)[g] = ovs::ransac_bound((side == 0 ? A.sig1 : A.sig2)[g], ok);
+    }
+}
+
+// Hypothesis k of problem b (pairs o .. o + n - 1): its triple, S_12 and S_21.
+__device__ void ransac_hypothesis(const RansacArgs& A, int b, int o, int n, int k, double* S12, double* S21) {
+    int idx[3];
+    ovs::sim3_ransac_triple(A.seed[b], k, n, idx);
+    double p1[9], p2[9];
+    for (int j = 0; j < 3; ++j)
+        for (int c = 0; c < 3; ++c) {
+            p1[3 * j + c] = A.pc1[3 * (size_t)(o + idx[j]) + c];
+            p2[3 * j + c] = A.pc2[3 * (size_t)(o + idx[j]) + c];
+        }
+    ovs::sim3_horn(p1, p2, A.fix_scale != 0, S12, S21);
+}
+
+__device__ __forceinline__ bool ransac_pair(const RansacArgs& A, const CameraD& c1, const CameraD& c2, const double* sR12,
+                                            const double* S12, const double* sR21, const double* S21, size_t i) {
+    const double pc1[3] = {A.pc1[3 * i], A.pc1[3 * i + 1], A.pc1[3 * i + 2]};
+    const double pc2[3] = {A.pc2[3 * i], A.pc2[3 * i + 1], A.pc2[3 * i + 2]};
+    const double r1[2] = {A.rp1[2 * i], A.rp1[2 * i + 1]}, r2[2] = {A.rp2[2 * i], A.rp2[2 * i + 1]};
+    return ovs::ransac_is_inlier(c1, c2, sR12, S12 + 9, sR21, S21 + 9, pc1, pc2, r1, r2, A.bd1[i], A.bd2[i]);
+}
+
+// find_via_ransac for every problem of the batch in one launch: grid (hypothesis blocks, problems), one warp per hypothesis
+// (every lane forms the same S_12; the lanes then take the pairs with a stride of 32 and count by ballot).  The best hypothesis is
+// the integer maximum of (count << 32) | ~k over the problem (atomicMax: order-independent), so the first of the hypotheses with
+// the most inliers wins, as in the reference's sequential loop; a hypothesis with no inlier is never best.  The last CTA of a
+// problem to finish writes S_12, the count, k, valid and the best hypothesis's inlier flags.
+__global__ void __launch_bounds__(kRansacThreads) k_sim3_ransac(RansacArgs A) {
+    const int b = blockIdx.y, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int o = A.off[b], n = A.off[b + 1] - o;
+    const bool runs = n >= 3 && n >= A.min_num_inliers;
+    const CameraD c1 = A.cam1[b], c2 = A.cam2[b];
+    const int k = blockIdx.x * kRansacWarps + warp;
+    if (runs && k < A.max_num_iter) {
+        double S12[13], S21[13], sR12[9], sR21[9];
+        ransac_hypothesis(A, b, o, n, k, S12, S21);
+        ovs::sim3_scaled_rotation(S12, sR12);
+        ovs::sim3_scaled_rotation(S21, sR21);
+        unsigned cnt = 0;
+        for (int base = 0; base < n; base += 32) {
+            const int i = base + lane;
+            const bool in = i < n && ransac_pair(A, c1, c2, sR12, S12, sR21, S21, (size_t)(o + i));
+            cnt += __popc(__ballot_sync(0xffffffffu, in));
+        }
+        if (lane == 0 && cnt > 0) {
+            atomicMax(&A.key[b], ((unsigned long long)cnt << 32) | (unsigned long long)(~(unsigned)k));
+            __threadfence();
+        }
+    }
+    __shared__ int s_last;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        __threadfence();
+        s_last = atomicAdd(&A.done[b], 1u) == gridDim.x - 1;
+    }
+    __syncthreads();
+    if (!s_last) return;
+    __threadfence();
+    const unsigned long long key = atomicOr(&A.key[b], 0ull);
+    const unsigned cnt = (unsigned)(key >> 32);
+    const int best = cnt > 0 ? (int)(~(unsigned)(key & 0xffffffffull)) : -1;
+    double S12[13], S21[13];
+    if (best >= 0) {
+        double sR12[9], sR21[9];
+        ransac_hypothesis(A, b, o, n, best, S12, S21);
+        ovs::sim3_scaled_rotation(S12, sR12);
+        ovs::sim3_scaled_rotation(S21, sR21);
+        for (int i = threadIdx.x; i < n; i += kRansacThreads)
+            A.inlier[o + i] = ransac_pair(A, c1, c2, sR12, S12, sR21, S21, (size_t)(o + i)) ? 1 : 0;
+    } else {
+        for (int m = 0; m < 13; ++m) S12[m] = (m == 0 || m == 4 || m == 8 || m == 12) ? 1.0 : 0.0;
+        for (int i = threadIdx.x; i < n; i += kRansacThreads) A.inlier[o + i] = 0;
+    }
+    if (threadIdx.x < 13) A.sim3[13 * (size_t)b + threadIdx.x] = S12[threadIdx.x];
+    if (threadIdx.x == 0) {
+        A.num_inliers[b] = (int)cnt;
+        A.best_iter[b] = best;
+        A.valid[b] = (runs && (int)cnt >= A.min_num_inliers) ? 1 : 0;
+    }
+}
+
+}  // namespace
+
+extern "C" int ovs_sim3_solve_ransac_host(ovs_optimizer* h, int B, const int32_t* pair_offsets, const ovs_camera* cam_1,
+                                          const double* pose_1w, const ovs_camera* cam_2, const double* pose_2w, const double* pos_w_1,
+                                          const float* sigma_sq_1, const double* pos_w_2, const float* sigma_sq_2, int fix_scale,
+                                          int min_num_inliers, int max_num_iter, const uint64_t* seeds, double* sim3_12, uint8_t* valid,
+                                          int32_t* num_inliers, int32_t* best_iter, uint8_t* inlier_out) {
+    OVS_REQUIRE(h && B >= 0 && B <= 65535, OVS_ERR_INVALID_ARG, "bad argument (B must be in 0 .. 65535)");
+    OVS_REQUIRE(min_num_inliers >= 0 && max_num_iter >= 0, OVS_ERR_INVALID_ARG, "min_num_inliers and max_num_iter must not be negative");
+    if (B == 0) return OVS_OK;
+    OVS_REQUIRE(pair_offsets && cam_1 && pose_1w && cam_2 && pose_2w && seeds && sim3_12 && valid && num_inliers && best_iter,
+                OVS_ERR_INVALID_ARG, "null argument");
+    OVS_REQUIRE(pair_offsets[0] == 0, OVS_ERR_INVALID_ARG, "pair_offsets[0] must be 0");
+    for (int b = 0; b < B; ++b) {
+        OVS_REQUIRE(pair_offsets[b + 1] >= pair_offsets[b], OVS_ERR_INVALID_ARG, "pair_offsets must be non-decreasing (problem %d)", b);
+        OVS_REQUIRE((cam_1[b].model == ovs::kCamPerspective || cam_1[b].model == ovs::kCamEquirectangular) &&
+                    (cam_2[b].model == ovs::kCamPerspective || cam_2[b].model == ovs::kCamEquirectangular),
+                    OVS_ERR_INVALID_ARG, "unknown camera model (problem %d)", b);
+    }
+    const int n_all = pair_offsets[B];
+    OVS_REQUIRE(n_all == 0 || (pos_w_1 && sigma_sq_1 && pos_w_2 && sigma_sq_2 && inlier_out), OVS_ERR_INVALID_ARG, "null argument");
+    for (int i = 0; i < n_all; ++i)
+        OVS_REQUIRE(sigma_sq_1[i] > 0.0f && std::isfinite(sigma_sq_1[i]) && sigma_sq_2[i] > 0.0f && std::isfinite(sigma_sq_2[i]),
+                    OVS_ERR_INVALID_ARG, "sigma_sq of pair %d must be positive and finite", i);
+    if (n_all == 0) {   // every problem has fewer than 3 pairs: no hypothesis, invalid
+        for (int b = 0; b < B; ++b) {
+            for (int m = 0; m < 13; ++m) sim3_12[13 * (size_t)b + m] = (m == 0 || m == 4 || m == 8 || m == 12) ? 1.0 : 0.0;
+            valid[b] = 0; num_inliers[b] = 0; best_iter[b] = -1;
+        }
+        return OVS_OK;
+    }
+    OVS_CUDA_CHECK(cudaSetDevice(h->device));
+    // carved from the same arenas as the pose optimiser: a prepared local-BA problem on this handle is gone
+    invalidate_plan(h);
+    if (h->pending) { OVS_CUDA_CHECK(ovs::sync_stream(h->stream)); h->pending = false; }
+    const size_t N = (size_t)n_all, NB = (size_t)B;
+    const size_t in_bytes_max = 256 * 12 + (NB + 1) * 4 + NB * 2 * sizeof(CameraD) + NB * 2 * 96 + N * 2 * (24 + 4) + NB * (8 + 8 + 4);
+    const size_t out_bytes_max = 256 * 5 + NB * (13 * 8 + 4 + 4 + 1) + N;
+    const size_t hbytes = in_bytes_max + out_bytes_max;
+    const size_t dbytes = hbytes + 256 * 6 + N * 2 * (24 + 16 + 4) + 4096;
+    int rc = ensure_arenas(h, dbytes, hbytes);
+    if (rc != OVS_OK) return rc;
+    Arena H{h->h_arena, 0, h->h_cap}, D{h->d_arena, 0, h->d_cap};
+    // inputs: the same carving sequence in both arenas, so one contiguous copy moves them
+    int* hoff = H.take<int>(NB + 1); CameraD* hc1 = H.take<CameraD>(NB); CameraD* hc2 = H.take<CameraD>(NB);
+    double* hp1 = H.take<double>(12 * NB); double* hp2 = H.take<double>(12 * NB);
+    double* hw1 = H.take<double>(3 * N); float* hs1 = H.take<float>(N); double* hw2 = H.take<double>(3 * N); float* hs2 = H.take<float>(N);
+    uint64_t* hseed = H.take<uint64_t>(NB); unsigned long long* hkey = H.take<unsigned long long>(NB); unsigned* hdone = H.take<unsigned>(NB);
+    const size_t in_bytes = H.off;
+    // outputs: one contiguous copy back
+    double* hS = H.take<double>(13 * NB);
+    const size_t out_begin = (size_t)((uint8_t*)hS - h->h_arena);
+    int* hnum = H.take<int>(NB); int* hbest = H.take<int>(NB); uint8_t* hvalid = H.take<uint8_t>(NB); uint8_t* hflags = H.take<uint8_t>(N);
+    const size_t out_end = H.off;
+    RansacArgs A;
+    A.B = B; A.N = n_all; A.fix_scale = fix_scale ? 1 : 0; A.min_num_inliers = min_num_inliers; A.max_num_iter = max_num_iter;
+    A.off = D.take<int>(NB + 1); A.cam1 = D.take<CameraD>(NB); A.cam2 = D.take<CameraD>(NB);
+    A.pose1 = D.take<double>(12 * NB); A.pose2 = D.take<double>(12 * NB);
+    A.pw1 = D.take<double>(3 * N); A.sig1 = D.take<float>(N); A.pw2 = D.take<double>(3 * N); A.sig2 = D.take<float>(N);
+    A.seed = D.take<uint64_t>(NB); A.key = D.take<unsigned long long>(NB); A.done = D.take<unsigned>(NB);
+    A.sim3 = D.take<double>(13 * NB); A.num_inliers = D.take<int>(NB); A.best_iter = D.take<int>(NB); A.valid = D.take<uint8_t>(NB);
+    A.inlier = D.take<uint8_t>(N);
+    A.pc1 = D.take<double>(3 * N); A.pc2 = D.take<double>(3 * N); A.rp1 = D.take<double>(2 * N); A.rp2 = D.take<double>(2 * N);
+    A.bd1 = D.take<float>(N); A.bd2 = D.take<float>(N);
+    memcpy(hoff, pair_offsets, 4 * (NB + 1));
+    for (int b = 0; b < B; ++b) { hc1[b] = to_cam(&cam_1[b]); hc2[b] = to_cam(&cam_2[b]); }
+    memcpy(hp1, pose_1w, 96 * NB); memcpy(hp2, pose_2w, 96 * NB);
+    memcpy(hw1, pos_w_1, 24 * N); memcpy(hs1, sigma_sq_1, 4 * N); memcpy(hw2, pos_w_2, 24 * N); memcpy(hs2, sigma_sq_2, 4 * N);
+    memcpy(hseed, seeds, 8 * NB); memset(hkey, 0, 8 * NB); memset(hdone, 0, 4 * NB);
+    cudaStream_t st = h->stream;
+    OVS_CUDA_CHECK(cudaMemcpyAsync(h->d_arena, h->h_arena, in_bytes, cudaMemcpyHostToDevice, st));
+    k_sim3_ransac_prep<<<(n_all + kRansacPrepThreads - 1) / kRansacPrepThreads, kRansacPrepThreads, 0, st>>>(A);
+    OVS_LAUNCH_CHECK();
+    const int hyp_blocks = max_num_iter > 0 ? (max_num_iter + kRansacWarps - 1) / kRansacWarps : 1;
+    k_sim3_ransac<<<dim3(hyp_blocks, B), kRansacThreads, 0, st>>>(A);
+    OVS_LAUNCH_CHECK();
+    OVS_CUDA_CHECK(cudaMemcpyAsync(h->h_arena + out_begin, h->d_arena + out_begin, out_end - out_begin, cudaMemcpyDeviceToHost, st));
+    OVS_CUDA_CHECK(ovs::sync_stream(st));
+    memcpy(sim3_12, hS, 13 * 8 * NB);
+    memcpy(num_inliers, hnum, 4 * NB); memcpy(best_iter, hbest, 4 * NB); memcpy(valid, hvalid, NB);
+    memcpy(inlier_out, hflags, N);
+    return OVS_OK;
+}
+
 // ------------------------------------------------------------------- local bundle adjuster
 // The call is split in three phases so that a prepared problem can be re-run with everything
 // resident in HBM: prepare (graph bookkeeping + upload + co-observation lists), run (the two

@@ -366,4 +366,168 @@ OVS_BA_HD void graph_edge(const double* S_ji, const double* S_i, const double* S
         for (int k = 0; k < 98; ++k) J[k] = 0.0;   // J_l is singular only at |omega| = 2 pi k: not reached by log's output
 }
 
+// ------------------------------------------------------------------ Sim3 RANSAC (solve::sim3_solver, loop detection)
+// Per hypothesis k: three distinct pairs from a counter-based sampler, Horn's closed-form Sim3 S_12 on them (S_21 its inverse),
+// and the count of pairs whose points reproject through S_21 / S_12 within 9.21 sigma^2 of their own reprojections.
+// Only + - * / sqrt are used (and atan2 / asin for the equirectangular projection), so with contraction off the host and the
+// device give the same bits.
+
+// splitmix64's output function
+OVS_BA_HD uint64_t splitmix64_mix(uint64_t z) {
+    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+    return z ^ (z >> 31);
+}
+
+// The three distinct pair indices of hypothesis k of a problem with n >= 3 pairs: w_j = mix(seed + golden * (3k + j + 1)),
+// i0 = w0 % n, i1 = w1 % (n - 1) skipping i0, i2 = w2 % (n - 2) skipping min(i0, i1), then max(i0, i1).  No rejection loop.
+OVS_BA_HD void sim3_ransac_triple(uint64_t seed, int k, int n, int* idx) {
+    const uint64_t g = 0x9E3779B97F4A7C15ull, base = 3ull * (uint64_t)k;
+    const uint64_t w0 = splitmix64_mix(seed + g * (base + 1)), w1 = splitmix64_mix(seed + g * (base + 2)),
+                   w2 = splitmix64_mix(seed + g * (base + 3));
+    const int i0 = (int)(w0 % (uint64_t)n);
+    const int c = (int)(w1 % (uint64_t)(n - 1));
+    const int i1 = c + (c >= i0 ? 1 : 0);
+    const int lo = i0 < i1 ? i0 : i1, hi = i0 < i1 ? i1 : i0;
+    int i2 = (int)(w2 % (uint64_t)(n - 2));
+    if (i2 >= lo) ++i2;
+    if (i2 >= hi) ++i2;
+    idx[0] = i0; idx[1] = i1; idx[2] = i2;
+}
+
+// Cyclic Jacobi on a symmetric 4 x 4 A (row-major, overwritten: its diagonal ends as the eigenvalues); V (row-major) gets the
+// eigenvectors as columns.  Sweeps visit (0,1) (0,2) (0,3) (1,2) (1,3) (2,3); a sweep starts only while the off-diagonal sum of
+// squares exceeds 1e-30 of the matrix's (at entry), at most 16 sweeps.  Rotation: theta = (a_qq - a_pp) / (2 a_pq),
+// t = sign(theta) / (|theta| + sqrt(theta^2 + 1)), c = 1 / sqrt(t^2 + 1), s = t c; a_pq is set to zero after it.
+OVS_BA_HD void jacobi4(double* A, double* V) {
+    for (int k = 0; k < 16; ++k) V[k] = (k % 5 == 0) ? 1.0 : 0.0;
+    double frob = 0.0;
+    for (int k = 0; k < 16; ++k) frob += A[k] * A[k];
+    for (int sweep = 0; sweep < 16; ++sweep) {
+        double off = 0.0;
+        for (int p = 0; p < 3; ++p)
+            for (int q = p + 1; q < 4; ++q) off += A[4 * p + q] * A[4 * p + q];
+        if (!(off > 1e-30 * frob)) break;
+        for (int p = 0; p < 3; ++p)
+            for (int q = p + 1; q < 4; ++q) {
+                const double apq = A[4 * p + q];
+                if (apq == 0.0) continue;
+                const double theta = (A[4 * q + q] - A[4 * p + p]) / (2.0 * apq);
+                double t = 1.0 / (fabs(theta) + sqrt(theta * theta + 1.0));
+                if (theta < 0.0) t = -t;
+                const double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
+                for (int r = 0; r < 4; ++r) {      // columns p, q
+                    const double arp = A[4 * r + p], arq = A[4 * r + q];
+                    A[4 * r + p] = c * arp - s * arq;
+                    A[4 * r + q] = s * arp + c * arq;
+                }
+                for (int r = 0; r < 4; ++r) {      // rows p, q
+                    const double apr = A[4 * p + r], aqr = A[4 * q + r];
+                    A[4 * p + r] = c * apr - s * aqr;
+                    A[4 * q + r] = s * apr + c * aqr;
+                }
+                A[4 * p + q] = 0.0; A[4 * q + p] = 0.0;
+                for (int r = 0; r < 4; ++r) {
+                    const double vrp = V[4 * r + p], vrq = V[4 * r + q];
+                    V[4 * r + p] = c * vrp - s * vrq;
+                    V[4 * r + q] = s * vrp + c * vrq;
+                }
+            }
+    }
+}
+
+// compute_Sim3 by Horn's closed form on three point pairs (p1[3 * j + c]: point j in keyframe 1's camera frame, p2 likewise):
+// centroids, M = A2 A1^T, Horn's 4 x 4 N, the quaternion (w, x, y, z) = the eigenvector of N's largest eigenvalue (lowest index
+// on ties), R_12 directly from it (divided by |q|^2), s = sum A1 . (R A2) / sum |A2|^2 (1 with fix_scale), t = c1 - s R c2.
+// S_21 = S_12^-1.  Coincident or collinear points are not special-cased.
+OVS_BA_HD void sim3_horn(const double* p1, const double* p2, bool fix_scale, double* S12, double* S21) {
+    double c1[3], c2[3], A1[9], A2[9];   // A[3 * r + j]: coordinate r of centred point j
+    for (int r = 0; r < 3; ++r) {
+        c1[r] = (p1[r] + p1[3 + r] + p1[6 + r]) / 3.0;
+        c2[r] = (p2[r] + p2[3 + r] + p2[6 + r]) / 3.0;
+        for (int j = 0; j < 3; ++j) { A1[3 * r + j] = p1[3 * j + r] - c1[r]; A2[3 * r + j] = p2[3 * j + r] - c2[r]; }
+    }
+    double M[9];
+    for (int a = 0; a < 3; ++a)
+        for (int b = 0; b < 3; ++b) M[3 * a + b] = A2[3 * a] * A1[3 * b] + A2[3 * a + 1] * A1[3 * b + 1] + A2[3 * a + 2] * A1[3 * b + 2];
+    const double Sxx = M[0], Sxy = M[1], Sxz = M[2], Syx = M[3], Syy = M[4], Syz = M[5], Szx = M[6], Szy = M[7], Szz = M[8];
+    double N[16] = {Sxx + Syy + Szz, Syz - Szy, Szx - Sxz, Sxy - Syx,
+                    Syz - Szy, Sxx - Syy - Szz, Sxy + Syx, Szx + Sxz,
+                    Szx - Sxz, Sxy + Syx, -Sxx + Syy - Szz, Syz + Szy,
+                    Sxy - Syx, Szx + Sxz, Syz + Szy, -Sxx - Syy + Szz};
+    double V[16];
+    jacobi4(N, V);
+    int m = 0;
+    for (int k = 1; k < 4; ++k)
+        if (N[5 * k] > N[5 * m]) m = k;
+    const double w = V[m], x = V[4 + m], y = V[8 + m], z = V[12 + m];
+    const double nq = w * w + x * x + y * y + z * z;
+    double* R = S12;
+    R[0] = (w * w + x * x - y * y - z * z) / nq; R[1] = 2.0 * (x * y - w * z) / nq;         R[2] = 2.0 * (x * z + w * y) / nq;
+    R[3] = 2.0 * (x * y + w * z) / nq;         R[4] = (w * w - x * x + y * y - z * z) / nq; R[5] = 2.0 * (y * z - w * x) / nq;
+    R[6] = 2.0 * (x * z - w * y) / nq;         R[7] = 2.0 * (y * z + w * x) / nq;         R[8] = (w * w - x * x - y * y + z * z) / nq;
+    double s = 1.0;
+    if (!fix_scale) {
+        double num = 0.0, den = 0.0;
+        for (int j = 0; j < 3; ++j) {
+            const double a2[3] = {A2[j], A2[3 + j], A2[6 + j]};
+            double ra[3];
+            mat3_vec(R, a2, ra);
+            num += A1[j] * ra[0] + A1[3 + j] * ra[1] + A1[6 + j] * ra[2];
+            den += a2[0] * a2[0] + a2[1] * a2[1] + a2[2] * a2[2];
+        }
+        s = num / den;
+    }
+    double rc2[3];
+    mat3_vec(R, c2, rc2);
+    for (int r = 0; r < 3; ++r) S12[9 + r] = c1[r] - s * rc2[r];
+    S12[12] = s;
+    sim3_inverse(S12, S21);
+}
+
+// camera::reproject_to_image(rot_cw, trans_cw, p) as the reference writes it, p_c = rot_cw p + trans_cw; false when the
+// perspective point is not in front of the camera (the reference returns before writing the reprojection).  The in-image
+// result is not reported.
+OVS_BA_HD bool ransac_reproject(const CameraD& cam, const double* rot, const double* trans, const double* p, double* uv) {
+    double pc[3];
+    mat3_vec(rot, p, pc);
+    for (int k = 0; k < 3; ++k) pc[k] += trans[k];
+    if (cam.model == kCamEquirectangular) {
+        const double L = sqrt(pc[0] * pc[0] + pc[1] * pc[1] + pc[2] * pc[2]);
+        const double bx = pc[0] / L, by = pc[1] / L, bz = pc[2] / L;
+        const double latitude = -asin(by), longitude = atan2(bx, bz);
+        uv[0] = cam.cols * (0.5 + longitude / (2.0 * kPi));
+        uv[1] = cam.rows * (0.5 - latitude / kPi);
+        return true;
+    }
+    if (pc[2] <= 0.0) return false;
+    const double z_inv = 1.0 / pc[2];
+    uv[0] = cam.fx * pc[0] * z_inv + cam.cx;
+    uv[1] = cam.fy * pc[1] * z_inv + cam.cy;
+    return true;
+}
+
+// rot_cw = s R, formed element-wise before the projection (reproject_to_other_image)
+OVS_BA_HD void sim3_scaled_rotation(const double* S, double* sR) {
+    for (int k = 0; k < 9; ++k) sR[k] = S[12] * S[k];
+}
+
+// The bound of one side of a pair: 9.21034f * sigma^2 in float, or -1 (never met) when the pair's own reprojection on that side
+// does not exist (a perspective point behind its camera).
+OVS_BA_HD float ransac_bound(float sigma_sq, bool own_ok) { return own_ok ? 9.21034f * sigma_sq : -1.0f; }
+
+// count_inliers for one pair: |pi_2(S_21 pc1) - reproj_2|^2 < bound_2 and |pi_1(S_12 pc2) - reproj_1|^2 < bound_1, both strict;
+// a projection behind its camera is not an inlier.  sR / t: the scaled rotations and translations of S_12 and S_21.
+OVS_BA_HD bool ransac_is_inlier(const CameraD& cam1, const CameraD& cam2, const double* sR12, const double* t12, const double* sR21,
+                                const double* t21, const double* pc1, const double* pc2, const double* reproj1, const double* reproj2,
+                                float bound1, float bound2) {
+    double u2[2], u1[2];
+    if (!ransac_reproject(cam2, sR21, t21, pc1, u2)) return false;
+    if (!ransac_reproject(cam1, sR12, t12, pc2, u1)) return false;
+    const double d2x = u2[0] - reproj2[0], d2y = u2[1] - reproj2[1];
+    const double d1x = u1[0] - reproj1[0], d1y = u1[1] - reproj1[1];
+    const double e2 = d2x * d2x + d2y * d2y, e1 = d1x * d1x + d1y * d1y;
+    return e2 < (double)bound2 && e1 < (double)bound1;
+}
+
 }  // namespace ovs

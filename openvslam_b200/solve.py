@@ -1,0 +1,64 @@
+"""Host-side mirror of openvslam::solve::sim3_solver (src/openvslam/solve/sim3_solver.h; names as in SURVEY.md 8a) over the C ABI
+of libovs_b200.so: loop detection's Sim3 RANSAC, solved on the GPU for a whole batch of loop candidates in one call.  The
+reference constructs one solver per candidate from two keyframes and their matched landmarks; here each candidate is a
+`problem` of flat arrays (see include/ovs_b200.h, ovs_sim3_solve_ransac_host, for the field-by-field mapping)."""
+import ctypes as C
+
+import numpy as np
+
+from . import _lib
+from .optimize import Camera, _optimizer_handle, _p
+
+
+class sim3_solver(_optimizer_handle):
+    """openvslam::solve::sim3_solver(keyfrm_1, keyfrm_2, matched_lms_in_keyfrm_2, fix_scale, min_num_inliers = 20), batched.
+
+    find_via_ransac(problems, max_num_iter=200, seeds=None): problems is a list of dicts with
+      cam_1, cam_2            optimize.Camera of keyframe 1 / keyframe 2,
+      pose_1w, pose_2w        cam_pose_cw of each keyframe as {R row-major (9), t (3)},
+      pos_w_1, pos_w_2        (n, 3) world positions of the matched landmarks (lm_1 of keyframe 1, lm_2 matched to it),
+      sigma_sq_1, sigma_sq_2  (n,) level_sigma_sq_ of each landmark's keypoint octave in its keyframe;
+    seeds: one sampler seed per problem (default: the problem's index).  A problem gives the same result alone or in a batch.
+    Returns one dict per problem: valid (solution_is_valid()), sim3_12 {R (9), t (3), s}, num_inliers, best_iter (-1: no
+    hypothesis had an inlier), inliers (n,) bool."""
+
+    def __init__(self, fix_scale, min_num_inliers=20, device=0):
+        super().__init__(device)
+        self.fix_scale_ = bool(fix_scale)
+        self.min_num_inliers_ = int(min_num_inliers)
+
+    def find_via_ransac(self, problems, max_num_iter=200, seeds=None):
+        B = len(problems)
+        counts = []
+        for p in problems:
+            n = len(np.asarray(p["sigma_sq_1"]).reshape(-1))
+            if not (np.asarray(p["pos_w_1"]).size == np.asarray(p["pos_w_2"]).size == 3 * n and np.asarray(p["sigma_sq_2"]).size == n):
+                raise ValueError("sim3_solver: pos_w_1 / pos_w_2 need (n, 3) and sigma_sq_1 / sigma_sq_2 n entries")
+            counts.append(n)
+        off = np.zeros(B + 1, np.int32)
+        off[1:] = np.cumsum(counts)
+        N = int(off[-1])
+        seeds = np.arange(B, dtype=np.uint64) if seeds is None else np.asarray(seeds, np.uint64).reshape(-1)
+        if len(seeds) != B:
+            raise ValueError("sim3_solver: one seed per problem")
+        cams_1 = (Camera * max(B, 1))(*[p["cam_1"] for p in problems])
+        cams_2 = (Camera * max(B, 1))(*[p["cam_2"] for p in problems])
+
+        def cat(key, width, dt):
+            if N == 0:
+                return np.zeros((1, width) if width > 1 else 1, dt)
+            return np.concatenate([np.asarray(p[key], dt).reshape(-1, width) if width > 1 else np.asarray(p[key], dt).reshape(-1)
+                                   for p in problems])
+        pose1, pp1 = _p(np.concatenate([np.asarray(p["pose_1w"], np.float64).reshape(12) for p in problems]) if B else np.zeros(12), np.float64)
+        pose2, pp2 = _p(np.concatenate([np.asarray(p["pose_2w"], np.float64).reshape(12) for p in problems]) if B else np.zeros(12), np.float64)
+        w1, pw1 = _p(cat("pos_w_1", 3, np.float64), np.float64); s1, ps1 = _p(cat("sigma_sq_1", 1, np.float32), np.float32)
+        w2, pw2 = _p(cat("pos_w_2", 3, np.float64), np.float64); s2, ps2 = _p(cat("sigma_sq_2", 1, np.float32), np.float32)
+        off_, po = _p(off, np.int32); seeds_, pseed = _p(seeds if B else np.zeros(1, np.uint64), np.uint64)
+        S = np.zeros((max(B, 1), 13)); valid = np.zeros(max(B, 1), np.uint8)
+        ninl = np.zeros(max(B, 1), np.int32); best = np.zeros(max(B, 1), np.int32); flags = np.zeros(max(N, 1), np.uint8)
+        vp = lambda a: a.ctypes.data_as(C.c_void_p)
+        _lib.check(_lib.lib().ovs_sim3_solve_ransac_host(self._h, B, po, cams_1, pp1, cams_2, pp2, pw1, ps1, pw2, ps2, int(self.fix_scale_),
+                                                         self.min_num_inliers_, int(max_num_iter), pseed, vp(S), vp(valid), vp(ninl), vp(best),
+                                                         vp(flags)))
+        return [dict(valid=bool(valid[b]), sim3_12=S[b].copy(), num_inliers=int(ninl[b]), best_iter=int(best[b]),
+                     inliers=flags[off[b]:off[b + 1]].astype(bool)) for b in range(B)]
