@@ -8,6 +8,9 @@
 //   optimize::local_bundle_adjuster::optimize(data::keyframe*, bool* const)                                      (optimize/local_bundle_adjuster.h)
 //   solve::sim3_solver(data::keyframe*, data::keyframe*, const std::vector<data::landmark*>&, bool, unsigned),
 //     find_via_ransac(unsigned), solution_is_valid(), get_best_{rotation,translation,scale}_12()                 (solve/sim3_solver.h)
+//   solve::pnp_solver(const eigen_alloc_vector<bearing_t>&, const std::vector<cv::KeyPoint>&, const eigen_alloc_vector<Vec3_t>&,
+//     const std::vector<float>&, unsigned), find_via_ransac(unsigned, bool), solution_is_valid(), get_best_{rotation,translation,
+//     cam_pose}(), get_inlier_flags()                                                                            (solve/pnp_solver.h)
 //
 // Include it INSTEAD of openvslam_b200.hpp in a translation unit that can see the reference's headers (here: the stand-ins
 // under tests/cpp/standin, which declare the members used below with the names recalled in SURVEY.md section 2 / 8b;
@@ -319,5 +322,60 @@ inline Vec3_t solve::sim3_solver::get_best_translation_12() const {
     for (int k = 0; k < 3; ++k) t(k) = best_.sim3_12[9 + k];
     return t;
 }
+
+// ------------------------------------------------------------------------------------------------ solve::pnp_solver
+// The reference's constructor takes, per correspondence, the frame keypoint's bearing, the keypoint (for its octave) and the
+// landmark's world position; max_cos_error is formed on the device from scale_factors[octave].  The sampler seed is a splitmix64
+// hash of the input bits, so the same input always gives the same solution.
+template <class BearingVector, class PointVector>
+inline solve::pnp_solver::pnp_solver(const BearingVector& valid_bearings, const std::vector<cv::KeyPoint>& valid_keypts,
+                                     const PointVector& valid_points, const std::vector<float>& scale_factors,
+                                     const unsigned int min_num_inliers)
+    : pnp_solver(min_num_inliers) {
+    const std::size_t n = valid_bearings.size();
+    std::uint64_t seed = 0x9E3779B97F4A7C15ull ^ static_cast<std::uint64_t>(n);
+    auto hash = [&seed](const void* p, const std::size_t bytes) {
+        const unsigned char* c = static_cast<const unsigned char*>(p);
+        for (std::size_t k = 0; k < bytes; k += 8) {
+            std::uint64_t w = 0;
+            std::memcpy(&w, c + k, std::min<std::size_t>(8, bytes - k));
+            std::uint64_t z = seed + w + 0x9E3779B97F4A7C15ull;   // splitmix64's output function over the running state
+            z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+            z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+            seed = z ^ (z >> 31);
+        }
+    };
+    for (std::size_t i = 0; i < n; ++i) {
+        const auto& b = valid_bearings[i];
+        const auto& p = valid_points.at(i);
+        for (int k = 0; k < 3; ++k) { own_bearings_.push_back(b(k)); own_pos_w_.push_back(p(k)); }
+        own_scale_factor_.push_back(scale_factors.at(static_cast<std::size_t>(valid_keypts.at(i).octave)));
+    }
+    hash(own_bearings_.data(), 8 * own_bearings_.size());
+    hash(own_pos_w_.data(), 8 * own_pos_w_.size());
+    hash(own_scale_factor_.data(), 4 * own_scale_factor_.size());
+    own_.num_corrs = static_cast<int>(n);
+    own_.bearings = own_bearings_.data(); own_.pos_w = own_pos_w_.data(); own_.scale_factor = own_scale_factor_.data();
+    own_.seed = seed;
+}
+
+inline void solve::pnp_solver::find_via_ransac(const unsigned int max_num_iter, const bool recompute) {
+    best_ = find_via_ransac(std::vector<problem_view>{own_}, max_num_iter, recompute).front();
+}
+
+inline Mat33_t solve::pnp_solver::get_best_rotation() const {
+    Mat33_t R;
+    for (int r = 0; r < 3; ++r)
+        for (int c = 0; c < 3; ++c) R(r, c) = best_.pose_cw[3 * r + c];
+    return R;
+}
+
+inline Vec3_t solve::pnp_solver::get_best_translation() const {
+    Vec3_t t;
+    for (int k = 0; k < 3; ++k) t(k) = best_.pose_cw[9 + k];
+    return t;
+}
+
+inline Mat44_t solve::pnp_solver::get_best_cam_pose() const { return adapters::from_Rt(best_.pose_cw); }
 
 }  // namespace openvslam

@@ -5,6 +5,7 @@
 //   openvslam::match::robust / projection / area / stereo (src/openvslam/match/*.h)
 //   openvslam::optimize::pose_optimizer / local_bundle_adjuster / transform_optimizer / graph_optimizer (src/openvslam/optimize/*.h)
 //   openvslam::solve::sim3_solver                         (src/openvslam/solve/sim3_solver.h)
+//   openvslam::solve::pnp_solver                          (src/openvslam/solve/pnp_solver.h)
 // [file names as recalled in SURVEY.md 8(a); /root/reference holds no source, so no line numbers].
 //
 // The reference's methods take cv::Mat / cv::KeyPoint / Eigen / data::frame / data::keyframe.  None of
@@ -598,6 +599,97 @@ private:
     problem_view own_{};                                   // the reference constructor's flattened candidate
     std::vector<double> own_pos_w_1_, own_pos_w_2_, own_poses_;
     std::vector<float> own_sigma_sq_1_, own_sigma_sq_2_;
+    solution best_{};
+};
+
+//! solve::pnp_solver (relocalisation): RANSAC over EPnP on minimal sets of 6 bearing-landmark correspondences, with an optional
+//! EPnP recompute on all inliers.  The reference builds one solver per relocalisation candidate; here
+//! find_via_ransac(problems, max_num_iter, recompute) solves a whole batch of candidates in one call, and the reference's
+//! per-candidate constructor / find_via_ransac(max_num_iter, recompute) / getters are in adapters.hpp.
+class pnp_solver {
+public:
+    //! One relocalisation candidate on array views (see include/ovs_b200.h, ovs_pnp_solve_ransac_host).
+    struct problem_view {
+        int num_corrs = 0;
+        const double* bearings = nullptr;                  // 3 per correspondence, unit
+        const double* pos_w = nullptr;                     // 3 per correspondence
+        const float* scale_factor = nullptr;               // scale_factors_[octave] per correspondence
+        std::uint64_t seed = 0;
+    };
+    struct solution {
+        bool valid = false;
+        double pose_cw[12] = {1, 0, 0, 0, 1, 0, 0, 0, 1, 0, 0, 0};   // {R row-major (9), t (3)}
+        unsigned int num_inliers = 0;
+        int best_iter = -1;
+        std::vector<std::uint8_t> is_inlier;
+    };
+
+    explicit pnp_solver(const unsigned int min_num_inliers = 10, const int device = 0) : min_num_inliers_(min_num_inliers) {
+        detail::check(ovs_optimizer_create(device, &h_));
+    }
+    ~pnp_solver() { ovs_optimizer_destroy(h_); }
+    pnp_solver(const pnp_solver&) = delete;
+    pnp_solver& operator=(const pnp_solver&) = delete;
+
+    //! find_via_ransac(max_num_iter, recompute) for every problem, one GPU call
+    std::vector<solution> find_via_ransac(const std::vector<problem_view>& problems, const unsigned int max_num_iter = 30,
+                                          const bool recompute = true) const {
+        const int B = static_cast<int>(problems.size());
+        std::vector<std::int32_t> off(static_cast<std::size_t>(B) + 1, 0);
+        for (int b = 0; b < B; ++b) off[b + 1] = off[b] + problems[b].num_corrs;
+        const std::size_t N = static_cast<std::size_t>(off[B]);
+        std::vector<double> bear(3 * N), pw(3 * N);
+        std::vector<float> sf(N);
+        std::vector<std::uint64_t> seeds(B);
+        for (int b = 0; b < B; ++b) {
+            const problem_view& p = problems[b];
+            seeds[b] = p.seed;
+            const std::size_t o = static_cast<std::size_t>(off[b]), n = static_cast<std::size_t>(p.num_corrs);
+            if (n == 0) continue;
+            std::memcpy(&bear[3 * o], p.bearings, 24 * n); std::memcpy(&pw[3 * o], p.pos_w, 24 * n);
+            std::memcpy(&sf[o], p.scale_factor, 4 * n);
+        }
+        std::vector<double> pose(12 * static_cast<std::size_t>(std::max(B, 1)));
+        std::vector<std::uint8_t> valid(std::max(B, 1)), flags(std::max<std::size_t>(N, 1));
+        std::vector<std::int32_t> num(std::max(B, 1)), best(std::max(B, 1));
+        detail::check(ovs_pnp_solve_ransac_host(h_, B, off.data(), bear.data(), pw.data(), sf.data(), static_cast<int>(min_num_inliers_),
+                                                static_cast<int>(max_num_iter), recompute ? 1 : 0, seeds.data(), pose.data(), valid.data(),
+                                                num.data(), best.data(), flags.data()));
+        std::vector<solution> out(B);
+        for (int b = 0; b < B; ++b) {
+            out[b].valid = valid[b] != 0;
+            std::memcpy(out[b].pose_cw, &pose[12 * static_cast<std::size_t>(b)], 12 * sizeof(double));
+            out[b].num_inliers = static_cast<unsigned int>(num[b]);
+            out[b].best_iter = best[b];
+            out[b].is_inlier.assign(flags.begin() + off[b], flags.begin() + off[b + 1]);
+        }
+        return out;
+    }
+
+#ifdef OVS_B200_WITH_REFERENCE_TYPES
+    //! The reference's signatures (solve/pnp_solver.h); bodies in adapters.hpp.  The constructor receives no frame or keyframe
+    //! id, so the sampler is seeded with a splitmix64 hash of the input bits (the batched call takes explicit seeds).  The bearing
+    //! and point containers are template parameters: the reference passes eigen_alloc_vector<bearing_t> / eigen_alloc_vector<Vec3_t>
+    //! (std::vector with Eigen's aligned allocator); any random-access container of 3-vectors indexed as v(k) is accepted.
+    template <class BearingVector, class PointVector>
+    pnp_solver(const BearingVector& valid_bearings, const std::vector<cv::KeyPoint>& valid_keypts, const PointVector& valid_points,
+               const std::vector<float>& scale_factors, const unsigned int min_num_inliers = 10);
+    void find_via_ransac(const unsigned int max_num_iter, const bool recompute = true);
+    bool solution_is_valid() const { return best_.valid; }
+    Mat33_t get_best_rotation() const;
+    Vec3_t get_best_translation() const;
+    Mat44_t get_best_cam_pose() const;
+    std::vector<bool> get_inlier_flags() const { return std::vector<bool>(best_.is_inlier.begin(), best_.is_inlier.end()); }
+#endif
+    //! the last find_via_ransac(max_num_iter, recompute) of a solver built with the reference's constructor
+    const solution& best_solution() const { return best_; }
+
+private:
+    const unsigned int min_num_inliers_;
+    ovs_optimizer* h_ = nullptr;
+    problem_view own_{};                                   // the reference constructor's flattened candidate
+    std::vector<double> own_bearings_, own_pos_w_;
+    std::vector<float> own_scale_factor_;
     solution best_{};
 };
 

@@ -405,6 +405,30 @@ int ovs_sim3_solve_ransac_host(ovs_optimizer* h, int B, const int32_t* pair_offs
                                const uint64_t* seeds, double* sim3_12, uint8_t* valid, int32_t* num_inliers, int32_t* best_iter,
                                uint8_t* inlier_out);
 
+/* solve::pnp_solver(valid_bearings, valid_keypts, valid_points, scale_factors, min_num_inliers).find_via_ransac(max_num_iter,
+ * recompute) (solve/pnp_solver.cc, relocalisation) for B independent problems (relocalisation candidates) in one call.  Problem b
+ * owns the correspondences corr_offsets[b] .. corr_offsets[b + 1] - 1 (corr_offsets[0] = 0, non-decreasing), in the order the
+ * reference's constructor receives them:
+ *  bearings[n*3]: frm.bearings_[idx] (unit; any camera model: ovs_undistort_keypoints_* produces them);
+ *  pos_w[n*3]: the matched landmark's get_pos_in_world();
+ *  scale_factor[n]: scale_factors_[octave of the keypoint], in (0, 90]: the bound is cos(pi / 180 * scale_factor), in double;
+ *  min_num_inliers (the reference's default 10), max_num_iter (the relocaliser's 30), recompute (default true): as in the
+ *  reference; seeds[B]: the sampler's seed per problem (a problem gives the same result alone or inside a batch).
+ * Per problem: pose_cw[b*12] = get_best_cam_pose() as {R row-major (9), t (3)} (identity when no hypothesis has an inlier);
+ * valid[b] = solution_is_valid(); num_inliers[b] = the number of inlier flags set; best_iter[b] = the best hypothesis (-1: none);
+ * inlier_out[n] = get_inlier_flags().  With fewer than 6 (the minimal set) or fewer than min_num_inliers correspondences no
+ * hypothesis runs and the problem is invalid.  With recompute, a valid problem whose best hypothesis has at least 6 inliers is
+ * solved again by EPnP on all of them and its flags are re-checked at that pose.  The sampler, EPnP, the fixed order of the
+ * recompute's sums and the conventions fixed here are described in DESIGN.md section 5.  B outside 0 .. 65535, invalid offsets,
+ * a non-finite position, a bearing that is not finite or not unit (|b.b - 1| > 1e-6), a scale factor outside (0, 90] or negative
+ * counts return OVS_ERR_INVALID_ARG; B == 0 or no correspondence at all returns without a launch.  Otherwise the call is three
+ * launches (two with max_num_iter == 0), one copy each way and one wait.  Like ovs_pose_optimize_host this call reuses the
+ * handle's device buffers: a local-BA problem prepared on the same handle is invalidated (ovs_local_ba_run / _fetch then fail
+ * with OVS_ERR_INVALID_ARG until it is prepared again). */
+int ovs_pnp_solve_ransac_host(ovs_optimizer* h, int B, const int32_t* corr_offsets, const double* bearings, const double* pos_w,
+                              const float* scale_factor, int min_num_inliers, int max_num_iter, int recompute, const uint64_t* seeds,
+                              double* pose_cw, uint8_t* valid, int32_t* num_inliers, int32_t* best_iter, uint8_t* inlier_out);
+
 /* graph_optimizer::optimize(loop_keyfrm, curr_keyfrm, non_corrected_Sim3s, pre_corrected_Sim3s, loop_connections)
  * (optimize/graph_optimizer.cc, loop closure) on plain arrays: one Sim3 vertex per keyframe, one relative Sim3 edge per keyframe
  * pair, e = log(S_ji S_i S_j^-1) with identity information and no robust kernel, g2o's Levenberg with the user lambda 1e-16.

@@ -47,6 +47,7 @@
 
 #include "ba_math.cuh"
 #include "ovs_common.h"
+#include "pnp_math.cuh"
 #include "sim3_math.cuh"
 
 namespace {
@@ -2808,6 +2809,245 @@ extern "C" int ovs_sim3_solve_ransac_host(ovs_optimizer* h, int B, const int32_t
     OVS_CUDA_CHECK(cudaMemcpyAsync(h->h_arena + out_begin, h->d_arena + out_begin, out_end - out_begin, cudaMemcpyDeviceToHost, st));
     OVS_CUDA_CHECK(ovs::sync_stream(st));
     memcpy(sim3_12, hS, 13 * 8 * NB);
+    memcpy(num_inliers, hnum, 4 * NB); memcpy(best_iter, hbest, 4 * NB); memcpy(valid, hvalid, NB);
+    memcpy(inlier_out, hflags, N);
+    return OVS_OK;
+}
+
+// ----------------------------------------------------------------------- PnP RANSAC solver
+namespace {
+
+constexpr int kPnpHypThreads = 64;                   // k_pnp_hypotheses: one thread per hypothesis (and per correspondence)
+constexpr int kPnpWarps = 4;                         // k_pnp_ransac: hypotheses per CTA, one warp each
+constexpr int kPnpThreads = 32 * kPnpWarps;
+constexpr int kPnpRefineThreads = ovs::kPnpSumSlots; // k_pnp_refine: one CTA per problem, one thread per partial sum
+constexpr int kPnpChunk = 8;                         // components reduced per pass of the CTA-wide sum
+
+struct PnpArgs {
+    int B, N, H, min_num_inliers, recompute;
+    const int* off;                                  // B + 1 correspondence offsets
+    const double* bear; const double* pw; const float* sf;   // per correspondence
+    const uint64_t* seed;                            // B
+    unsigned long long* key;                         // B, zero on entry: max over hypotheses of (count << 32) | ~k
+    double* bound;                                   // per correspondence: max_cos_error, written by k_pnp_hypotheses
+    double* hyp;                                     // B x H x 12: every hypothesis's pose
+    int* cidx;                                       // per correspondence: the best hypothesis's inliers, compacted per problem
+    double* pose; int* num_inliers; int* best_iter; uint8_t* valid; uint8_t* inlier;   // out
+};
+
+__device__ __forceinline__ bool pnp_runs(const PnpArgs& A, int n) { return n >= ovs::kPnpMinSet && n >= A.min_num_inliers; }
+
+__device__ __forceinline__ bool pnp_corr(const PnpArgs& A, const double* pose, size_t i) {
+    const double pw[3] = {A.pw[3 * i], A.pw[3 * i + 1], A.pw[3 * i + 2]};
+    const double b[3] = {A.bear[3 * i], A.bear[3 * i + 1], A.bear[3 * i + 2]};
+    return ovs::pnp_is_inlier(pose, pw, b, A.bound[i]);
+}
+
+// One thread per (problem, hypothesis): the minimal set of the counter-based sampler and its EPnP pose.  The first N threads
+// also form the correspondences' bounds.
+__global__ void __launch_bounds__(kPnpHypThreads) k_pnp_hypotheses(PnpArgs A) {
+    const size_t g = (size_t)blockIdx.x * kPnpHypThreads + threadIdx.x;
+    if (g < (size_t)A.N) A.bound[g] = ovs::pnp_max_cos(A.sf[g]);
+    if (A.H == 0 || g >= (size_t)A.B * (size_t)A.H) return;
+    const int b = (int)(g / (size_t)A.H), k = (int)(g % (size_t)A.H);
+    const int o = A.off[b], n = A.off[b + 1] - o;
+    if (!pnp_runs(A, n)) return;
+    int idx[ovs::kPnpMinSet];
+    ovs::ransac_sample<ovs::kPnpMinSet>(A.seed[b], k, n, idx);
+    const ovs::PnpPoints P{A.pw + 3 * (size_t)o, A.bear + 3 * (size_t)o, idx, ovs::kPnpMinSet};
+    ovs::epnp_pose(P, ovs::PnpSeqSum{ovs::kPnpMinSet}, A.hyp + 12 * g);
+}
+
+// check_inliers of every hypothesis: grid (hypothesis blocks, problems), one warp per hypothesis, the lanes take the
+// correspondences with a stride of 32 and count by ballot.  The best hypothesis is the integer maximum of (count << 32) | ~k
+// (atomicMax: order-independent), so the first of the hypotheses with the most inliers wins, as in the sequential loop; a
+// hypothesis with no inlier is never best.
+__global__ void __launch_bounds__(kPnpThreads) k_pnp_ransac(PnpArgs A) {
+    const int b = blockIdx.y, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int o = A.off[b], n = A.off[b + 1] - o;
+    const int k = blockIdx.x * kPnpWarps + warp;
+    if (!pnp_runs(A, n) || k >= A.H) return;
+    const double* hp = A.hyp + 12 * ((size_t)b * A.H + k);
+    double pose[12];
+    for (int m = 0; m < 12; ++m) pose[m] = hp[m];
+    unsigned cnt = 0;
+    for (int base = 0; base < n; base += 32) {
+        const int i = base + lane;
+        const bool in = i < n && pnp_corr(A, pose, (size_t)(o + i));
+        cnt += __popc(__ballot_sync(0xffffffffu, in));
+    }
+    if (lane == 0 && cnt > 0) atomicMax(&A.key[b], ((unsigned long long)cnt << 32) | (unsigned long long)(~(unsigned)k));
+}
+
+// pnp_sum across the CTA: thread t forms partial s_t over the points t, t + 256, ..; then, kPnpChunk components at a time,
+// thread c adds the 256 partials of component c in order.  Same bits as PnpSeqSum.
+struct PnpBlockSum {
+    int n;
+    double* red;                                     // shared, kPnpChunk x 256
+    double* res;                                     // shared, 78
+    template <int K, class F> __device__ void run(F f, double* out) const {
+        const int t = threadIdx.x;
+        double s[K], v[K];
+        for (int c = 0; c < K; ++c) s[c] = 0.0;
+        for (int i = t; i < n; i += kPnpRefineThreads) {
+            f(i, v);
+            for (int c = 0; c < K; ++c) s[c] += v[c];
+        }
+#pragma unroll
+        for (int c0 = 0; c0 < K; c0 += kPnpChunk) {
+#pragma unroll
+            for (int c = c0; c < c0 + kPnpChunk && c < K; ++c) red[(c - c0) * kPnpRefineThreads + t] = s[c];
+            __syncthreads();
+            if (t < kPnpChunk && c0 + t < K) {
+                double acc = 0.0;
+                for (int u = 0; u < kPnpRefineThreads; ++u) acc += red[t * kPnpRefineThreads + u];
+                res[c0 + t] = acc;
+            }
+            __syncthreads();
+        }
+        for (int c = 0; c < K; ++c) out[c] = res[c];
+        __syncthreads();
+    }
+};
+
+// One CTA per problem: the best hypothesis (or none), its inlier flags, `valid`, and with recompute (valid and at least
+// kPnpMinSet inliers) EPnP on the compacted inliers with the CTA-wide sums and the flags re-checked at that pose.
+__global__ void __launch_bounds__(kPnpRefineThreads) k_pnp_refine(PnpArgs A) {
+    __shared__ double s_red[kPnpChunk * kPnpRefineThreads];
+    __shared__ double s_res[78];
+    __shared__ int s_warp[kPnpRefineThreads / 32];
+    const int b = blockIdx.x, t = threadIdx.x, lane = t & 31, warp = t >> 5;
+    const int o = A.off[b], n = A.off[b + 1] - o;
+    const bool runs = pnp_runs(A, n);
+    const unsigned long long key = A.key[b];
+    const unsigned cnt = (unsigned)(key >> 32);
+    const int best = cnt > 0 ? (int)(~(unsigned)(key & 0xffffffffull)) : -1;
+    double pose[12];
+    if (best >= 0) {
+        const double* hp = A.hyp + 12 * ((size_t)b * A.H + best);
+        for (int m = 0; m < 12; ++m) pose[m] = hp[m];
+    } else {
+        ovs::pnp_identity(pose);
+    }
+    for (int i = t; i < n; i += kPnpRefineThreads) A.inlier[o + i] = (best >= 0 && pnp_corr(A, pose, (size_t)(o + i))) ? 1 : 0;
+    const bool valid = runs && (int)cnt >= A.min_num_inliers;
+    int num = (int)cnt;
+    if (valid && A.recompute && best >= 0 && (int)cnt >= ovs::kPnpMinSet) {
+        int running = 0;
+        for (int base = 0; base < n; base += kPnpRefineThreads) {   // compaction in index order
+            const int i = base + t;
+            const bool f = i < n && pnp_corr(A, pose, (size_t)(o + i));
+            const unsigned bal = __ballot_sync(0xffffffffu, f);
+            if (lane == 0) s_warp[warp] = __popc(bal);
+            __syncthreads();
+            int before = running;
+            for (int w = 0; w < warp; ++w) before += s_warp[w];
+            if (f) A.cidx[o + before + __popc(bal & ((1u << lane) - 1u))] = i;
+            for (int w = 0; w < kPnpRefineThreads / 32; ++w) running += s_warp[w];
+            __syncthreads();
+        }
+        __syncthreads();
+        const ovs::PnpPoints P{A.pw + 3 * (size_t)o, A.bear + 3 * (size_t)o, A.cidx + o, (int)cnt};
+        double np[12];
+        ovs::epnp_pose(P, PnpBlockSum{(int)cnt, s_red, s_res}, np);
+        for (int m = 0; m < 12; ++m) pose[m] = np[m];
+        int c2 = 0;
+        for (int base = 0; base < n; base += kPnpRefineThreads) {
+            const int i = base + t;
+            const bool f = i < n && pnp_corr(A, pose, (size_t)(o + i));
+            if (i < n) A.inlier[o + i] = f ? 1 : 0;
+            c2 += __syncthreads_count(f);
+        }
+        num = c2;
+    }
+    if (t < 12) A.pose[12 * (size_t)b + t] = pose[t];
+    if (t == 0) {
+        A.num_inliers[b] = num;
+        A.best_iter[b] = best;
+        A.valid[b] = valid ? 1 : 0;
+    }
+}
+
+}  // namespace
+
+extern "C" int ovs_pnp_solve_ransac_host(ovs_optimizer* h, int B, const int32_t* corr_offsets, const double* bearings,
+                                         const double* pos_w, const float* scale_factor, int min_num_inliers, int max_num_iter,
+                                         int recompute, const uint64_t* seeds, double* pose_cw, uint8_t* valid, int32_t* num_inliers,
+                                         int32_t* best_iter, uint8_t* inlier_out) {
+    OVS_REQUIRE(h && B >= 0 && B <= 65535, OVS_ERR_INVALID_ARG, "bad argument (B must be in 0 .. 65535)");
+    OVS_REQUIRE(min_num_inliers >= 0 && max_num_iter >= 0, OVS_ERR_INVALID_ARG, "min_num_inliers and max_num_iter must not be negative");
+    if (B == 0) return OVS_OK;
+    OVS_REQUIRE(corr_offsets && seeds && pose_cw && valid && num_inliers && best_iter, OVS_ERR_INVALID_ARG, "null argument");
+    OVS_REQUIRE(corr_offsets[0] == 0, OVS_ERR_INVALID_ARG, "corr_offsets[0] must be 0");
+    for (int b = 0; b < B; ++b)
+        OVS_REQUIRE(corr_offsets[b + 1] >= corr_offsets[b], OVS_ERR_INVALID_ARG, "corr_offsets must be non-decreasing (problem %d)", b);
+    const int n_all = corr_offsets[B];
+    OVS_REQUIRE(n_all == 0 || (bearings && pos_w && scale_factor && inlier_out), OVS_ERR_INVALID_ARG, "null argument");
+    for (int i = 0; i < n_all; ++i) {
+        const double* p = pos_w + 3 * (size_t)i;
+        const double* v = bearings + 3 * (size_t)i;
+        OVS_REQUIRE(std::isfinite(p[0]) && std::isfinite(p[1]) && std::isfinite(p[2]), OVS_ERR_INVALID_ARG,
+                    "pos_w of correspondence %d is not finite", i);
+        OVS_REQUIRE(std::isfinite(v[0]) && std::isfinite(v[1]) && std::isfinite(v[2]) &&
+                    std::fabs(v[0] * v[0] + v[1] * v[1] + v[2] * v[2] - 1.0) <= 1e-6,
+                    OVS_ERR_INVALID_ARG, "bearing of correspondence %d is not a finite unit vector", i);
+        OVS_REQUIRE(scale_factor[i] > 0.0f && scale_factor[i] <= 90.0f, OVS_ERR_INVALID_ARG,
+                    "scale_factor of correspondence %d must be in (0, 90]", i);
+    }
+    if (n_all == 0) {   // no correspondence at all: no hypothesis, invalid
+        for (int b = 0; b < B; ++b) {
+            ovs::pnp_identity(pose_cw + 12 * (size_t)b);
+            valid[b] = 0; num_inliers[b] = 0; best_iter[b] = -1;
+        }
+        return OVS_OK;
+    }
+    OVS_CUDA_CHECK(cudaSetDevice(h->device));
+    // carved from the same arenas as the pose optimiser: a prepared local-BA problem on this handle is gone
+    invalidate_plan(h);
+    if (h->pending) { OVS_CUDA_CHECK(ovs::sync_stream(h->stream)); h->pending = false; }
+    const size_t N = (size_t)n_all, NB = (size_t)B, H = (size_t)max_num_iter;
+    const size_t in_bytes_max = 256 * 7 + (NB + 1) * 4 + N * (24 + 24 + 4) + NB * (8 + 8);
+    const size_t out_bytes_max = 256 * 5 + NB * (12 * 8 + 4 + 4 + 1) + N;
+    const size_t hbytes = in_bytes_max + out_bytes_max;
+    const size_t dbytes = hbytes + 256 * 3 + N * (8 + 4) + NB * H * 96 + 4096;
+    int rc = ensure_arenas(h, dbytes, hbytes);
+    if (rc != OVS_OK) return rc;
+    Arena Hh{h->h_arena, 0, h->h_cap}, D{h->d_arena, 0, h->d_cap};
+    // inputs: the same carving sequence in both arenas, so one contiguous copy moves them
+    int* hoff = Hh.take<int>(NB + 1);
+    double* hbear = Hh.take<double>(3 * N); double* hpw = Hh.take<double>(3 * N); float* hsf = Hh.take<float>(N);
+    uint64_t* hseed = Hh.take<uint64_t>(NB); unsigned long long* hkey = Hh.take<unsigned long long>(NB);
+    const size_t in_bytes = Hh.off;
+    // outputs: one contiguous copy back
+    double* hpose = Hh.take<double>(12 * NB);
+    const size_t out_begin = (size_t)((uint8_t*)hpose - h->h_arena);
+    int* hnum = Hh.take<int>(NB); int* hbest = Hh.take<int>(NB); uint8_t* hvalid = Hh.take<uint8_t>(NB); uint8_t* hflags = Hh.take<uint8_t>(N);
+    const size_t out_end = Hh.off;
+    PnpArgs A;
+    A.B = B; A.N = n_all; A.H = max_num_iter; A.min_num_inliers = min_num_inliers; A.recompute = recompute ? 1 : 0;
+    A.off = D.take<int>(NB + 1);
+    A.bear = D.take<double>(3 * N); A.pw = D.take<double>(3 * N); A.sf = D.take<float>(N);
+    A.seed = D.take<uint64_t>(NB); A.key = D.take<unsigned long long>(NB);
+    A.pose = D.take<double>(12 * NB); A.num_inliers = D.take<int>(NB); A.best_iter = D.take<int>(NB); A.valid = D.take<uint8_t>(NB);
+    A.inlier = D.take<uint8_t>(N);
+    A.bound = D.take<double>(N); A.cidx = D.take<int>(N); A.hyp = D.take<double>(12 * NB * H);
+    memcpy(hoff, corr_offsets, 4 * (NB + 1));
+    memcpy(hbear, bearings, 24 * N); memcpy(hpw, pos_w, 24 * N); memcpy(hsf, scale_factor, 4 * N);
+    memcpy(hseed, seeds, 8 * NB); memset(hkey, 0, 8 * NB);
+    cudaStream_t st = h->stream;
+    OVS_CUDA_CHECK(cudaMemcpyAsync(h->d_arena, h->h_arena, in_bytes, cudaMemcpyHostToDevice, st));
+    const size_t hyp_threads = std::max(N, NB * H);
+    k_pnp_hypotheses<<<(unsigned)((hyp_threads + kPnpHypThreads - 1) / kPnpHypThreads), kPnpHypThreads, 0, st>>>(A);
+    OVS_LAUNCH_CHECK();
+    if (max_num_iter > 0) {
+        k_pnp_ransac<<<dim3((max_num_iter + kPnpWarps - 1) / kPnpWarps, B), kPnpThreads, 0, st>>>(A);
+        OVS_LAUNCH_CHECK();
+    }
+    k_pnp_refine<<<B, kPnpRefineThreads, 0, st>>>(A);
+    OVS_LAUNCH_CHECK();
+    OVS_CUDA_CHECK(cudaMemcpyAsync(h->h_arena + out_begin, h->d_arena + out_begin, out_end - out_begin, cudaMemcpyDeviceToHost, st));
+    OVS_CUDA_CHECK(ovs::sync_stream(st));
+    memcpy(pose_cw, hpose, 12 * 8 * NB);
     memcpy(num_inliers, hnum, 4 * NB); memcpy(best_iter, hbest, 4 * NB); memcpy(valid, hvalid, NB);
     memcpy(inlier_out, hflags, N);
     return OVS_OK;

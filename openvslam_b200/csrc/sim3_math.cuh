@@ -379,77 +379,75 @@ OVS_BA_HD uint64_t splitmix64_mix(uint64_t z) {
     return z ^ (z >> 31);
 }
 
-// The three distinct pair indices of hypothesis k of a problem with n >= 3 pairs: w_j = mix(seed + golden * (3k + j + 1)),
-// i0 = w0 % n, i1 = w1 % (n - 1) skipping i0, i2 = w2 % (n - 2) skipping min(i0, i1), then max(i0, i1).  No rejection loop.
-OVS_BA_HD void sim3_ransac_triple(uint64_t seed, int k, int n, int* idx) {
-    const uint64_t g = 0x9E3779B97F4A7C15ull, base = 3ull * (uint64_t)k;
-    const uint64_t w0 = splitmix64_mix(seed + g * (base + 1)), w1 = splitmix64_mix(seed + g * (base + 2)),
-                   w2 = splitmix64_mix(seed + g * (base + 3));
-    const int i0 = (int)(w0 % (uint64_t)n);
-    const int c = (int)(w1 % (uint64_t)(n - 1));
-    const int i1 = c + (c >= i0 ? 1 : 0);
-    const int lo = i0 < i1 ? i0 : i1, hi = i0 < i1 ? i1 : i0;
-    int i2 = (int)(w2 % (uint64_t)(n - 2));
-    if (i2 >= lo) ++i2;
-    if (i2 >= hi) ++i2;
-    idx[0] = i0; idx[1] = i1; idx[2] = i2;
+// The m distinct indices of hypothesis k of a problem with n >= m entries: w_j = mix(seed + golden * (m k + j + 1)),
+// c_j = w_j % (n - j), then c_j steps past the indices drawn before it, visited in ascending order (+1 for each one <= it).
+// No rejection loop.  m = 3 is the Sim3 solver's triple, m = 6 the PnP solver's minimal set.
+template <int m>
+OVS_BA_HD void ransac_sample(uint64_t seed, int k, int n, int* idx) {
+    const uint64_t g = 0x9E3779B97F4A7C15ull, base = (uint64_t)m * (uint64_t)k;
+    int sorted[m];                                   // the indices drawn so far, ascending
+    for (int j = 0; j < m; ++j) {
+        int c = (int)(splitmix64_mix(seed + g * (base + (uint64_t)j + 1)) % (uint64_t)(n - j));
+        int pos = 0;
+        for (; pos < j && c >= sorted[pos]; ++pos) ++c;
+        for (int a = j; a > pos; --a) sorted[a] = sorted[a - 1];
+        sorted[pos] = c;
+        idx[j] = c;
+    }
 }
 
-// Cyclic Jacobi on a symmetric 4 x 4 A (row-major, overwritten: its diagonal ends as the eigenvalues); V (row-major) gets the
-// eigenvectors as columns.  Sweeps visit (0,1) (0,2) (0,3) (1,2) (1,3) (2,3); a sweep starts only while the off-diagonal sum of
+// The three distinct pair indices of hypothesis k of a problem with n >= 3 pairs: ransac_sample with m = 3, i.e.
+// i0 = w0 % n, i1 = w1 % (n - 1) skipping i0, i2 = w2 % (n - 2) skipping min(i0, i1), then max(i0, i1).
+OVS_BA_HD void sim3_ransac_triple(uint64_t seed, int k, int n, int* idx) { ransac_sample<3>(seed, k, n, idx); }
+
+// Cyclic Jacobi on a symmetric N x N A (row-major, overwritten: its diagonal ends as the eigenvalues); V (row-major) gets the
+// eigenvectors as columns.  Sweeps visit (p, q) for p < q in row-major order; a sweep starts only while the off-diagonal sum of
 // squares exceeds 1e-30 of the matrix's (at entry), at most 16 sweeps.  Rotation: theta = (a_qq - a_pp) / (2 a_pq),
 // t = sign(theta) / (|theta| + sqrt(theta^2 + 1)), c = 1 / sqrt(t^2 + 1), s = t c; a_pq is set to zero after it.
-OVS_BA_HD void jacobi4(double* A, double* V) {
-    for (int k = 0; k < 16; ++k) V[k] = (k % 5 == 0) ? 1.0 : 0.0;
+template <int N>
+OVS_BA_HD void jacobi_sym(double* A, double* V) {
+    for (int k = 0; k < N * N; ++k) V[k] = (k % (N + 1) == 0) ? 1.0 : 0.0;
     double frob = 0.0;
-    for (int k = 0; k < 16; ++k) frob += A[k] * A[k];
+    for (int k = 0; k < N * N; ++k) frob += A[k] * A[k];
     for (int sweep = 0; sweep < 16; ++sweep) {
         double off = 0.0;
-        for (int p = 0; p < 3; ++p)
-            for (int q = p + 1; q < 4; ++q) off += A[4 * p + q] * A[4 * p + q];
+        for (int p = 0; p < N - 1; ++p)
+            for (int q = p + 1; q < N; ++q) off += A[N * p + q] * A[N * p + q];
         if (!(off > 1e-30 * frob)) break;
-        for (int p = 0; p < 3; ++p)
-            for (int q = p + 1; q < 4; ++q) {
-                const double apq = A[4 * p + q];
+        for (int p = 0; p < N - 1; ++p)
+            for (int q = p + 1; q < N; ++q) {
+                const double apq = A[N * p + q];
                 if (apq == 0.0) continue;
-                const double theta = (A[4 * q + q] - A[4 * p + p]) / (2.0 * apq);
+                const double theta = (A[N * q + q] - A[N * p + p]) / (2.0 * apq);
                 double t = 1.0 / (fabs(theta) + sqrt(theta * theta + 1.0));
                 if (theta < 0.0) t = -t;
                 const double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
-                for (int r = 0; r < 4; ++r) {      // columns p, q
-                    const double arp = A[4 * r + p], arq = A[4 * r + q];
-                    A[4 * r + p] = c * arp - s * arq;
-                    A[4 * r + q] = s * arp + c * arq;
+                for (int r = 0; r < N; ++r) {      // columns p, q
+                    const double arp = A[N * r + p], arq = A[N * r + q];
+                    A[N * r + p] = c * arp - s * arq;
+                    A[N * r + q] = s * arp + c * arq;
                 }
-                for (int r = 0; r < 4; ++r) {      // rows p, q
-                    const double apr = A[4 * p + r], aqr = A[4 * q + r];
-                    A[4 * p + r] = c * apr - s * aqr;
-                    A[4 * q + r] = s * apr + c * aqr;
+                for (int r = 0; r < N; ++r) {      // rows p, q
+                    const double apr = A[N * p + r], aqr = A[N * q + r];
+                    A[N * p + r] = c * apr - s * aqr;
+                    A[N * q + r] = s * apr + c * aqr;
                 }
-                A[4 * p + q] = 0.0; A[4 * q + p] = 0.0;
-                for (int r = 0; r < 4; ++r) {
-                    const double vrp = V[4 * r + p], vrq = V[4 * r + q];
-                    V[4 * r + p] = c * vrp - s * vrq;
-                    V[4 * r + q] = s * vrp + c * vrq;
+                A[N * p + q] = 0.0; A[N * q + p] = 0.0;
+                for (int r = 0; r < N; ++r) {
+                    const double vrp = V[N * r + p], vrq = V[N * r + q];
+                    V[N * r + p] = c * vrp - s * vrq;
+                    V[N * r + q] = s * vrp + c * vrq;
                 }
             }
     }
 }
 
-// compute_Sim3 by Horn's closed form on three point pairs (p1[3 * j + c]: point j in keyframe 1's camera frame, p2 likewise):
-// centroids, M = A2 A1^T, Horn's 4 x 4 N, the quaternion (w, x, y, z) = the eigenvector of N's largest eigenvalue (lowest index
-// on ties), R_12 directly from it (divided by |q|^2), s = sum A1 . (R A2) / sum |A2|^2 (1 with fix_scale), t = c1 - s R c2.
-// S_21 = S_12^-1.  Coincident or collinear points are not special-cased.
-OVS_BA_HD void sim3_horn(const double* p1, const double* p2, bool fix_scale, double* S12, double* S21) {
-    double c1[3], c2[3], A1[9], A2[9];   // A[3 * r + j]: coordinate r of centred point j
-    for (int r = 0; r < 3; ++r) {
-        c1[r] = (p1[r] + p1[3 + r] + p1[6 + r]) / 3.0;
-        c2[r] = (p2[r] + p2[3 + r] + p2[6 + r]) / 3.0;
-        for (int j = 0; j < 3; ++j) { A1[3 * r + j] = p1[3 * j + r] - c1[r]; A2[3 * r + j] = p2[3 * j + r] - c2[r]; }
-    }
-    double M[9];
-    for (int a = 0; a < 3; ++a)
-        for (int b = 0; b < 3; ++b) M[3 * a + b] = A2[3 * a] * A1[3 * b] + A2[3 * a + 1] * A1[3 * b + 1] + A2[3 * a + 2] * A1[3 * b + 2];
+OVS_BA_HD void jacobi4(double* A, double* V) { jacobi_sym<4>(A, V); }
+
+// The rotation of absolute orientation from the correlation M = sum (a - a0)(b - b0)^T of centred source points a and target
+// points b (M[3 * r + c]: source coordinate r, target coordinate c): Horn's 4 x 4 N, the quaternion (w, x, y, z) = the
+// eigenvector of N's largest eigenvalue (lowest index on ties), R (row-major, b ~ R a) directly from it (divided by |q|^2).
+OVS_BA_HD void horn_rotation(const double* M, double* R) {
     const double Sxx = M[0], Sxy = M[1], Sxz = M[2], Syx = M[3], Syy = M[4], Syz = M[5], Szx = M[6], Szy = M[7], Szz = M[8];
     double N[16] = {Sxx + Syy + Szz, Syz - Szy, Szx - Sxz, Sxy - Syx,
                     Syz - Szy, Sxx - Syy - Szz, Sxy + Syx, Szx + Sxz,
@@ -462,10 +460,26 @@ OVS_BA_HD void sim3_horn(const double* p1, const double* p2, bool fix_scale, dou
         if (N[5 * k] > N[5 * m]) m = k;
     const double w = V[m], x = V[4 + m], y = V[8 + m], z = V[12 + m];
     const double nq = w * w + x * x + y * y + z * z;
-    double* R = S12;
     R[0] = (w * w + x * x - y * y - z * z) / nq; R[1] = 2.0 * (x * y - w * z) / nq;         R[2] = 2.0 * (x * z + w * y) / nq;
     R[3] = 2.0 * (x * y + w * z) / nq;         R[4] = (w * w - x * x + y * y - z * z) / nq; R[5] = 2.0 * (y * z - w * x) / nq;
     R[6] = 2.0 * (x * z - w * y) / nq;         R[7] = 2.0 * (y * z + w * x) / nq;         R[8] = (w * w - x * x - y * y + z * z) / nq;
+}
+
+// compute_Sim3 by Horn's closed form on three point pairs (p1[3 * j + c]: point j in keyframe 1's camera frame, p2 likewise):
+// centroids, M = A2 A1^T, R_12 = horn_rotation(M), s = sum A1 . (R A2) / sum |A2|^2 (1 with fix_scale), t = c1 - s R c2.
+// S_21 = S_12^-1.  Coincident or collinear points are not special-cased.
+OVS_BA_HD void sim3_horn(const double* p1, const double* p2, bool fix_scale, double* S12, double* S21) {
+    double c1[3], c2[3], A1[9], A2[9];   // A[3 * r + j]: coordinate r of centred point j
+    for (int r = 0; r < 3; ++r) {
+        c1[r] = (p1[r] + p1[3 + r] + p1[6 + r]) / 3.0;
+        c2[r] = (p2[r] + p2[3 + r] + p2[6 + r]) / 3.0;
+        for (int j = 0; j < 3; ++j) { A1[3 * r + j] = p1[3 * j + r] - c1[r]; A2[3 * r + j] = p2[3 * j + r] - c2[r]; }
+    }
+    double M[9];
+    for (int a = 0; a < 3; ++a)
+        for (int b = 0; b < 3; ++b) M[3 * a + b] = A2[3 * a] * A1[3 * b] + A2[3 * a + 1] * A1[3 * b + 1] + A2[3 * a + 2] * A1[3 * b + 2];
+    double* R = S12;
+    horn_rotation(M, R);
     double s = 1.0;
     if (!fix_scale) {
         double num = 0.0, den = 0.0;

@@ -1,7 +1,8 @@
-"""Host-side mirror of openvslam::solve::sim3_solver (src/openvslam/solve/sim3_solver.h; names as in SURVEY.md 8a) over the C ABI
-of libovs_b200.so: loop detection's Sim3 RANSAC, solved on the GPU for a whole batch of loop candidates in one call.  The
-reference constructs one solver per candidate from two keyframes and their matched landmarks; here each candidate is a
-`problem` of flat arrays (see include/ovs_b200.h, ovs_sim3_solve_ransac_host, for the field-by-field mapping)."""
+"""Host-side mirror of openvslam::solve::sim3_solver and solve::pnp_solver (src/openvslam/solve/{sim3,pnp}_solver.h; names as in
+SURVEY.md 8a) over the C ABI of libovs_b200.so: loop detection's Sim3 RANSAC and relocalisation's PnP RANSAC, each solved on the
+GPU for a whole batch of candidates in one call.  The reference constructs one solver per candidate; here each candidate is a
+`problem` of flat arrays (see include/ovs_b200.h, ovs_sim3_solve_ransac_host / ovs_pnp_solve_ransac_host, for the field-by-field
+mapping)."""
 import ctypes as C
 
 import numpy as np
@@ -61,4 +62,51 @@ class sim3_solver(_optimizer_handle):
                                                          self.min_num_inliers_, int(max_num_iter), pseed, vp(S), vp(valid), vp(ninl), vp(best),
                                                          vp(flags)))
         return [dict(valid=bool(valid[b]), sim3_12=S[b].copy(), num_inliers=int(ninl[b]), best_iter=int(best[b]),
+                     inliers=flags[off[b]:off[b + 1]].astype(bool)) for b in range(B)]
+
+
+class pnp_solver(_optimizer_handle):
+    """openvslam::solve::pnp_solver(valid_bearings, valid_keypts, valid_points, scale_factors, min_num_inliers = 10), batched.
+
+    find_via_ransac(problems, max_num_iter=30, recompute=True, seeds=None): problems is a list of dicts with
+      bearings      (n, 3) unit bearings of the frame keypoints (frm.bearings_),
+      pos_w         (n, 3) world positions of the matched landmarks,
+      scale_factor  (n,) scale_factors_[octave] of each keypoint, in (0, 90];
+    seeds: one sampler seed per problem (default: the problem's index).  A problem gives the same result alone or in a batch.
+    Returns one dict per problem: valid (solution_is_valid()), pose_cw {R row-major (9), t (3)} (get_best_cam_pose()),
+    num_inliers, best_iter (-1: no hypothesis had an inlier), inliers (n,) bool (get_inlier_flags())."""
+
+    def __init__(self, min_num_inliers=10, device=0):
+        super().__init__(device)
+        self.min_num_inliers_ = int(min_num_inliers)
+
+    def find_via_ransac(self, problems, max_num_iter=30, recompute=True, seeds=None):
+        B = len(problems)
+        counts = []
+        for p in problems:
+            n = len(np.asarray(p["scale_factor"]).reshape(-1))
+            if not (np.asarray(p["bearings"]).size == np.asarray(p["pos_w"]).size == 3 * n):
+                raise ValueError("pnp_solver: bearings / pos_w need (n, 3) and scale_factor n entries")
+            counts.append(n)
+        off = np.zeros(B + 1, np.int32)
+        off[1:] = np.cumsum(counts)
+        N = int(off[-1])
+        seeds = np.arange(B, dtype=np.uint64) if seeds is None else np.asarray(seeds, np.uint64).reshape(-1)
+        if len(seeds) != B:
+            raise ValueError("pnp_solver: one seed per problem")
+
+        def cat(key, width, dt):
+            if N == 0:
+                return np.zeros((1, width) if width > 1 else 1, dt)
+            return np.concatenate([np.asarray(p[key], dt).reshape(-1, width) if width > 1 else np.asarray(p[key], dt).reshape(-1)
+                                   for p in problems])
+        b, pb = _p(cat("bearings", 3, np.float64), np.float64); w, pw = _p(cat("pos_w", 3, np.float64), np.float64)
+        s, ps = _p(cat("scale_factor", 1, np.float32), np.float32)
+        off_, po = _p(off, np.int32); seeds_, pseed = _p(seeds if B else np.zeros(1, np.uint64), np.uint64)
+        pose = np.zeros((max(B, 1), 12)); valid = np.zeros(max(B, 1), np.uint8)
+        ninl = np.zeros(max(B, 1), np.int32); best = np.zeros(max(B, 1), np.int32); flags = np.zeros(max(N, 1), np.uint8)
+        vp = lambda a: a.ctypes.data_as(C.c_void_p)
+        _lib.check(_lib.lib().ovs_pnp_solve_ransac_host(self._h, B, po, pb, pw, ps, self.min_num_inliers_, int(max_num_iter),
+                                                        int(bool(recompute)), pseed, vp(pose), vp(valid), vp(ninl), vp(best), vp(flags)))
+        return [dict(valid=bool(valid[b]), pose_cw=pose[b].copy(), num_inliers=int(ninl[b]), best_iter=int(best[b]),
                      inliers=flags[off[b]:off[b + 1]].astype(bool)) for b in range(B)]
