@@ -11,6 +11,10 @@
 //   solve::pnp_solver(const eigen_alloc_vector<bearing_t>&, const std::vector<cv::KeyPoint>&, const eigen_alloc_vector<Vec3_t>&,
 //     const std::vector<float>&, unsigned), find_via_ransac(unsigned, bool), solution_is_valid(), get_best_{rotation,translation,
 //     cam_pose}(), get_inlier_flags()                                                                            (solve/pnp_solver.h)
+//   solve::essential_solver(const eigen_alloc_vector<bearing_t>&, const eigen_alloc_vector<bearing_t>&,
+//     const std::vector<std::pair<int, int>>&), find_via_ransac(unsigned, bool), solution_is_valid(), get_best_E_21(),
+//     get_inlier_matches()                                                                                       (solve/essential_solver.h)
+//   match::robust::match_frame_and_keyframe(data::frame&, data::keyframe*, std::vector<data::landmark*>&)       (match/robust.h)
 //
 // Include it INSTEAD of openvslam_b200.hpp in a translation unit that can see the reference's headers (here: the stand-ins
 // under tests/cpp/standin, which declare the members used below with the names recalled in SURVEY.md section 2 / 8b;
@@ -104,6 +108,33 @@ struct frame_arrays {
     }
 };
 
+//! The sampler seed of a solver built with the reference's constructor: a splitmix64 hash of the input bits (8-byte words, the
+//! last one zero-padded), so the same input always gives the same solution.
+struct input_hash {
+    std::uint64_t seed;
+    explicit input_hash(const std::size_t n) : seed(0x9E3779B97F4A7C15ull ^ static_cast<std::uint64_t>(n)) {}
+    void add(const void* p, const std::size_t bytes) {
+        const unsigned char* c = static_cast<const unsigned char*>(p);
+        for (std::size_t k = 0; k < bytes; k += 8) {
+            std::uint64_t w = 0;
+            std::memcpy(&w, c + k, std::min<std::size_t>(8, bytes - k));
+            std::uint64_t z = seed + w + 0x9E3779B97F4A7C15ull;   // splitmix64's output function over the running state
+            z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+            z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+            seed = z ^ (z >> 31);
+        }
+    }
+};
+
+//! bearings_ of a frame or keyframe as 3 doubles per keypoint
+template <class BearingVector>
+std::vector<double> flat_bearings(const BearingVector& bearings) {
+    std::vector<double> out(3 * bearings.size());
+    for (std::size_t i = 0; i < bearings.size(); ++i)
+        for (int k = 0; k < 3; ++k) out[3 * i + k] = bearings[i](k);
+    return out;
+}
+
 }  // namespace adapters
 
 // ---------------------------------------------------------------------------------------------------- match::robust
@@ -116,6 +147,31 @@ inline unsigned int match::robust::brute_force_match(data::frame& frm, data::key
     for (int i = 0; i < n1; ++i) std::memcpy(&d1[32 * static_cast<std::size_t>(i)], frm.descriptors_.ptr(i), 32);
     for (int i = 0; i < n2; ++i) std::memcpy(&d2[32 * static_cast<std::size_t>(i)], keyfrm->descriptors_.ptr(i), 32);
     return brute_force_match(d1.data(), n1, d2.data(), n2, valid.data(), matches);
+}
+
+// match_frame_and_keyframe: the brute force over the same arrays as brute_force_match, the essential-matrix RANSAC on the pairs
+// (find_via_ransac(50, false)), and matched_lms_in_frm[idx_1] = keyfrm->get_landmarks()[idx_2] for each inlier pair of a valid
+// solution.  The sampler seed hashes both bearing sets.  Frame / Keyframe are data::frame / data::keyframe in the reference tree.
+template <class Frame, class Keyframe>
+inline unsigned int match::robust::match_frame_and_keyframe(Frame& frm, Keyframe* keyfrm,
+                                                            std::vector<data::landmark*>& matched_lms_in_frm) const {
+    const auto lms_2 = keyfrm->get_landmarks();
+    const int n1 = static_cast<int>(frm.num_keypts_), n2 = static_cast<int>(keyfrm->num_keypts_);
+    std::vector<std::uint8_t> valid(static_cast<std::size_t>(std::max(n2, 1)), 0);
+    for (int i = 0; i < n2 && i < static_cast<int>(lms_2.size()); ++i) valid[i] = lms_2[i] && !lms_2[i]->will_be_erased();
+    std::vector<std::uint8_t> d1(static_cast<std::size_t>(n1) * 32), d2(static_cast<std::size_t>(n2) * 32);
+    for (int i = 0; i < n1; ++i) std::memcpy(&d1[32 * static_cast<std::size_t>(i)], frm.descriptors_.ptr(i), 32);
+    for (int i = 0; i < n2; ++i) std::memcpy(&d2[32 * static_cast<std::size_t>(i)], keyfrm->descriptors_.ptr(i), 32);
+    const std::vector<double> b1 = adapters::flat_bearings(frm.bearings_), b2 = adapters::flat_bearings(keyfrm->bearings_);
+    adapters::input_hash hash(b1.size() + b2.size());
+    hash.add(b1.data(), 8 * b1.size());
+    hash.add(b2.data(), 8 * b2.size());
+    std::vector<int> idx_2;
+    const unsigned int num = match_frame_and_keyframe(d1.data(), b1.data(), n1, d2.data(), b2.data(), n2, valid.data(), idx_2, 50, hash.seed);
+    matched_lms_in_frm.assign(static_cast<std::size_t>(n1), nullptr);
+    for (int i = 0; i < n1; ++i)
+        if (idx_2[i] >= 0) matched_lms_in_frm[i] = lms_2.at(static_cast<std::size_t>(idx_2[i]));
+    return num;
 }
 
 // ------------------------------------------------------------------------------------------------ match::projection
@@ -333,30 +389,19 @@ inline solve::pnp_solver::pnp_solver(const BearingVector& valid_bearings, const 
                                      const unsigned int min_num_inliers)
     : pnp_solver(min_num_inliers) {
     const std::size_t n = valid_bearings.size();
-    std::uint64_t seed = 0x9E3779B97F4A7C15ull ^ static_cast<std::uint64_t>(n);
-    auto hash = [&seed](const void* p, const std::size_t bytes) {
-        const unsigned char* c = static_cast<const unsigned char*>(p);
-        for (std::size_t k = 0; k < bytes; k += 8) {
-            std::uint64_t w = 0;
-            std::memcpy(&w, c + k, std::min<std::size_t>(8, bytes - k));
-            std::uint64_t z = seed + w + 0x9E3779B97F4A7C15ull;   // splitmix64's output function over the running state
-            z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-            z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-            seed = z ^ (z >> 31);
-        }
-    };
+    adapters::input_hash hash(n);
     for (std::size_t i = 0; i < n; ++i) {
         const auto& b = valid_bearings[i];
         const auto& p = valid_points.at(i);
         for (int k = 0; k < 3; ++k) { own_bearings_.push_back(b(k)); own_pos_w_.push_back(p(k)); }
         own_scale_factor_.push_back(scale_factors.at(static_cast<std::size_t>(valid_keypts.at(i).octave)));
     }
-    hash(own_bearings_.data(), 8 * own_bearings_.size());
-    hash(own_pos_w_.data(), 8 * own_pos_w_.size());
-    hash(own_scale_factor_.data(), 4 * own_scale_factor_.size());
+    hash.add(own_bearings_.data(), 8 * own_bearings_.size());
+    hash.add(own_pos_w_.data(), 8 * own_pos_w_.size());
+    hash.add(own_scale_factor_.data(), 4 * own_scale_factor_.size());
     own_.num_corrs = static_cast<int>(n);
     own_.bearings = own_bearings_.data(); own_.pos_w = own_pos_w_.data(); own_.scale_factor = own_scale_factor_.data();
-    own_.seed = seed;
+    own_.seed = hash.seed;
 }
 
 inline void solve::pnp_solver::find_via_ransac(const unsigned int max_num_iter, const bool recompute) {
@@ -377,5 +422,37 @@ inline Vec3_t solve::pnp_solver::get_best_translation() const {
 }
 
 inline Mat44_t solve::pnp_solver::get_best_cam_pose() const { return adapters::from_Rt(best_.pose_cw); }
+
+// ------------------------------------------------------------------------------------------- solve::essential_solver
+// The reference's constructor takes both views' bearings and the matches (idx_1, idx_2); the bearings are gathered per match here.
+// The sampler seed is a splitmix64 hash of the gathered bearings (the PnP adapter's rule).
+template <class BearingVector>
+inline solve::essential_solver::essential_solver(const BearingVector& bearings_1, const BearingVector& bearings_2,
+                                                 const std::vector<std::pair<int, int>>& matches_12)
+    : essential_solver() {
+    const std::size_t n = matches_12.size();
+    for (const auto& m : matches_12) {
+        const auto& b1 = bearings_1.at(static_cast<std::size_t>(m.first));
+        const auto& b2 = bearings_2.at(static_cast<std::size_t>(m.second));
+        for (int k = 0; k < 3; ++k) { own_bearings_1_.push_back(b1(k)); own_bearings_2_.push_back(b2(k)); }
+    }
+    adapters::input_hash hash(n);
+    hash.add(own_bearings_1_.data(), 8 * own_bearings_1_.size());
+    hash.add(own_bearings_2_.data(), 8 * own_bearings_2_.size());
+    own_.num_matches = static_cast<int>(n);
+    own_.bearings_1 = own_bearings_1_.data(); own_.bearings_2 = own_bearings_2_.data();
+    own_.seed = hash.seed;
+}
+
+inline void solve::essential_solver::find_via_ransac(const unsigned int max_num_iter, const bool recompute) {
+    best_ = find_via_ransac(std::vector<problem_view>{own_}, max_num_iter, recompute).front();
+}
+
+inline Mat33_t solve::essential_solver::get_best_E_21() const {
+    Mat33_t E;
+    for (int r = 0; r < 3; ++r)
+        for (int c = 0; c < 3; ++c) E(r, c) = best_.E_21[3 * r + c];
+    return E;
+}
 
 }  // namespace openvslam

@@ -6,6 +6,7 @@
 //   openvslam::optimize::pose_optimizer / local_bundle_adjuster / transform_optimizer / graph_optimizer (src/openvslam/optimize/*.h)
 //   openvslam::solve::sim3_solver                         (src/openvslam/solve/sim3_solver.h)
 //   openvslam::solve::pnp_solver                          (src/openvslam/solve/pnp_solver.h)
+//   openvslam::solve::essential_solver                    (src/openvslam/solve/essential_solver.h)
 // [file names as recalled in SURVEY.md 8(a); /root/reference holds no source, so no line numbers].
 //
 // The reference's methods take cv::Mat / cv::KeyPoint / Eigen / data::frame / data::keyframe.  None of
@@ -243,9 +244,28 @@ public:
         for (int i = 0; i < n; ++i) matches.emplace_back(pairs[2 * i], pairs[2 * i + 1]);
         return static_cast<unsigned int>(n);
     }
+    //! match_frame_and_keyframe(frm, keyfrm, matched_lms_in_frm) on arrays: brute_force_match, then the essential-matrix RANSAC on
+    //! the pairs (find_via_ransac(max_num_iter, false)); matched_keyfrm_idx_of_frm[idx_1] = idx_2 of each inlier pair, else -1.
+    //! bearings_*: 3 doubles per keypoint (frm.bearings_, keyfrm->bearings_).  Returns the reference's count (0: no valid solution).
+    unsigned int match_frame_and_keyframe(const std::uint8_t* descs_frm, const double* bearings_frm, const int num_keypts_frm,
+                                          const std::uint8_t* descs_keyfrm, const double* bearings_keyfrm, const int num_keypts_keyfrm,
+                                          const std::uint8_t* keyfrm_lm_valid, std::vector<int>& matched_keyfrm_idx_of_frm,
+                                          const unsigned int max_num_iter = 50, const std::uint64_t seed = 0) const {
+        std::vector<std::int32_t> m(static_cast<std::size_t>(std::max(1, num_keypts_frm)), -1);
+        int n = 0;
+        detail::check(ovs_robust_match_frame_and_keyframe_host(h_, descs_frm, bearings_frm, num_keypts_frm, descs_keyfrm, bearings_keyfrm,
+                                                               num_keypts_keyfrm, keyfrm_lm_valid, lowe_ratio_, static_cast<int>(max_num_iter),
+                                                               seed, m.data(), &n));
+        matched_keyfrm_idx_of_frm.assign(m.begin(), m.begin() + std::max(0, num_keypts_frm));
+        return static_cast<unsigned int>(n);
+    }
 #ifdef OVS_B200_WITH_REFERENCE_TYPES
-    //! The reference's signature (match/robust.h); body in adapters.hpp.
+    //! The reference's signatures (match/robust.h); bodies in adapters.hpp.  match_frame_and_keyframe reads bearings_ of the frame
+    //! and the keyframe: it is a template deduced from the arguments (data::frame / data::keyframe in the reference tree), so its
+    //! body is compiled only where it is called, and a data model whose frame does not carry bearings_ can use the other methods.
     unsigned int brute_force_match(data::frame& frm, data::keyframe* keyfrm, std::vector<std::pair<int, int>>& matches) const;
+    template <class Frame, class Keyframe>
+    unsigned int match_frame_and_keyframe(Frame& frm, Keyframe* keyfrm, std::vector<data::landmark*>& matched_lms_in_frm) const;
 #endif
     //! match_for_triangulation(keyfrm_1, keyfrm_2, E_12, matched_idx_pairs): the keyframes' BoW feature vectors come in as
     //! per-keypoint node ids; matched pairs = (idx in keyframe 1, idx in keyframe 2)
@@ -690,6 +710,87 @@ private:
     problem_view own_{};                                   // the reference constructor's flattened candidate
     std::vector<double> own_bearings_, own_pos_w_;
     std::vector<float> own_scale_factor_;
+    solution best_{};
+};
+
+//! solve::essential_solver (the tracker's robust match, equirectangular map initialisation): RANSAC over the eight-point algorithm
+//! on bearing matches, with an optional refit on all inliers.  The reference builds one solver per pair of views; here
+//! find_via_ransac(problems, max_num_iter, recompute) solves a whole batch in one call, and the reference's constructor /
+//! find_via_ransac(max_num_iter, recompute) / getters are in adapters.hpp.
+class essential_solver {
+public:
+    //! One problem on array views (see include/ovs_b200.h, ovs_essential_solve_ransac_host).
+    struct problem_view {
+        int num_matches = 0;
+        const double* bearings_1 = nullptr;               // 3 per match, unit: bearings_1_[matches_12_[i].first]
+        const double* bearings_2 = nullptr;               // 3 per match, unit: bearings_2_[matches_12_[i].second]
+        std::uint64_t seed = 0;
+    };
+    struct solution {
+        bool valid = false;
+        double E_21[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};     // row-major, b2^T E_21 b1 = 0
+        unsigned int num_inliers = 0;
+        int best_iter = -1;
+        double best_score = 0.0;
+        std::vector<std::uint8_t> is_inlier;
+    };
+
+    explicit essential_solver(const int device = 0) { detail::check(ovs_matcher_create(device, &h_)); }
+    ~essential_solver() { ovs_matcher_destroy(h_); }
+    essential_solver(const essential_solver&) = delete;
+    essential_solver& operator=(const essential_solver&) = delete;
+
+    //! find_via_ransac(max_num_iter, recompute) for every problem, one GPU call
+    std::vector<solution> find_via_ransac(const std::vector<problem_view>& problems, const unsigned int max_num_iter,
+                                          const bool recompute = true) const {
+        const int B = static_cast<int>(problems.size());
+        std::vector<std::int32_t> off(static_cast<std::size_t>(B) + 1, 0);
+        for (int b = 0; b < B; ++b) off[b + 1] = off[b] + problems[b].num_matches;
+        const std::size_t N = static_cast<std::size_t>(off[B]);
+        std::vector<double> b1(std::max<std::size_t>(3 * N, 3)), b2(std::max<std::size_t>(3 * N, 3));
+        std::vector<std::uint64_t> seeds(std::max(B, 1));
+        for (int b = 0; b < B; ++b) {
+            const problem_view& p = problems[b];
+            seeds[b] = p.seed;
+            const std::size_t o = static_cast<std::size_t>(off[b]), n = static_cast<std::size_t>(p.num_matches);
+            if (n == 0) continue;
+            std::memcpy(&b1[3 * o], p.bearings_1, 24 * n); std::memcpy(&b2[3 * o], p.bearings_2, 24 * n);
+        }
+        std::vector<double> E(9 * static_cast<std::size_t>(std::max(B, 1))), score(std::max(B, 1));
+        std::vector<std::uint8_t> valid(std::max(B, 1)), flags(std::max<std::size_t>(N, 1));
+        std::vector<std::int32_t> num(std::max(B, 1)), best(std::max(B, 1));
+        detail::check(ovs_essential_solve_ransac_host(h_, B, off.data(), b1.data(), b2.data(), static_cast<int>(max_num_iter), recompute ? 1 : 0,
+                                                      seeds.data(), E.data(), valid.data(), num.data(), best.data(), score.data(), flags.data()));
+        std::vector<solution> out(B);
+        for (int b = 0; b < B; ++b) {
+            out[b].valid = valid[b] != 0;
+            std::memcpy(out[b].E_21, &E[9 * static_cast<std::size_t>(b)], 9 * sizeof(double));
+            out[b].num_inliers = static_cast<unsigned int>(num[b]);
+            out[b].best_iter = best[b];
+            out[b].best_score = score[b];
+            out[b].is_inlier.assign(flags.begin() + off[b], flags.begin() + off[b + 1]);
+        }
+        return out;
+    }
+
+#ifdef OVS_B200_WITH_REFERENCE_TYPES
+    //! The reference's signatures (solve/essential_solver.h); bodies in adapters.hpp.  The sampler is seeded with a splitmix64 hash
+    //! of the input bits (the batched call takes explicit seeds).  The bearing container is a template parameter: the reference
+    //! passes eigen_alloc_vector<bearing_t>; any random-access container of 3-vectors indexed as v(k) is accepted.
+    template <class BearingVector>
+    essential_solver(const BearingVector& bearings_1, const BearingVector& bearings_2, const std::vector<std::pair<int, int>>& matches_12);
+    void find_via_ransac(const unsigned int max_num_iter, const bool recompute = true);
+    bool solution_is_valid() const { return best_.valid; }
+    Mat33_t get_best_E_21() const;
+    std::vector<bool> get_inlier_matches() const { return std::vector<bool>(best_.is_inlier.begin(), best_.is_inlier.end()); }
+#endif
+    //! the last find_via_ransac(max_num_iter, recompute) of a solver built with the reference's constructor
+    const solution& best_solution() const { return best_; }
+
+private:
+    ovs_matcher* h_ = nullptr;
+    problem_view own_{};                                   // the reference constructor's flattened matches
+    std::vector<double> own_bearings_1_, own_bearings_2_;
     solution best_{};
 };
 

@@ -187,6 +187,42 @@ int ovs_robust_brute_force_match_host(ovs_matcher* h, const uint8_t* desc_frm, i
 int ovs_robust_brute_force_match_device(ovs_matcher* h, const uint8_t* d_desc_frm, int n1, const uint8_t* d_desc_keyfrm, int n2,
                                         const uint8_t* lm_valid_2, float lowe_ratio,
                                         int32_t* pairs_out, int capacity, int* num_matches);
+/* solve::essential_solver(bearings_1, bearings_2, matches_12).find_via_ransac(max_num_iter, recompute) (solve/essential_solver.cc)
+ * for B independent problems in one call.  Problem b owns the matches match_offsets[b] .. match_offsets[b + 1] - 1
+ * (match_offsets[0] = 0, non-decreasing); the bearings are gathered per match: bearings_1[i*3] = bearings_1_[matches_12_[i].first],
+ * bearings_2[i*3] = bearings_2_[matches_12_[i].second] (unit; any camera model: ovs_undistort_keypoints_* produces them).
+ * seeds[B]: the sampler's seed per problem (a problem gives the same result alone or inside a batch).
+ * Per problem: E_21[b*9] = get_best_E_21() row-major (b2^T E_21 b1 = 0; zero when no hypothesis scored above 0), valid[b] =
+ * solution_is_valid() (best score > 0 and at least 8 inliers), num_inliers[b] = the number of inlier flags set, best_iter[b] = the best
+ * hypothesis (-1: none), best_score[b] = its score (after the recompute, when one ran), inlier_out[n] = get_inlier_matches().
+ * Fewer than 8 matches: no hypothesis runs and the problem is invalid.  With recompute, a valid problem is solved again by the
+ * eight-point algorithm on all inliers and its flags, count and score are re-checked at that E_21 (valid keeps its value).  The
+ * sampler, the rank-2 projection, the inlier test, the score and their fixed summation orders are described in DESIGN.md section 5.
+ * B outside 0 .. 65535, invalid offsets, a bearing that is not finite or not unit (|b.b - 1| > 1e-6) or a negative max_num_iter
+ * return OVS_ERR_INVALID_ARG; B == 0 or no match at all returns without a launch.  Otherwise the call is three launches (one with
+ * max_num_iter == 0), one copy each way and one wait.  The solve has its own buffers on the handle: the brute-force entry points
+ * above are unaffected by it. */
+int ovs_essential_solve_ransac_host(ovs_matcher* h, int B, const int32_t* match_offsets, const double* bearings_1, const double* bearings_2,
+                                    int max_num_iter, int recompute, const uint64_t* seeds, double* E_21, uint8_t* valid,
+                                    int32_t* num_inliers, int32_t* best_iter, double* best_score, uint8_t* inlier_out);
+/* match::robust::match_frame_and_keyframe(frm, keyfrm, matched_lms_in_frm) (match/robust.cc), the tracker's robust-match fallback:
+ * ovs_robust_brute_force_match_host (the same pairs, bit for bit), then the essential solver on them with recompute off
+ * (the reference calls find_via_ransac(50, false); pass max_num_iter = 50).  bearings_frm[n1*3] = frm.bearings_,
+ * bearings_keyfrm[n2*3] = keyfrm->bearings_ (unit), gathered by pair index on the device; seed: the sampler's seed.
+ * matched_keyfrm_idx_of_frm[n1] = idx_2 of the inlier pair of frame keypoint idx_1 (the keypoint whose landmark
+ * matched_lms_in_frm[idx_1] receives) or -1; *num_inlier_matches = the reference's return value (0 when the solution is invalid,
+ * e.g. with fewer than 8 pairs). */
+int ovs_robust_match_frame_and_keyframe_host(ovs_matcher* h, const uint8_t* desc_frm, const double* bearings_frm, int n1,
+                                             const uint8_t* desc_keyfrm, const double* bearings_keyfrm, int n2, const uint8_t* lm_valid_2,
+                                             float lowe_ratio, int max_num_iter, uint64_t seed, int32_t* matched_keyfrm_idx_of_frm,
+                                             int* num_inlier_matches);
+/* The same with descriptors and bearings resident in device memory (the outputs of ovs_extract_device and
+ * ovs_undistort_keypoints_device; descriptors 16-byte aligned): only the pair list goes to the device and the flags come back.
+ * lm_valid_2 / matched_keyfrm_idx_of_frm: host. */
+int ovs_robust_match_frame_and_keyframe_device(ovs_matcher* h, const uint8_t* d_desc_frm, const double* d_bearings_frm, int n1,
+                                               const uint8_t* d_desc_keyfrm, const double* d_bearings_keyfrm, int n2, const uint8_t* lm_valid_2,
+                                               float lowe_ratio, int max_num_iter, uint64_t seed, int32_t* matched_keyfrm_idx_of_frm,
+                                               int* num_inlier_matches);
 /* Diagnostic: how many single-query GPU re-searches the greedy replays of this handle have needed. */
 int ovs_matcher_num_requeries(const ovs_matcher* h, int* out);
 /* Device time (CUDA events, microseconds) of the Hamming kernels of the last call. */

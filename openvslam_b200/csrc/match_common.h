@@ -20,6 +20,9 @@ struct ovs_matcher {
     unsigned* d_mask = nullptr; size_t d_mask_cap = 0;
     unsigned* h_keys = nullptr; size_t h_keys_cap = 0;  // pinned
     uint8_t* h_stage = nullptr; size_t h_stage_cap = 0; // pinned
+    // the essential solver's own arenas (essential_ransac.cu): a solve leaves the brute-force buffers above untouched
+    uint8_t* d_ess = nullptr; size_t d_ess_cap = 0;
+    uint8_t* h_ess = nullptr; size_t h_ess_cap = 0;     // pinned
     cudaEvent_t ev[2]{};
     float last_kernel_us = 0.f;
     int num_requeries = 0;   // GPU re-queries issued by the greedy replays so far (diagnostic)

@@ -46,6 +46,7 @@
 
 
 #include "ba_math.cuh"
+#include "block_sum.cuh"
 #include "ovs_common.h"
 #include "pnp_math.cuh"
 #include "sim3_math.cuh"
@@ -2820,8 +2821,8 @@ namespace {
 constexpr int kPnpHypThreads = 64;                   // k_pnp_hypotheses: one thread per hypothesis (and per correspondence)
 constexpr int kPnpWarps = 4;                         // k_pnp_ransac: hypotheses per CTA, one warp each
 constexpr int kPnpThreads = 32 * kPnpWarps;
-constexpr int kPnpRefineThreads = ovs::kPnpSumSlots; // k_pnp_refine: one CTA per problem, one thread per partial sum
-constexpr int kPnpChunk = 8;                         // components reduced per pass of the CTA-wide sum
+constexpr int kPnpRefineThreads = ovs::kBlockSumThreads;   // k_pnp_refine: one CTA per problem, one thread per partial sum
+constexpr int kPnpChunk = ovs::kBlockSumChunk;       // components reduced per pass of the CTA-wide sum
 
 struct PnpArgs {
     int B, N, H, min_num_inliers, recompute;
@@ -2879,36 +2880,8 @@ __global__ void __launch_bounds__(kPnpThreads) k_pnp_ransac(PnpArgs A) {
     if (lane == 0 && cnt > 0) atomicMax(&A.key[b], ((unsigned long long)cnt << 32) | (unsigned long long)(~(unsigned)k));
 }
 
-// pnp_sum across the CTA: thread t forms partial s_t over the points t, t + 256, ..; then, kPnpChunk components at a time,
-// thread c adds the 256 partials of component c in order.  Same bits as PnpSeqSum.
-struct PnpBlockSum {
-    int n;
-    double* red;                                     // shared, kPnpChunk x 256
-    double* res;                                     // shared, 78
-    template <int K, class F> __device__ void run(F f, double* out) const {
-        const int t = threadIdx.x;
-        double s[K], v[K];
-        for (int c = 0; c < K; ++c) s[c] = 0.0;
-        for (int i = t; i < n; i += kPnpRefineThreads) {
-            f(i, v);
-            for (int c = 0; c < K; ++c) s[c] += v[c];
-        }
-#pragma unroll
-        for (int c0 = 0; c0 < K; c0 += kPnpChunk) {
-#pragma unroll
-            for (int c = c0; c < c0 + kPnpChunk && c < K; ++c) red[(c - c0) * kPnpRefineThreads + t] = s[c];
-            __syncthreads();
-            if (t < kPnpChunk && c0 + t < K) {
-                double acc = 0.0;
-                for (int u = 0; u < kPnpRefineThreads; ++u) acc += red[t * kPnpRefineThreads + u];
-                res[c0 + t] = acc;
-            }
-            __syncthreads();
-        }
-        for (int c = 0; c < K; ++c) out[c] = res[c];
-        __syncthreads();
-    }
-};
+// pnp_sum across the CTA (block_sum.cuh): same bits as PnpSeqSum.
+using ovs::PnpBlockSum;
 
 // One CTA per problem: the best hypothesis (or none), its inlier flags, `valid`, and with recompute (valid and at least
 // kPnpMinSet inliers) EPnP on the compacted inliers with the CTA-wide sums and the flags re-checked at that pose.

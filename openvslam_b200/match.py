@@ -90,6 +90,33 @@ class robust(_matcher_handle):
                                                                   C.c_float(self.lowe_ratio_), pairs.ctypes.data_as(C.c_void_p), cap, C.byref(n)))
         return pairs[:n.value].copy()
 
+    def match_frame_and_keyframe(self, desc_frm, bearings_frm, desc_keyfrm, bearings_keyfrm, lm_valid_2=None, max_num_iter=50, seed=0):
+        """robust::match_frame_and_keyframe(frm, keyfrm, matched_lms_in_frm): brute_force_match, then the essential-matrix RANSAC on
+        the pairs (find_via_ransac(max_num_iter, false)) -> (num_inlier_matches, matched_keyfrm_idx_of_frm[n1]): the keyframe keypoint
+        whose landmark frame keypoint i receives, or -1.  bearings_*: (n, 3) unit bearings (frm.bearings_, keyfrm->bearings_)."""
+        d1, p1 = _desc(desc_frm); d2, p2 = _desc(desc_keyfrm)
+        b1, pb1 = _f64(bearings_frm); b2, pb2 = _f64(bearings_keyfrm)
+        if b1.size != 3 * len(d1) or b2.size != 3 * len(d2):
+            raise ValueError("match_frame_and_keyframe: one bearing (3 doubles) per keypoint")
+        _keep, vp = _u8p(lm_valid_2)
+        out = np.full(max(len(d1), 1), -1, np.int32); n = C.c_int(0)
+        _lib.check(_lib.lib().ovs_robust_match_frame_and_keyframe_host(self._h, p1, pb1, len(d1), p2, pb2, len(d2), vp, C.c_float(self.lowe_ratio_),
+                                                                       int(max_num_iter), C.c_uint64(int(seed) & (2 ** 64 - 1)),
+                                                                       out.ctypes.data_as(C.c_void_p), C.byref(n)))
+        return n.value, out[:len(d1)]
+
+    def match_frame_and_keyframe_device(self, d_desc_frm, d_bearings_frm, n1, d_desc_keyfrm, d_bearings_keyfrm, n2, lm_valid_2=None,
+                                        max_num_iter=50, seed=0):
+        """The same on descriptors and bearings resident in device memory (device pointers as ints; the outputs of extract_device
+        and undistort_keypoints_device): only the pair list goes to the device and the flags come back."""
+        _keep, vp = _u8p(lm_valid_2)
+        out = np.full(max(int(n1), 1), -1, np.int32); n = C.c_int(0)
+        _lib.check(_lib.lib().ovs_robust_match_frame_and_keyframe_device(self._h, C.c_void_p(int(d_desc_frm)), C.c_void_p(int(d_bearings_frm)), int(n1),
+                                                                         C.c_void_p(int(d_desc_keyfrm)), C.c_void_p(int(d_bearings_keyfrm)), int(n2), vp,
+                                                                         C.c_float(self.lowe_ratio_), int(max_num_iter),
+                                                                         C.c_uint64(int(seed) & (2 ** 64 - 1)), out.ctypes.data_as(C.c_void_p), C.byref(n)))
+        return n.value, out[:int(n1)]
+
     def match_for_triangulation(self, desc_1, bearing_1, octave_1, angle_1, has_lm_1, is_stereo_1, bow_node_1,
                                 desc_2, bearing_2, angle_2, has_lm_2, is_stereo_2, bow_node_2, E_12, epipole_in_2, scale_factors_1):
         """robust::match_for_triangulation(keyfrm_1, keyfrm_2, E_12, matched_idx_pairs) -> (num_matches, matched_idx_2_of_1[n1]);

@@ -1,13 +1,15 @@
-"""Host-side mirror of openvslam::solve::sim3_solver and solve::pnp_solver (src/openvslam/solve/{sim3,pnp}_solver.h; names as in
-SURVEY.md 8a) over the C ABI of libovs_b200.so: loop detection's Sim3 RANSAC and relocalisation's PnP RANSAC, each solved on the
-GPU for a whole batch of candidates in one call.  The reference constructs one solver per candidate; here each candidate is a
-`problem` of flat arrays (see include/ovs_b200.h, ovs_sim3_solve_ransac_host / ovs_pnp_solve_ransac_host, for the field-by-field
-mapping)."""
+"""Host-side mirror of openvslam::solve::sim3_solver, solve::pnp_solver and solve::essential_solver
+(src/openvslam/solve/{sim3,pnp,essential}_solver.h; names as in SURVEY.md 8a) over the C ABI of libovs_b200.so: loop detection's
+Sim3 RANSAC, relocalisation's PnP RANSAC and the tracker's essential-matrix RANSAC, each solved on the GPU for a whole batch of
+problems in one call.  The reference constructs one solver per problem; here each problem is a `problem` of flat arrays (see
+include/ovs_b200.h, ovs_sim3_solve_ransac_host / ovs_pnp_solve_ransac_host / ovs_essential_solve_ransac_host, for the
+field-by-field mapping)."""
 import ctypes as C
 
 import numpy as np
 
 from . import _lib
+from .match import _matcher_handle
 from .optimize import Camera, _optimizer_handle, _p
 
 
@@ -110,3 +112,44 @@ class pnp_solver(_optimizer_handle):
                                                         int(bool(recompute)), pseed, vp(pose), vp(valid), vp(ninl), vp(best), vp(flags)))
         return [dict(valid=bool(valid[b]), pose_cw=pose[b].copy(), num_inliers=int(ninl[b]), best_iter=int(best[b]),
                      inliers=flags[off[b]:off[b + 1]].astype(bool)) for b in range(B)]
+
+
+class essential_solver(_matcher_handle):
+    """openvslam::solve::essential_solver(bearings_1, bearings_2, matches_12), batched, on a matcher handle (its own buffers: the
+    handle's brute-force matchers are unaffected).
+
+    find_via_ransac(problems, max_num_iter, recompute=True, seeds=None): problems is a list of dicts with
+      bearings_1  (n, 3) unit bearings of camera 1 gathered per match (bearings_1_[matches_12_[i].first]),
+      bearings_2  (n, 3) the same for camera 2 (bearings_2_[matches_12_[i].second]);
+    seeds: one sampler seed per problem (default: the problem's index).  A problem gives the same result alone or in a batch.
+    Returns one dict per problem: valid (solution_is_valid()), E_21 (3, 3) (get_best_E_21(); zero when no hypothesis scored),
+    num_inliers, best_iter (-1: none), best_score, inliers (n,) bool (get_inlier_matches())."""
+
+    def find_via_ransac(self, problems, max_num_iter, recompute=True, seeds=None):
+        B = len(problems)
+        counts = []
+        for p in problems:
+            n = np.asarray(p["bearings_1"]).size // 3
+            if not (np.asarray(p["bearings_1"]).size == np.asarray(p["bearings_2"]).size == 3 * n):
+                raise ValueError("essential_solver: bearings_1 / bearings_2 need (n, 3) each")
+            counts.append(n)
+        off = np.zeros(B + 1, np.int32)
+        off[1:] = np.cumsum(counts)
+        N = int(off[-1])
+        seeds = np.arange(B, dtype=np.uint64) if seeds is None else np.asarray(seeds, np.uint64).reshape(-1)
+        if len(seeds) != B:
+            raise ValueError("essential_solver: one seed per problem")
+
+        def cat(key):
+            if N == 0:
+                return np.zeros((1, 3))
+            return np.concatenate([np.asarray(p[key], np.float64).reshape(-1, 3) for p in problems])
+        b1, pb1 = _p(cat("bearings_1"), np.float64); b2, pb2 = _p(cat("bearings_2"), np.float64)
+        off_, po = _p(off, np.int32); seeds_, pseed = _p(seeds if B else np.zeros(1, np.uint64), np.uint64)
+        E = np.zeros((max(B, 1), 9)); valid = np.zeros(max(B, 1), np.uint8); score = np.zeros(max(B, 1))
+        ninl = np.zeros(max(B, 1), np.int32); best = np.zeros(max(B, 1), np.int32); flags = np.zeros(max(N, 1), np.uint8)
+        vp = lambda a: a.ctypes.data_as(C.c_void_p)
+        _lib.check(_lib.lib().ovs_essential_solve_ransac_host(self._h, B, po, pb1, pb2, int(max_num_iter), int(bool(recompute)), pseed,
+                                                              vp(E), vp(valid), vp(ninl), vp(best), vp(score), vp(flags)))
+        return [dict(valid=bool(valid[b]), E_21=E[b].reshape(3, 3).copy(), num_inliers=int(ninl[b]), best_iter=int(best[b]),
+                     best_score=float(score[b]), inliers=flags[off[b]:off[b + 1]].astype(bool)) for b in range(B)]
