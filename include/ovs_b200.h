@@ -36,7 +36,8 @@ extern "C" {
 #define OVS_ERR_CUDA (-2)
 #define OVS_ERR_NO_DEVICE (-3)
 #define OVS_ERR_CAPACITY (-4)      /* caller-provided output capacity too small */
-#define OVS_ERR_OVERFLOW (-5)      /* internal candidate buffer overflow (pathological image) */
+#define OVS_ERR_OVERFLOW (-5)      /* an internal buffer overflowed: the extractor sizes its candidate and selection buffers
+                                      from bounds that hold for every image, so this reports a library defect */
 #define OVS_ERR_UNSUPPORTED (-6)
 #define OVS_ERR_NUMERIC (-7)       /* linear solve failed (not positive definite) */
 

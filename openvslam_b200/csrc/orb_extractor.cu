@@ -1251,12 +1251,16 @@ int configure(ovs_extractor* h, int w, int hgt) {
         src += h->pyr_groups.back().nlev;
     }
 
-    // detection cells, in the order compute_fast_keypoints visits them
+    // detection cells, in the order compute_fast_keypoints visits them.  A level's candidate slice holds what its cells can emit at
+    // most: the survivors of one cell's strict-max NMS are pairwise non-adjacent, so an rw x rh band yields at most
+    // ceil(rw / 2) * ceil(rh / 2) of them (kCellCap for a full cell).  The bands of neighbouring cells abut and pixels outside a band
+    // count as 0, so survivors on either side of a seam can be adjacent: the per-cell bounds add up.  A dense image comes close to a
+    // quarter of the level's pixels (a lattice of bright pixels at (x + 2 y) % 4 == 0 does).
     h->h_cells.clear(); h->cell_roi.clear();
     size_t cand_cap = 0;
+    size_t level_cand_cap[kMaxLevels] = {};
     for (int l = 0; l < L; ++l) {
         h->level_cell_begin[l] = (int)h->h_cells.size();
-        cand_cap += (size_t)T.w[l] * T.h[l] / 8 + 1024;
         if (T.w[l] <= 2 * kBorder || T.h[l] <= 2 * kBorder) continue;
         const unsigned min_bx = kBorder, min_by = kBorder;
         const unsigned max_bx = T.w[l] - kBorder, max_by = T.h[l] - kBorder;
@@ -1280,8 +1284,12 @@ int configure(ovs_extractor* h, int w, int hgt) {
                 h->h_cells.push_back(ci);
                 h->cell_roi.push_back((int)min_x); h->cell_roi.push_back((int)min_y);
                 h->cell_roi.push_back((int)max_x); h->cell_roi.push_back((int)max_y);
+                level_cand_cap[l] += (size_t)((ci.rw + 1) / 2) * ((ci.rh + 1) / 2);
             }
         }
+        // the tree kernel keeps a candidate's index within its level in 24 bits (the low bits of its best-response keys)
+        OVS_REQUIRE(level_cand_cap[l] < (1u << 24), OVS_ERR_UNSUPPORTED, "image %dx%d: more than 2^24 candidate slots at level %d", w, hgt, l);
+        cand_cap += level_cand_cap[l];
     }
     h->level_cell_begin[L] = (int)h->h_cells.size();
     const size_t nc = h->h_cells.size();
@@ -1293,7 +1301,6 @@ int configure(ovs_extractor* h, int w, int hgt) {
         OVS_CUDA_CHECK(cudaMalloc(&h->d_cell_skip, nc));
         OVS_CUDA_CHECK(cudaHostAlloc(&h->h_cell_skip, nc, cudaHostAllocDefault));
     }
-    OVS_REQUIRE(cand_cap < (1u << 24), OVS_ERR_UNSUPPORTED, "image %dx%d: more than 2^24 candidate slots", w, hgt);
     h->cand_cap = (int)cand_cap;
 
     // tree distribution: initial nodes per level (orb_extractor::initialize_nodes), scratch, selection segments
@@ -1309,7 +1316,7 @@ int configure(ovs_extractor* h, int w, int hgt) {
             A.sf[l] = h->sf[l];
             V.target = (int)h->per_level[l];
             V.cell_begin = h->level_cell_begin[l]; V.cell_end = h->level_cell_begin[l + 1];
-            V.cand_off = (int)cands; V.cand_cap = (int)((size_t)T.w[l] * T.h[l] / 8 + 1024);
+            V.cand_off = (int)cands; V.cand_cap = (int)level_cand_cap[l];
             cands += V.cand_cap;
             const int min_x = kBorder, max_x = T.w[l] - kBorder, min_y = kBorder, max_y = T.h[l] - kBorder;
             V.gx = 1; V.nini = 1; V.delta_x = 1; V.delta_y = 1;

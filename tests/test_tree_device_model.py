@@ -6,6 +6,7 @@ import pytest
 
 from openvslam_b200 import synth
 
+import extractor_limit_cases as lc
 import tree_device_model as tm
 
 
@@ -41,3 +42,30 @@ def test_model_ties_and_clusters(oracle):
         ref = oracle.distribute_via_tree(cl, 19, 619, 19, 419, N)
         got = tm.distribute(cl["x"], cl["y"], cl["score"], 19, 619, 19, 419, N)
         assert np.array_equal(got, ref), N
+
+
+@pytest.mark.parametrize("case", list(lc.TREE_CASES))
+def test_limit_cases_reach_their_sort_branch(oracle, case):
+    """Each tree case of the GPU limit tests reaches the sort branch it is there for: the kernel sorts the largest-first pool and
+    the final selection in shared memory up to SORT_SMEM keys and in global scratch beyond.  The model also equals the oracle's
+    list-based tree at these sizes."""
+    make, n, levels, pool_global, fin_global = lc.TREE_CASES[case]
+    img = make()
+    P = oracle.params(n, num_levels=levels)
+    pyr = oracle.build_pyramid(img, P)
+    sf = oracle.scale_factors(1.2, levels)
+    target = oracle.keypts_per_level(n, 1.2, levels)
+    stats = []
+    for l in range(levels):
+        h, w = pyr[l].shape
+        c = oracle.level_candidates(P, pyr[l], float(sf[l]))
+        st = {}
+        got = tm.distribute(c["x"], c["y"], c["score"], 19, w - 19, 19, h - 19, int(target[l]), stats=st)
+        assert np.array_equal(got, oracle.distribute_via_tree(c, 19, w - 19, 19, h - 19, int(target[l]))), (case, l)
+        assert st["nfin"] == len(got)
+        stats.append(st)
+    assert stats[0]["pool_m"] > 0, stats                    # the largest-first phase is reached
+    assert tuple(l for l, st in enumerate(stats) if st["pool_m"] > lc.SORT_SMEM) == pool_global, stats
+    assert tuple(l for l, st in enumerate(stats) if st["nfin"] > lc.SORT_SMEM) == fin_global, stats
+    if case == "noise1920-n9000":
+        assert stats[0]["pool_m"] == lc.SORT_SMEM          # the largest pool that still sorts in shared memory

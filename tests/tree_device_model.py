@@ -22,9 +22,14 @@ def _child_boxes(pb, k):
     return np.stack([bx, by, ex, ey], 1)
 
 
-def distribute(x, y, score, min_x, max_x, min_y, max_y, num_keypts):
-    """x, y relative to the level border, in candidate (row-major per cell) order.  Returns candidate indices."""
+def distribute(x, y, score, min_x, max_x, min_y, max_y, num_keypts, stats=None):
+    """x, y relative to the level border, in candidate (row-major per cell) order.  Returns candidate indices.
+
+    `stats`, if given, receives the sizes that decide where the kernel sorts: "pool_m", the largest node pool of the
+    largest-first phase (0 if the phase is not reached), and "nfin", the length of the selection."""
     n = len(x)
+    if stats is not None:
+        stats.update(pool_m=0, nfin=0)
     if n == 0:
         return np.zeros(0, np.int64)
     x = np.asarray(x, np.int64); y = np.asarray(y, np.int64); score = np.asarray(score, np.int64)
@@ -100,6 +105,8 @@ def distribute(x, y, score, min_x, max_x, min_y, max_y, num_keypts):
     while phase_b:                                 # phase B: largest nodes first, stop at the budget
         if m == 0:
             break
+        if stats is not None:
+            stats["pool_m"] = max(stats["pool_m"], m)
         prev = Lsize
         order = np.lexsort((np.arange(m), -cnt))   # (count desc, serial desc) == (count desc, index asc)
         rank = np.empty(m, np.int64); rank[order] = np.arange(m)
@@ -131,6 +138,8 @@ def distribute(x, y, score, min_x, max_x, min_y, max_y, num_keypts):
         best = best_of(node[live], live, m)
         for r in range(m):
             fin_key.append((0x7FFFFFFF - ser[r]) if ser[r] >= nini else (0x80000000 + ser[r])); fin_cand.append(best[r])
+    if stats is not None:
+        stats["nfin"] = len(fin_key)
     fk = np.asarray(fin_key, np.int64); fc = np.asarray(fin_cand, np.int64)
     assert len(np.unique(fk)) == len(fk)
     return fc[np.argsort(fk)]
