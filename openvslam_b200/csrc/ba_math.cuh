@@ -147,4 +147,90 @@ OVS_BA_HD bool inv3_sym(const double* D, double* Di) {
 OVS_BA_HD int sym3(int i, int j) { return i <= j ? (i * 3 - i * (i - 1) / 2 + (j - i)) : (j * 3 - j * (j - 1) / 2 + (i - j)); }
 OVS_BA_HD int sym6(int i, int j) { return i <= j ? (i * 6 - i * (i - 1) / 2 + (j - i)) : (j * 6 - j * (j - 1) / 2 + (i - j)); }
 
+// ---- per-edge blocks of the normal equations from the edge's Jacobians, residual and robust weight ww (= rho'(chi2) * info)
+// The bundle adjusters store only {Jp, Jl, ww, e} per edge and form these blocks where they are read, in several kernels; the
+// results must not depend on which kernel forms them, so every product and sum is rounded explicitly, in one fixed order:
+// h = 0, then h += (J[d][a] * ww) * J'[d][b] for d < dim.  dim is the edge's own row count (2, or 3 for a stereo edge); rows
+// beyond it are never added, not even as zeros (+0.0 would turn a -0.0 sum into +0.0).  R = rows of the arrays (>= dim).
+OVS_BA_HD double rn_mul(double a, double b) {
+#if defined(__CUDA_ARCH__)
+    return __dmul_rn(a, b);
+#else
+    return a * b;
+#endif
+}
+OVS_BA_HD double rn_add(double a, double b) {
+#if defined(__CUDA_ARCH__)
+    return __dadd_rn(a, b);
+#else
+    return a + b;
+#endif
+}
+OVS_BA_HD double rn_sub(double a, double b) {
+#if defined(__CUDA_ARCH__)
+    return __dsub_rn(a, b);
+#else
+    return a - b;
+#endif
+}
+
+// Jp' W Jl (6 x 3): out(a, b, element) as each element is formed (a consumer that parks the block elsewhere keeps no copy)
+template <int R, class Out>
+OVS_BA_HD void edge_hpl_each(const double* Jp, const double* Jl, double ww, int dim, Out&& out) {
+    for (int a = 0; a < 6; ++a)
+        for (int b = 0; b < 3; ++b) {
+            double h = 0;
+            for (int d = 0; d < R; ++d)
+                if (d < dim) h = rn_add(h, rn_mul(rn_mul(Jp[6 * d + a], ww), Jl[3 * d + b]));
+            out(a, b, h);
+        }
+}
+// Jp' W Jl (6 x 3, row-major): W[3 a + b]
+template <int R>
+OVS_BA_HD void edge_hpl(const double* Jp, const double* Jl, double ww, int dim, double* W) {
+    edge_hpl_each<R>(Jp, Jl, ww, dim, [W](int a, int b, double h) { W[3 * a + b] = h; });
+}
+// Jl' W Jl (3 x 3, packed upper triangle, sym3)
+template <int R>
+OVS_BA_HD void edge_hll(const double* Jl, double ww, int dim, double* A) {
+    for (int a = 0; a < 3; ++a)
+        for (int b = a; b < 3; ++b) {
+            double h = 0;
+            for (int d = 0; d < R; ++d)
+                if (d < dim) h = rn_add(h, rn_mul(rn_mul(Jl[3 * d + a], ww), Jl[3 * d + b]));
+            A[sym3(a, b)] = h;
+        }
+}
+// Jp' W Jp (6 x 6, packed upper triangle, sym6)
+template <int R>
+OVS_BA_HD void edge_hpp(const double* Jp, double ww, int dim, double* C) {
+    for (int a = 0; a < 6; ++a)
+        for (int b = a; b < 6; ++b) {
+            double h = 0;
+            for (int d = 0; d < R; ++d)
+                if (d < dim) h = rn_add(h, rn_mul(rn_mul(Jp[6 * d + a], ww), Jp[6 * d + b]));
+            C[sym6(a, b)] = h;
+        }
+}
+// -Jp' W e (6)
+template <int R>
+OVS_BA_HD void edge_bp(const double* Jp, double ww, const double* e, int dim, double* bp) {
+    for (int a = 0; a < 6; ++a) {
+        double g = 0;
+        for (int d = 0; d < R; ++d)
+            if (d < dim) g = rn_sub(g, rn_mul(rn_mul(Jp[6 * d + a], ww), e[d]));
+        bp[a] = g;
+    }
+}
+// -Jl' W e (3)
+template <int R>
+OVS_BA_HD void edge_bl(const double* Jl, double ww, const double* e, int dim, double* bl) {
+    for (int a = 0; a < 3; ++a) {
+        double g = 0;
+        for (int d = 0; d < R; ++d)
+            if (d < dim) g = rn_sub(g, rn_mul(rn_mul(Jl[3 * d + a], ww), e[d]));
+        bl[a] = g;
+    }
+}
+
 }  // namespace ovs

@@ -6,9 +6,8 @@
 // north-star tolerance is 1e-4 relative on the final reprojection error).
 //
 // Local BA, per LM iteration (state on the device, one host sync per batch of LM trials):
-//   k_ba_linearize         per observation: residual, Jacobians, robust weight -> per-edge blocks
-//                          Jl'WJl (3x3), Jp'WJp (6x6), Jp'WJl (6x3) and gradients
-//   k_ba_landmark_accum    per landmark: Hll, bl           (observations are grouped by landmark)
+//   k_ba_linearize         per observation: residual, Jacobians, robust weight -> one edge record {Jp, Jl, ww, e};
+//                          per landmark: Hll, bl           (observations are grouped by landmark)
 //   k_ba_pose_accum_chunk  per free keyframe: Hpp, bp      (two-stage deterministic reduction over its edge
 //   / _final               list)
 //  per batch of up to 4 speculative LM trials (damping values lambda, 2 lambda, 8 lambda, 64 lambda):
@@ -169,127 +168,119 @@ struct BaDev {
 };
 
 // --------------------------------------------------------------------------- linearisation
-// One thread per observation.  The per-edge blocks are written edge-major (the layout the gathers of the Schur stage want),
-// which makes a thread's own stores 144 / 168 / 48 bytes apart from its neighbour's: they are staged in shared memory in the
-// same layout and leave the block as contiguous 16-byte stores (two phases, 30 KB).  Edges outside the graph (outliers of the
-// first round) and the pose blocks of edges on fixed keyframes are written as zeros; no consumer reads them.
-__global__ void __launch_bounds__(128) k_ba_linearize(BaDev P, const LmCtl* __restrict__ ctl, double* __restrict__ Hpl, double* __restrict__ Cpp,
-                                                       double* __restrict__ bpo, double* __restrict__ All, double* __restrict__ blo) {
-    if (!ctl->active) return;
-    __shared__ __align__(16) double sm[128 * 30];
+// Edge record: what the normal equations of an edge are made of, {Jp (R x 6), Jl (R x 3), ww, e (R)}, padded to an even
+// number of doubles (16-byte aligned records).  R = 2 for a problem without stereo edges, 3 otherwise (chosen in prepare).
+// The per-edge blocks Jp'WJl, Jl'WJl, Jp'WJp and the gradients are formed from it where they are read (ba_math.cuh,
+// edge_*): storing the products costs far more memory traffic than forming them again.  Jp, Jl and ww come first, so the
+// gathers that only need Jp'WJl read a prefix of the record.
+template <int R> struct EdgeRec {
+    static constexpr int kJl = 6 * R, kWw = 9 * R, kE = 9 * R + 1;
+    static constexpr int kSize = (10 * R + 2) / 2 * 2;     // doubles per record: 22 (R = 2), 32 (R = 3)
+    static constexpr int kHpl2 = (9 * R + 2) / 2;          // double2 loads covering Jp, Jl, ww
+    static constexpr int kTail0 = 9 * R / 2, kTail1 = (10 * R + 2) / 2;   // double2 loads [kTail0, kTail1) cover ww and e
+};
+// landmark block table of k_ba_linearize (k_ba_landmark_blocks): segments of kLbSegEdges edges, up to kLbSegCap blocks each
+constexpr int kLbSegEdges = 2048, kLbSegCap = 2 * (kLbSegEdges / 128) + 2, kLbThreads = 256;
+// rows of edge i: 3 for a stereo observation of a 3-row problem
+template <int R> __device__ __forceinline__ int edge_dim(const BaDev& P, size_t i) { return R == 3 && P.obs_xr[i] >= 0.0f ? 3 : 2; }
+
+// One block per entry of the landmark block table ({first landmark, end landmark, first edge, end edge}: consecutive
+// landmarks with at most 128 edges in all, k_ba_landmark_blocks; grid = segments x kLbSegCap), one thread per edge.  A thread evaluates its edge and
+// stores the record; the records are staged in shared memory and leave the block as contiguous 16-byte stores.  Edges
+// outside the graph (outliers of the first round) store zeros, edges on fixed keyframes a zero Jp; no consumer reads them.
+// The landmark blocks Hll, bl are summed here too, one thread per landmark, sequentially in edge order from 0.0 over the
+// per-edge Jl'WJl / bl parked in shared memory.  A landmark with more than 128 edges has a block of its own and walks its
+// edges in passes of 128, its thread carrying the sums.
+template <int R>
+__global__ void __launch_bounds__(128) k_ba_linearize(BaDev P, const LmCtl* __restrict__ ctl, const int* __restrict__ nblocks,
+                                                       const int4* __restrict__ lblocks, double* __restrict__ rec,
+                                                       double* __restrict__ Hll, double* __restrict__ bl, double* __restrict__ maxdiag) {
+    using ER = EdgeRec<R>;
+    constexpr int RS = ER::kSize;
+    __shared__ __align__(16) double s_rec[128 * RS];
+    __shared__ double s_hll[128 * 6], s_bl[128 * 3];
+    __shared__ unsigned char s_live[128];
+    if (!ctl->active || (int)(blockIdx.x % kLbSegCap) >= nblocks[blockIdx.x / kLbSegCap]) return;
     P.poses = P.poses_ring + (size_t)ctl->cur * 12 * P.K; P.points = P.points_ring + (size_t)ctl->cur * 3 * P.L;
     P.use_huber = ctl->use_huber;
-    const int base = blockIdx.x * 128, t = threadIdx.x;
-    const int i = base + t;
-    const int nedge = min(128, P.M - base);
-    const bool live = i < P.M && !P.level[i];
-    int dim = 0, fi = -1;
-    double e[3] = {0, 0, 0}, Jp[18], Jl[9], ww = 0;
+    const int4 blk = lblocks[blockIdx.x];
+    const int t = threadIdx.x;
+    double H[6] = {0, 0, 0, 0, 0, 0}, b[3] = {0, 0, 0}, md = 0;
+    for (int base = blk.z; base < blk.w; base += 128) {
+        const int i = base + t;
+        const int nedge = min(128, blk.w - base);
+        const bool live = i < blk.w && !P.level[i];
+        int dim = 0, fi = -1;
+        double e[3] = {0, 0, 0}, Jp[18], Jl[9], ww = 0;
 #pragma unroll
-    for (int k = 0; k < 18; ++k) Jp[k] = 0;
+        for (int k = 0; k < 18; ++k) Jp[k] = 0;
 #pragma unroll
-    for (int k = 0; k < 9; ++k) Jl[k] = 0;
-    if (live) {
-        const int kf = P.obs_kf[i], lm = P.obs_lm[i];
-        fi = P.free_idx[kf];
-        const float xr = P.obs_xr ? P.obs_xr[i] : -1.0f;
-        const bool stereo = xr >= 0.0f;
-        const float2 xy = P.obs_xy[i];
-        const double obs[3] = {(double)xy.x, (double)xy.y, (double)xr};
-        double pose[12], pw[3];
+        for (int k = 0; k < 9; ++k) Jl[k] = 0;
+        if (live) {
+            const int kf = P.obs_kf[i], lm = P.obs_lm[i];
+            fi = P.free_idx[kf];
+            const float xr = P.obs_xr ? P.obs_xr[i] : -1.0f;
+            const bool stereo = xr >= 0.0f;
+            const float2 xy = P.obs_xy[i];
+            const double obs[3] = {(double)xy.x, (double)xy.y, (double)xr};
+            double pose[12], pw[3];
 #pragma unroll
-        for (int k = 0; k < 12; ++k) pose[k] = P.poses[12 * (size_t)kf + k];
+            for (int k = 0; k < 12; ++k) pose[k] = P.poses[12 * (size_t)kf + k];
 #pragma unroll
-        for (int k = 0; k < 3; ++k) pw[k] = P.points[3 * (size_t)lm + k];
-        dim = ovs::edge_eval(P.cam, pose, pw, obs, stereo, e, Jp, Jl);
-        const double w = (double)P.inv_sigma_sq[i];
-        double chi = 0;
-        for (int d = 0; d < dim; ++d) chi += w * e[d] * e[d];
-        double rho0 = chi, rho1 = 1.0;
-        if (P.use_huber) ovs::huber(chi, P.delta, &rho0, &rho1);
-        ww = rho1 * w;
-    }
-    // ---- phase 1: Hpl (18) | bp (6) | Jl'WJl (6), each region edge-major like its global array
-    double* sW = sm; double* sbp = sm + 128 * 18; double* sA = sbp + 128 * 6;
-    {
-        double* A = sA + 6 * t;
-        for (int a = 0; a < 3; ++a)
-            for (int b = a; b < 3; ++b) {
-                double h = 0;
-                for (int d = 0; d < dim; ++d) h += Jl[3 * d + a] * ww * Jl[3 * d + b];
-                A[ovs::sym3(a, b)] = h;
+            for (int k = 0; k < 3; ++k) pw[k] = P.points[3 * (size_t)lm + k];
+            dim = ovs::edge_eval(P.cam, pose, pw, obs, stereo, e, Jp, Jl);
+            const double w = (double)P.inv_sigma_sq[i];
+            double chi = 0;
+            for (int d = 0; d < dim; ++d) chi += w * e[d] * e[d];
+            double rho0 = chi, rho1 = 1.0;
+            if (P.use_huber) ovs::huber(chi, P.delta, &rho0, &rho1);
+            ww = rho1 * w;
+        }
+        {
+            double* r = s_rec + RS * t;
+            const bool fr = fi >= 0;
+#pragma unroll
+            for (int k = 0; k < 6 * R; ++k) r[k] = fr ? Jp[k] : 0.0;
+#pragma unroll
+            for (int k = 0; k < 3 * R; ++k) r[ER::kJl + k] = Jl[k];
+            r[ER::kWw] = ww;
+#pragma unroll
+            for (int k = 0; k < R; ++k) r[ER::kE + k] = e[k];
+#pragma unroll
+            for (int k = ER::kE + R; k < RS; ++k) r[k] = 0.0;
+            ovs::edge_hll<R>(Jl, ww, dim, s_hll + 6 * t);
+            ovs::edge_bl<R>(Jl, ww, e, dim, s_bl + 3 * t);
+            s_live[t] = live ? 1 : 0;
+        }
+        __syncthreads();
+        {
+            const double2* s2 = reinterpret_cast<const double2*>(s_rec); double2* g2 = reinterpret_cast<double2*>(rec + RS * (size_t)base);
+            for (int q = t; q < (RS / 2) * nedge; q += 128) g2[q] = s2[q];
+        }
+        for (int l = blk.x + t; l < blk.y; l += 128) {     // several passes only for a block of one landmark (thread 0)
+            const int p0 = max(P.lm_first[l], base), p1 = min(P.lm_first[l + 1], base + nedge);
+            if (blk.y - blk.x > 1) {
+#pragma unroll
+                for (int k = 0; k < 6; ++k) H[k] = 0;
+#pragma unroll
+                for (int k = 0; k < 3; ++k) b[k] = 0;
             }
-        double* W = sW + 18 * t; double* bp = sbp + 6 * t;
-        const bool fr = fi >= 0;
-        for (int a = 0; a < 6; ++a) {
-            double g = 0;
-            for (int d = 0; d < dim; ++d) g -= Jp[6 * d + a] * ww * e[d];
-            bp[a] = fr ? g : 0.0;
-            for (int b = 0; b < 3; ++b) {
-                double h = 0;
-                for (int d = 0; d < dim; ++d) h += Jp[6 * d + a] * ww * Jl[3 * d + b];
-                W[3 * a + b] = fr ? h : 0.0;
+            for (int p = p0; p < p1; ++p) {
+                if (!s_live[p - base]) continue;
+#pragma unroll
+                for (int k = 0; k < 6; ++k) H[k] += s_hll[6 * (p - base) + k];
+#pragma unroll
+                for (int k = 0; k < 3; ++k) b[k] += s_bl[3 * (p - base) + k];
+            }
+            if (base + 128 >= blk.w) {                   // the landmark's last pass
+#pragma unroll
+                for (int k = 0; k < 6; ++k) Hll[6 * (size_t)l + k] = H[k];
+#pragma unroll
+                for (int k = 0; k < 3; ++k) bl[3 * (size_t)l + k] = b[k];
+                md = fmax(md, fmax(fabs(H[0]), fmax(fabs(H[3]), fabs(H[5]))));
             }
         }
-    }
-    __syncthreads();
-    {
-        const double2* s2 = reinterpret_cast<const double2*>(sW); double2* g2 = reinterpret_cast<double2*>(Hpl + 18 * (size_t)base);
-        for (int q = t; q < 9 * nedge; q += 128) g2[q] = s2[q];
-        s2 = reinterpret_cast<const double2*>(sbp); g2 = reinterpret_cast<double2*>(bpo + 6 * (size_t)base);
-        for (int q = t; q < 3 * nedge; q += 128) g2[q] = s2[q];
-        s2 = reinterpret_cast<const double2*>(sA); g2 = reinterpret_cast<double2*>(All + 6 * (size_t)base);
-        for (int q = t; q < 3 * nedge; q += 128) g2[q] = s2[q];
-    }
-    __syncthreads();
-    // ---- phase 2: Jp'WJp (21) | bl (3)
-    double* sC = sm; double* sbl = sm + 128 * 21;
-    {
-        double* C = sC + 21 * t; double* bl = sbl + 3 * t;
-        const bool fr = fi >= 0;
-        for (int a = 0; a < 6; ++a)
-            for (int b = a; b < 6; ++b) {
-                double h = 0;
-                for (int d = 0; d < dim; ++d) h += Jp[6 * d + a] * ww * Jp[6 * d + b];
-                C[ovs::sym6(a, b)] = fr ? h : 0.0;
-            }
-        for (int a = 0; a < 3; ++a) {
-            double g = 0;
-            for (int d = 0; d < dim; ++d) g -= Jl[3 * d + a] * ww * e[d];
-            bl[a] = g;
-        }
-    }
-    __syncthreads();
-    {
-        // 21 doubles per edge: the block's region starts 16-byte aligned only for even `base * 21` -- base is a multiple of 128
-        const double2* s2 = reinterpret_cast<const double2*>(sC); double2* g2 = reinterpret_cast<double2*>(Cpp + 21 * (size_t)base);
-        const int nd = 21 * nedge;
-        for (int q = t; q < nd / 2; q += 128) g2[q] = s2[q];
-        if ((nd & 1) && t == 0) Cpp[21 * (size_t)base + nd - 1] = sC[nd - 1];
-        const int nb = 3 * nedge;
-        for (int q = t; q < nb; q += 128) blo[3 * (size_t)base + q] = sbl[q];
-    }
-}
-
-__global__ void __launch_bounds__(128) k_ba_landmark_accum(BaDev P, const LmCtl* __restrict__ ctl, const double* __restrict__ All, const double* __restrict__ blo,
-                                                            double* __restrict__ Hll, double* __restrict__ bl, double* __restrict__ maxdiag) {
-    if (!ctl->active) return;
-    const int l = blockIdx.x * 128 + threadIdx.x;
-    double md = 0;
-    if (l < P.L) {
-        double H[6] = {0, 0, 0, 0, 0, 0}, b[3] = {0, 0, 0};
-        for (int p = P.lm_first[l]; p < P.lm_first[l + 1]; ++p) {
-            if (P.level[p]) continue;
-#pragma unroll
-            for (int k = 0; k < 6; ++k) H[k] += All[6 * (size_t)p + k];
-#pragma unroll
-            for (int k = 0; k < 3; ++k) b[k] += blo[3 * (size_t)p + k];
-        }
-#pragma unroll
-        for (int k = 0; k < 6; ++k) Hll[6 * (size_t)l + k] = H[k];
-#pragma unroll
-        for (int k = 0; k < 3; ++k) bl[3 * (size_t)l + k] = b[k];
-        md = fmax(fabs(H[0]), fmax(fabs(H[3]), fabs(H[5])));
+        __syncthreads();
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) md = fmax(md, __shfl_xor_sync(0xffffffffu, md, o));
@@ -298,12 +289,14 @@ __global__ void __launch_bounds__(128) k_ba_landmark_accum(BaDev P, const LmCtl*
 
 // Hpp / bp of the free keyframes: two-stage deterministic reduction over the (a, a) co-observation
 // segment of each keyframe (its edge list), cut into chunks of 128 edges (one edge per thread) so the
-// dependent-load latency of a chunk overlaps with that of many others.
+// dependent-load latency of a chunk overlaps with that of many others.  Each thread forms its edge's
+// Jp'WJp and -Jp'We from the record (Jp, ww, e).
 // chunk = {keyframe a, begin, end, unused}; ppart[chunk][27] = {Hpp packed 21, bp 6}.
+template <int R>
 __global__ void __launch_bounds__(128) k_ba_pose_accum_chunk(BaDev P, const LmCtl* __restrict__ ctl, const int* __restrict__ nchunks,
                                                               const int4* __restrict__ pair_rec, const int4* __restrict__ chunks,
-                                                              const double* __restrict__ Cpp, const double* __restrict__ bpo,
-                                                              double* __restrict__ ppart) {
+                                                              const double* __restrict__ rec, double* __restrict__ ppart) {
+    using ER = EdgeRec<R>;
     __shared__ double red[27][4];
     if (!ctl->active || (int)blockIdx.x >= *nchunks) return;
     const int4 ch = chunks[blockIdx.x];
@@ -312,13 +305,18 @@ __global__ void __launch_bounds__(128) k_ba_pose_accum_chunk(BaDev P, const LmCt
 #pragma unroll
     for (int k = 0; k < 27; ++k) acc[k] = 0;
     if (e < ch.z) {
-        const int4 rec = pair_rec[e];           // diagonal pair: both edges are this keyframe's edge
-        const int o = rec.x;
-        if (!rec.w) {
+        const int4 pr = pair_rec[e];           // diagonal pair: both edges are this keyframe's edge
+        const int o = pr.x;
+        if (!pr.w) {
+            const double2* r2 = reinterpret_cast<const double2*>(rec + ER::kSize * (size_t)o);
+            double r[2 * ER::kTail1];
 #pragma unroll
-            for (int k = 0; k < 21; ++k) acc[k] = Cpp[21 * (size_t)o + k];
+            for (int k = 0; k < 3 * R; ++k) { const double2 v = r2[k]; r[2 * k] = v.x; r[2 * k + 1] = v.y; }
 #pragma unroll
-            for (int k = 0; k < 6; ++k) acc[21 + k] = bpo[6 * (size_t)o + k];
+            for (int k = ER::kTail0; k < ER::kTail1; ++k) { const double2 v = r2[k]; r[2 * k] = v.x; r[2 * k + 1] = v.y; }
+            const int dim = edge_dim<R>(P, o);
+            ovs::edge_hpp<R>(r, r[ER::kWw], dim, acc);
+            ovs::edge_bp<R>(r, r[ER::kWw], r + ER::kE, dim, acc + 21);
         }
     }
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -371,11 +369,13 @@ __device__ __forceinline__ void dmma_m8n8k4(double& d0, double& d1, double a, do
 // A record-per-lane layout costs 3-4 wavefronts per fragment load.  41 KB per block: the solver's clusters need SMs with free
 // shared memory while eight streams share the GPU, a larger footprint here costs more there than it saves.
 constexpr int kSGY = 76, kSGW = 84;
+template <int R>
 __global__ void __launch_bounds__(128, 4) k_ba_schur_chunk(BaDev P, const LmCtl* __restrict__ ctl, const int* __restrict__ nchunks,
                                                          const int4* __restrict__ pair_rec, const int4* __restrict__ chunks,
                                                          const int2* __restrict__ pair_ab, const double* __restrict__ Hll,
-                                                         const double* __restrict__ Hpl, const double* __restrict__ bl,
+                                                         const double* __restrict__ rec, const double* __restrict__ bl,
                                                          double* __restrict__ spart, size_t spart_stride) {
+    using ER = EdgeRec<R>;
     // The Jacobian blocks Hpl_a, Hpl_b of a co-observation do not depend on lambda: they are loaded once
     // and all `nbatch` speculative damping values are processed by the same block (only (Hll + lambda I)^-1
     // differs).  per warp: 32 co-observations x {Y (6x3), W = Hpl_b (6x3) + bl (3)}
@@ -394,37 +394,58 @@ __global__ void __launch_bounds__(128, 4) k_ba_schur_chunk(BaDev P, const LmCtl*
     double wa[18], hl[6] = {0, 0, 0, 0, 0, 0};
     int lm = -1;
     {
-        double wb[18], gl[3] = {0, 0, 0};
+        // Hpl_a, Hpl_b are formed from the prefix {Jp, Jl, ww} of the two edge records; Hpl_b goes to shared memory element by
+        // element as it is formed, Hpl_a stays in registers.  Two-row records: all loads are issued first.  Three-row records
+        // do not fit in registers together with the rest: record b is loaded into the registers of record a, which is loaded
+        // once Hpl_b is parked.
+        constexpr bool kLoadAFirst = R == 2;
+        double gl[3] = {0, 0, 0}, ra[2 * ER::kHpl2], rb2[2 * ER::kHpl2];
+        double (&rb)[2 * ER::kHpl2] = kLoadAFirst ? rb2 : ra;
+        const double2* pa = nullptr;
+        bool live = false, same = true;
+        int da = 2, db = 2;
+        auto load_rec = [](const double2* p, double (&r)[2 * ER::kHpl2]) {
 #pragma unroll
-        for (int k = 0; k < 18; ++k) { wa[k] = 0; wb[k] = 0; }
+            for (int k = 0; k < ER::kHpl2; ++k) { const double2 v = p[k]; r[2 * k] = v.x; r[2 * k + 1] = v.y; }
+        };
+#pragma unroll
+        for (int k = 0; k < 18; ++k) wa[k] = 0;
         if (e < ch.z) {
             const int4 ob = pair_rec[e];      // {edge on a, edge on b, landmark, either edge excluded}
             if (!ob.w) {
+                live = true;
                 lm = ob.z;
-                const double2* pa = reinterpret_cast<const double2*>(Hpl + 18 * (size_t)ob.x);
-                const double2* pb = reinterpret_cast<const double2*>(Hpl + 18 * (size_t)ob.y);
-#pragma unroll
-                for (int k = 0; k < 9; ++k) { const double2 v = pa[k]; wa[2 * k] = v.x; wa[2 * k + 1] = v.y; }
-                if (ob.x == ob.y) {              // the records of a diagonal pair name the same edge twice (uniform over such a chunk)
-#pragma unroll
-                    for (int k = 0; k < 18; ++k) wb[k] = wa[k];
-                } else {
-#pragma unroll
-                    for (int k = 0; k < 9; ++k) { const double2 v = pb[k]; wb[2 * k] = v.x; wb[2 * k + 1] = v.y; }
-                }
+                same = ob.x == ob.y;             // the records of a diagonal pair name the same edge twice (uniform over such a chunk)
+                pa = reinterpret_cast<const double2*>(rec + ER::kSize * (size_t)ob.x);
+                if (kLoadAFirst || same) load_rec(pa, ra);
+                if (!same) load_rec(reinterpret_cast<const double2*>(rec + ER::kSize * (size_t)ob.y), rb);
                 const double2* ph = reinterpret_cast<const double2*>(Hll + 6 * (size_t)lm);
 #pragma unroll
                 for (int k = 0; k < 3; ++k) { const double2 v = ph[k]; hl[2 * k] = v.x; hl[2 * k + 1] = v.y; }
                 if (diag) { gl[0] = bl[3 * (size_t)lm]; gl[1] = bl[3 * (size_t)lm + 1]; gl[2] = bl[3 * (size_t)lm + 2]; }
+                da = edge_dim<R>(P, ob.x); db = edge_dim<R>(P, ob.y);
             }
         }
         // B operand: element (column c, K slot 3 en + kc) = Hpl_b[c][kc] (c < 6), bl[kc] (c = 6); column 7 is never read
+        int sb[3];
 #pragma unroll
-        for (int kc = 0; kc < 3; ++kc) {
-            const int kk = 3 * (lane & 3) + kc, base = (lane >> 2) * kSGW + (kk >> 2) * 28 + (kk & 3);
+        for (int kc = 0; kc < 3; ++kc) { const int kk = 3 * (lane & 3) + kc; sb[kc] = (lane >> 2) * kSGW + (kk >> 2) * 28 + (kk & 3); }
+        auto park = [&](int c, int kc, double v) { sWw[sb[kc] + 4 * c] = v; };
+        if (!live) {
 #pragma unroll
-            for (int c = 0; c < 6; ++c) sWw[base + 4 * c] = wb[3 * c + kc];
-            sWw[base + 24] = gl[kc];
+            for (int c = 0; c < 6; ++c)
+#pragma unroll
+                for (int kc = 0; kc < 3; ++kc) park(c, kc, 0.0);
+        } else if (same) {
+            ovs::edge_hpl_each<R>(ra, ra + ER::kJl, ra[ER::kWw], da, park);
+        } else {
+            ovs::edge_hpl_each<R>(rb, rb + ER::kJl, rb[ER::kWw], db, park);
+        }
+#pragma unroll
+        for (int kc = 0; kc < 3; ++kc) sWw[sb[kc] + 24] = gl[kc];
+        if (live) {
+            if (!kLoadAFirst && !same) load_rec(pa, ra);
+            ovs::edge_hpl<R>(ra, ra + ER::kJl, ra[ER::kWw], da, wa);
         }
     }
     // (Hll + lambda I)^-1 of this lane's landmark for damping value bt (zeros for an inactive lane or a singular block: the
@@ -1161,7 +1182,8 @@ __global__ void __launch_bounds__(512) k_chol_big_backsolve(const LmCtl* __restr
 // Also the LM scale term sum x (lambda x + b), one partial per block and damping value.
 // All damping values of the batch are handled by the same thread: the Jacobian blocks and the edge indices of a landmark
 // are read once, only x, (Hll + lambda I)^-1 and the candidate slot differ.
-__global__ void __launch_bounds__(128) k_ba_update(BaDev P, const LmCtl* __restrict__ ctl, const double* __restrict__ Hpl, const double* __restrict__ Hll,
+template <int R>
+__global__ void __launch_bounds__(128) k_ba_update(BaDev P, const LmCtl* __restrict__ ctl, const double* __restrict__ rec, const double* __restrict__ Hll,
                                                     const double* __restrict__ bl, const double* __restrict__ bp, const double* __restrict__ x,
                                                     double* poses_ring, double* points_ring,
                                                     double* __restrict__ partial_scale, int* __restrict__ fail) {
@@ -1185,10 +1207,12 @@ __global__ void __launch_bounds__(128) k_ba_update(BaDev P, const LmCtl* __restr
         for (int p = P.lm_first[l]; p < P.lm_first[l + 1]; ++p) {
             const int fi = P.free_idx[P.obs_kf[p]];
             if (P.level[p] || fi < 0) continue;
-            double W[18];
-            const double2* pw = reinterpret_cast<const double2*>(Hpl + 18 * (size_t)p);
+            using ER = EdgeRec<R>;
+            double W[18], er[2 * ER::kHpl2];
+            const double2* pw = reinterpret_cast<const double2*>(rec + ER::kSize * (size_t)p);
 #pragma unroll
-            for (int k = 0; k < 9; ++k) { const double2 v = pw[k]; W[2 * k] = v.x; W[2 * k + 1] = v.y; }
+            for (int k = 0; k < ER::kHpl2; ++k) { const double2 v = pw[k]; er[2 * k] = v.x; er[2 * k + 1] = v.y; }
+            ovs::edge_hpl<R>(er, er + ER::kJl, er[ER::kWw], edge_dim<R>(P, p), W);
 #pragma unroll
             for (int bt = 0; bt < kSpec; ++bt) {
                 if (bt < nbatch) {
@@ -1509,7 +1533,7 @@ __global__ void __launch_bounds__(1024) k_ba_pose_final_plan(LmCtl* ctl, int nfr
     if (threadIdx.x != 0) return;
     if (halted) return;             // halted: the parked batch and the Hessian of the undecided iteration must survive
     for (int w = 0; w < 32; ++w) md = fmax(md, smax[w]);
-    md = fmax(md, maxdiag[0]);      // the landmark blocks' share (k_ba_landmark_accum)
+    md = fmax(md, maxdiag[0]);      // the landmark blocks' share (k_ba_linearize)
     maxdiag[0] = 0; maxdiag[1] = 0;
     lm_plan_iteration(ctl, 1e-5 * md, stop_word, fail, mirror);
 }
@@ -1587,9 +1611,10 @@ __global__ void __launch_bounds__(1024) k_ba_free_index(int K, const unsigned ch
 }
 
 __global__ void __launch_bounds__(256) k_ba_landmark_index(int M, int L, int K, const int* __restrict__ obs_kf, const int* __restrict__ obs_lm,
-                                                            int* __restrict__ lm_first, long long* counts) {
+                                                            const float* __restrict__ obs_xr, int* __restrict__ lm_first, long long* counts) {
     const int i = blockIdx.x * 256 + threadIdx.x;
     if (i >= M) return;
+    if (obs_xr[i] >= 0.0f) counts[5] = 1;          // a stereo edge: the edge records have 3 rows
     const int l = obs_lm[i], k = obs_kf[i];
     int err = 0;
     if (l < 0 || l >= L || k < 0 || k >= K) err = 1;
@@ -1604,6 +1629,63 @@ __global__ void __launch_bounds__(256) k_ba_landmark_index(int M, int L, int K, 
         for (int q = max(lp, -1) + 1; q <= l; ++q) lm_first[q] = i;      // landmarks without observations start where the next one does
     if (i == M - 1)
         for (int q = l + 1; q <= L; ++q) lm_first[q] = M;
+}
+
+// Landmark block table of k_ba_linearize: consecutive landmarks with at most 128 edges in all; a landmark with more than 128 edges
+// gets a block of its own.  Entry = {first landmark, end landmark, first edge, end edge}.  The landmarks are split into segments
+// by where their edges start (segment k: lm_first in [kLbSegEdges k, kLbSegEdges (k + 1))), and each segment is cut greedily in
+// landmark order by one CTA, independently of the others; its entries go to blocks[k * kLbSegCap ..], their number to nblocks[k].
+// Two consecutive blocks hold more than 128 edges together and all but the last block of a segment lie inside its edge window,
+// so a segment has at most 2 (kLbSegEdges - 1) / 129 + 2 <= kLbSegCap blocks.
+// Per CTA: lm_first is staged in shared memory kLbThreads landmarks at a time, warp 0 cuts it 32 landmarks per step (the first
+// landmark that does not fit is found by a ballot).
+__device__ __forceinline__ int lower_bound_first(const int* __restrict__ lm_first, int L, int v) {
+    int lo = 0, hi = L;                                 // first landmark l with lm_first[l] >= v (L if none)
+    while (lo < hi) { const int mid = (lo + hi) >> 1; if (lm_first[mid] < v) lo = mid + 1; else hi = mid; }
+    return lo;
+}
+__global__ void __launch_bounds__(kLbThreads) k_ba_landmark_blocks(int L, const int* __restrict__ lm_first, int4* __restrict__ blocks, int* __restrict__ nblocks) {
+    __shared__ int s_first[kLbThreads + 1];
+    __shared__ int s_range[2];
+    const int lane = threadIdx.x & 31, seg = blockIdx.x;
+    if (threadIdx.x < 2) s_range[threadIdx.x] = lower_bound_first(lm_first, L, (seg + (int)threadIdx.x) * kLbSegEdges);
+    __syncthreads();
+    const int l0 = s_range[0], l1 = (seg + 1 == (int)gridDim.x) ? L : s_range[1];
+    blocks += (size_t)seg * kLbSegCap;
+    int start = l0, s = l0 < L ? lm_first[l0] : 0, nb = 0;   // warp 0: first landmark and first edge of the open block, blocks emitted
+    for (int c0 = l0; c0 < l1; c0 += kLbThreads) {
+        __syncthreads();
+        for (int q = threadIdx.x; q <= kLbThreads; q += kLbThreads)
+            if (c0 + q <= l1) s_first[q] = lm_first[c0 + q];
+        __syncthreads();
+        if (threadIdx.x >= 32) continue;
+        const int cn = min(kLbThreads, l1 - c0);
+        for (int g = 0; g < cn; g += 32) {
+            const int j = g + lane;
+            const bool in = j < cn;
+            const int eb = in ? s_first[j] : 0, ee = in ? s_first[j + 1] : 0;
+            int cur = c0 + g;                           // first landmark of this step not placed yet
+            for (;;) {
+                const unsigned over = __ballot_sync(0xffffffffu, in && c0 + j >= cur && ee - s > 128);
+                if (!over) break;
+                const int f = __ffs(over) - 1, lf = c0 + g + f;
+                const int bf = __shfl_sync(0xffffffffu, eb, f), ef = __shfl_sync(0xffffffffu, ee, f);
+                if (lf == start) {                      // alone and still more than 128 edges: a block of its own
+                    if (lane == 0) blocks[nb] = make_int4(start, lf + 1, s, ef);
+                    start = lf + 1; s = ef;
+                } else {
+                    if (lane == 0) blocks[nb] = make_int4(start, lf, s, bf);
+                    start = lf; s = bf;
+                }
+                cur = start;
+                ++nb;
+            }
+        }
+    }
+    if (threadIdx.x == 0) {
+        if (start < l1) blocks[nb++] = make_int4(start, l1, s, lm_first[l1]);
+        nblocks[seg] = nb;
+    }
 }
 
 // observations on free keyframes per landmark (one thread per landmark: the dependent index loads of 20 k landmarks overlap),
@@ -3049,7 +3131,9 @@ struct ovs_ba_plan {
     uint8_t* dout = nullptr;
     LmCtl* dctl = nullptr; int* dexec = nullptr;
     size_t spart_stride = 0, S_stride = 0, invL_stride = 0;
-    double *dHpl = nullptr, *dCpp = nullptr, *dbpo = nullptr, *dAll = nullptr, *dblo = nullptr;
+    int rows = 2;                                               // rows of the edge records: 3 if any edge is stereo
+    double* drec = nullptr;                                     // M edge records (EdgeRec<rows>)
+    int4* dlblocks = nullptr; int* dnlblocks = nullptr; int nlseg = 0;   // landmark block table of the linearisation (per segment)
     double *dHll = nullptr, *dbl = nullptr, *dHpp = nullptr, *dbp = nullptr;
     double *dS = nullptr, *dbS = nullptr, *dx = nullptr, *dinvL = nullptr;
     int4* d_pair_rec = nullptr; int *dsegb = nullptr, *dsege = nullptr; int2* dpab = nullptr; int* ddiag = nullptr;
@@ -3112,6 +3196,7 @@ int prepare_impl(ovs_optimizer* h, const ovs_camera* cam, int setup_is_mono, int
     const size_t sM = (size_t)M, sL = (size_t)L, sK = (size_t)K;
     const int nb_obs = (M + 127) / 128, nb_upd = (L + K + 127) / 128;
     const int exec_cap = 1024;
+    const int nlseg = M / kLbSegEdges + 1;           // k_ba_landmark_blocks: segments of the landmark block table
     double* hposes; double* hpoints; int *hkf, *hlm; float *hxy, *hxr, *hw; uint8_t* hfixed; uint8_t* hout; long long* hcounts;
     double* dposes_in; double* dpoints_in; int *dkf, *dlm; float *dxy, *dxr, *dw; uint8_t* dfixed;
     int *dfree, *dlmf, *dpoff; long long* dcounts;
@@ -3130,8 +3215,7 @@ int prepare_impl(ovs_optimizer* h, const ovs_camera* cam, int setup_is_mono, int
         pl.dout = D.take<uint8_t>(sM); pl.dctl = D.take<LmCtl>(1); pl.dexec = D.take<int>(exec_cap);
         pl.dposes_ring = D.take<double>((kSpec + 1) * 12 * sK); pl.dpoints_ring = D.take<double>((kSpec + 1) * 3 * sL);
         pl.dlevel = D.take<uint8_t>(sM); pl.derr = D.take<double>(kSpec * 3 * sM);
-        pl.dHpl = D.take<double>(18 * sM); pl.dCpp = D.take<double>(21 * sM); pl.dbpo = D.take<double>(6 * sM);
-        pl.dAll = D.take<double>(6 * sM); pl.dblo = D.take<double>(3 * sM);
+        pl.dlblocks = D.take<int4>((size_t)nlseg * kLbSegCap); pl.dnlblocks = D.take<int>(nlseg);
         pl.dHll = D.take<double>(6 * sL); pl.dbl = D.take<double>(3 * sL);
         pl.dpchi = D.take<double>(kSpec * (size_t)nb_obs); pl.dpscale = D.take<double>(kSpec * (size_t)nb_upd);
         pl.dfail = D.take<int>(kSpec); pl.dmaxdiag = D.take<double>(2); pl.dclk = D.take<long long>(192); pl.dnchunks = D.take<int>(2);
@@ -3162,17 +3246,17 @@ int prepare_impl(ovs_optimizer* h, const ovs_camera* cam, int setup_is_mono, int
         OVS_CUDA_CHECK(cudaMemcpyAsync(dfixed, in.fixed, sK, dd, st));
     }
     // graph bookkeeping + validation on the device, then the one read-back of prepare
-    hcounts[0] = 0; hcounts[1] = 0; hcounts[2] = 0; hcounts[3] = 0; hcounts[4] = 0x7fffffffffffffffll;
-    OVS_CUDA_CHECK(cudaMemcpyAsync(dcounts, hcounts, 5 * sizeof(long long), cudaMemcpyHostToDevice, st));
+    hcounts[0] = 0; hcounts[1] = 0; hcounts[2] = 0; hcounts[3] = 0; hcounts[4] = 0x7fffffffffffffffll; hcounts[5] = 0;
+    OVS_CUDA_CHECK(cudaMemcpyAsync(dcounts, hcounts, 6 * sizeof(long long), cudaMemcpyHostToDevice, st));
     k_ba_free_index<<<1, 1024, 0, st>>>(K, dfixed, dfree, dcounts);
     OVS_LAUNCH_CHECK();
-    k_ba_landmark_index<<<(M + 255) / 256, 256, 0, st>>>(M, L, K, dkf, dlm, dlmf, dcounts);
+    k_ba_landmark_index<<<(M + 255) / 256, 256, 0, st>>>(M, L, K, dkf, dlm, dxr, dlmf, dcounts);
     OVS_LAUNCH_CHECK();
     k_ba_pair_counts<<<(L + 255) / 256, 256, 0, st>>>(L, dlmf, dkf, dfree, dpoff, dcounts);
     OVS_LAUNCH_CHECK();
     k_ba_pair_offsets<<<1, 1024, 0, st>>>(L, dpoff, dcounts);
     OVS_LAUNCH_CHECK();
-    OVS_CUDA_CHECK(cudaMemcpyAsync(hcounts, dcounts, 5 * sizeof(long long), cudaMemcpyDeviceToHost, st));
+    OVS_CUDA_CHECK(cudaMemcpyAsync(hcounts, dcounts, 6 * sizeof(long long), cudaMemcpyDeviceToHost, st));
     OVS_CUDA_CHECK(ovs::sync_stream(st));
     if (hcounts[4] != 0x7fffffffffffffffll) {
         const long long i = hcounts[4] >> 2;
@@ -3190,6 +3274,8 @@ int prepare_impl(ovs_optimizer* h, const ovs_camera* cam, int setup_is_mono, int
     OVS_REQUIRE(n <= kMaxReducedDimBig, OVS_ERR_UNSUPPORTED, "more than %d free keyframes", kMaxReducedDimBig / 6);
     OVS_REQUIRE(npair_entries < (1ll << 30), OVS_ERR_UNSUPPORTED, "too many co-observations");
     const int npairs = nfree * (nfree + 1) / 2;
+    const int rows = hcounts[5] ? 3 : 2;
+    const size_t rec_doubles = (size_t)(rows == 3 ? EdgeRec<3>::kSize : EdgeRec<2>::kSize) * sM;
 
     // ---- phase 2: what depends on the number of free keyframes and of co-observations
     const size_t sE = (size_t)std::max<long long>(npair_entries, 1);
@@ -3197,6 +3283,7 @@ int prepare_impl(ovs_optimizer* h, const ovs_camera* cam, int setup_is_mono, int
     const size_t max_dchunks = (size_t)nfree_edges / 128 + (size_t)nfree + 8;   // the same over the diagonal pairs
     unsigned *dkeys, *dkeys2; unsigned long long *dvals, *dvals2; int4* dprec; int* dsort;
     auto carve2 = [&](Arena& W) {
+        pl.drec = W.take<double>(rec_doubles);
         pl.dpab = W.take<int2>(npairs); pl.ddiag = W.take<int>(nfree);
         pl.dHpp = W.take<double>(21 * (size_t)nfree); pl.dbp = W.take<double>(6 * (size_t)nfree);
         pl.S_stride = ((size_t)(n + 1) * n + 31) / 32 * 32; pl.invL_stride = (size_t)((n + kNB - 1) / kNB) * kNB * kNB;
@@ -3232,6 +3319,9 @@ int prepare_impl(ovs_optimizer* h, const ovs_camera* cam, int setup_is_mono, int
     const float chi_sq_2D = 5.99146f, chi_sq_3D = 7.81473f;
     P.use_huber = 1; P.delta = (double)(setup_is_mono ? sqrtf(chi_sq_2D) : sqrtf(chi_sq_3D));
 
+    k_ba_landmark_blocks<<<nlseg, kLbThreads, 0, st>>>(L, dlmf, pl.dlblocks, pl.dnlblocks);
+    OVS_LAUNCH_CHECK();
+
     // ---- co-observation lists, sorted by keyframe pair (stable: landmark order kept inside a pair), flattened to one
     //      16-byte record per co-observation; chunk tables (<= 128 co-observations per chunk) of the two-stage reductions
     k_ba_pair_table<<<nfree, 128, 0, st>>>(nfree, pl.dpab, pl.ddiag);
@@ -3260,6 +3350,7 @@ int prepare_impl(ovs_optimizer* h, const ovs_camera* cam, int setup_is_mono, int
     OVS_LAUNCH_CHECK();
 
     pl.K = K; pl.L = L; pl.M = M; pl.nfree = nfree; pl.n = n; pl.npairs = npairs; pl.nb_obs = nb_obs; pl.nb_upd = nb_upd;
+    pl.rows = rows; pl.nlseg = nlseg;
     pl.npair_entries = npair_entries;
     {
         DenseSolve ds{};
@@ -3524,7 +3615,8 @@ int run_impl(ovs_optimizer* h, int rounds, int huber_first, int num_first_iter, 
             }
             OVS_CUDA_CHECK(cudaEventRecord(h->solver_ev[4 * slot], st));
         }
-        k_ba_schur_chunk<<<pl.max_chunks, 128, 0, st>>>(P, ctl, pl.dnchunks, pl.d_pair_rec, pl.dchunks, pl.dpab, pl.dHll, pl.dHpl, pl.dbl, pl.dspart, pl.spart_stride);
+        if (pl.rows == 3) k_ba_schur_chunk<3><<<pl.max_chunks, 128, 0, st>>>(P, ctl, pl.dnchunks, pl.d_pair_rec, pl.dchunks, pl.dpab, pl.dHll, pl.drec, pl.dbl, pl.dspart, pl.spart_stride);
+        else k_ba_schur_chunk<2><<<pl.max_chunks, 128, 0, st>>>(P, ctl, pl.dnchunks, pl.d_pair_rec, pl.dchunks, pl.dpab, pl.dHll, pl.drec, pl.dbl, pl.dspart, pl.spart_stride);
         OVS_LAUNCH_CHECK();
         k_ba_schur_final<<<dim3(npairs, kSpec), 64, 0, st>>>(n, ctl, pl.dpair_chunk_begin, pl.dpab, pl.dspart, pl.spart_stride, pl.dHpp, pl.dbp, pl.dS, pl.S_stride);
         OVS_LAUNCH_CHECK();
@@ -3533,7 +3625,8 @@ int run_impl(ovs_optimizer* h, int rounds, int huber_first, int num_first_iter, 
         const int rc_solve = launch_dense_solve(h, st, ctl, ds);
         if (rc_solve != OVS_OK) return rc_solve;
         if (ev) OVS_CUDA_CHECK(cudaEventRecord(h->solver_ev[4 * slot + 3], st));
-        k_ba_update<<<nb_upd, 128, 0, st>>>(P, ctl, pl.dHpl, pl.dHll, pl.dbl, pl.dbp, pl.dx, pl.dposes_ring, pl.dpoints_ring, pl.dpscale, pl.dfail);
+        if (pl.rows == 3) k_ba_update<3><<<nb_upd, 128, 0, st>>>(P, ctl, pl.drec, pl.dHll, pl.dbl, pl.dbp, pl.dx, pl.dposes_ring, pl.dpoints_ring, pl.dpscale, pl.dfail);
+        else k_ba_update<2><<<nb_upd, 128, 0, st>>>(P, ctl, pl.drec, pl.dHll, pl.dbl, pl.dbp, pl.dx, pl.dposes_ring, pl.dpoints_ring, pl.dpscale, pl.dfail);
         OVS_LAUNCH_CHECK();
         k_ba_errors<<<dim3(nb_obs, kSpec), 128, 0, st>>>(P, ctl, 0, pl.derr, pl.dpchi);
         OVS_LAUNCH_CHECK();
@@ -3546,11 +3639,12 @@ int run_impl(ovs_optimizer* h, int rounds, int huber_first, int num_first_iter, 
 
     // the static part of one Levenberg iteration: buildSystem (linearise + accumulate), plan, the first trial batch
     auto iteration_head = [&](bool in_graph, bool halt_if_undecided) -> int {
-        k_ba_linearize<<<nb_obs, 128, 0, st>>>(P, ctl, pl.dHpl, pl.dCpp, pl.dbpo, pl.dAll, pl.dblo);
+        const unsigned nb_lin = (unsigned)(pl.nlseg * kLbSegCap);
+        if (pl.rows == 3) k_ba_linearize<3><<<nb_lin, 128, 0, st>>>(P, ctl, pl.dnlblocks, pl.dlblocks, pl.drec, pl.dHll, pl.dbl, pl.dmaxdiag);
+        else k_ba_linearize<2><<<nb_lin, 128, 0, st>>>(P, ctl, pl.dnlblocks, pl.dlblocks, pl.drec, pl.dHll, pl.dbl, pl.dmaxdiag);
         OVS_LAUNCH_CHECK();
-        k_ba_landmark_accum<<<(L + 127) / 128, 128, 0, st>>>(P, ctl, pl.dAll, pl.dblo, pl.dHll, pl.dbl, pl.dmaxdiag);
-        OVS_LAUNCH_CHECK();
-        k_ba_pose_accum_chunk<<<pl.max_dchunks, 128, 0, st>>>(P, ctl, pl.dnchunks + 1, pl.d_pair_rec, pl.ddchunks, pl.dCpp, pl.dbpo, pl.dppart);
+        if (pl.rows == 3) k_ba_pose_accum_chunk<3><<<pl.max_dchunks, 128, 0, st>>>(P, ctl, pl.dnchunks + 1, pl.d_pair_rec, pl.ddchunks, pl.drec, pl.dppart);
+        else k_ba_pose_accum_chunk<2><<<pl.max_dchunks, 128, 0, st>>>(P, ctl, pl.dnchunks + 1, pl.d_pair_rec, pl.ddchunks, pl.drec, pl.dppart);
         OVS_LAUNCH_CHECK();
         k_ba_pose_final_plan<<<1, 1024, 0, st>>>(ctl, nfree, pl.dkf_chunk_begin, pl.dppart, pl.dHpp, pl.dbp, pl.dmaxdiag, pl.dfail, stop_word, mirror);
         OVS_LAUNCH_CHECK();
