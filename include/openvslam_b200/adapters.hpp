@@ -15,6 +15,9 @@
 //     const std::vector<std::pair<int, int>>&), find_via_ransac(unsigned, bool), solution_is_valid(), get_best_E_21(),
 //     get_inlier_matches()                                                                                       (solve/essential_solver.h)
 //   match::robust::match_frame_and_keyframe(data::frame&, data::keyframe*, std::vector<data::landmark*>&)       (match/robust.h)
+//   solve::homography_solver / solve::fundamental_solver(const std::vector<cv::KeyPoint>&, const std::vector<cv::KeyPoint>&,
+//     const std::vector<std::pair<int, int>>&, float), find_via_ransac(unsigned, bool), solution_is_valid(), get_best_score(),
+//     get_best_H_21() / get_best_F_21(), get_inlier_matches()                    (solve/{homography,fundamental}_solver.h)
 //
 // Include it INSTEAD of openvslam_b200.hpp in a translation unit that can see the reference's headers (here: the stand-ins
 // under tests/cpp/standin, which declare the members used below with the names recalled in SURVEY.md section 2 / 8b;
@@ -454,5 +457,62 @@ inline Mat33_t solve::essential_solver::get_best_E_21() const {
         for (int c = 0; c < 3; ++c) E(r, c) = best_.E_21[3 * r + c];
     return E;
 }
+
+// ------------------------------------------------------------------ solve::homography_solver / solve::fundamental_solver
+namespace adapters {
+//! The reference constructors' problem: all keypoints of both views (cv::KeyPoint is layout-compatible with ovs_keypoint) and the
+//! matches.  The sampler seed is a splitmix64 hash of the keypoint coordinates and the matches (the PnP adapter's rule).
+inline void two_view_problem(const std::vector<cv::KeyPoint>& k1, const std::vector<cv::KeyPoint>& k2,
+                             const std::vector<std::pair<int, int>>& matches_12, std::vector<ovs_keypoint>& own_1,
+                             std::vector<ovs_keypoint>& own_2, std::vector<std::int32_t>& own_m,
+                             solve::two_view_solver_base::problem_view& view) {
+    static_assert(sizeof(cv::KeyPoint) == sizeof(ovs_keypoint), "cv::KeyPoint layout changed");
+    own_1.resize(k1.size()); own_2.resize(k2.size());
+    if (!k1.empty()) std::memcpy(own_1.data(), k1.data(), sizeof(ovs_keypoint) * k1.size());
+    if (!k2.empty()) std::memcpy(own_2.data(), k2.data(), sizeof(ovs_keypoint) * k2.size());
+    own_m.clear();
+    for (const auto& m : matches_12) { own_m.push_back(m.first); own_m.push_back(m.second); }
+    input_hash hash(k1.size() + k2.size() + matches_12.size());
+    for (const auto& k : own_1) { hash.add(&k.x, 4); hash.add(&k.y, 4); }
+    for (const auto& k : own_2) { hash.add(&k.x, 4); hash.add(&k.y, 4); }
+    hash.add(own_m.data(), 4 * own_m.size());
+    view.num_keypts_1 = static_cast<int>(own_1.size()); view.keypts_1 = own_1.data();
+    view.num_keypts_2 = static_cast<int>(own_2.size()); view.keypts_2 = own_2.data();
+    view.num_matches = static_cast<int>(matches_12.size()); view.matches_12 = own_m.data();
+    view.seed = hash.seed;
+}
+inline Mat33_t to_mat33(const double* M) {
+    Mat33_t out;
+    for (int r = 0; r < 3; ++r)
+        for (int c = 0; c < 3; ++c) out(r, c) = M[3 * r + c];
+    return out;
+}
+}  // namespace adapters
+
+inline solve::homography_solver::homography_solver(const std::vector<cv::KeyPoint>& undist_keypts_1,
+                                                   const std::vector<cv::KeyPoint>& undist_keypts_2,
+                                                   const std::vector<std::pair<int, int>>& matches_12, const float sigma)
+    : homography_solver(sigma) {
+    adapters::two_view_problem(undist_keypts_1, undist_keypts_2, matches_12, own_keypts_1_, own_keypts_2_, own_matches_, own_);
+}
+
+inline void solve::homography_solver::find_via_ransac(const unsigned int max_num_iter, const bool recompute) {
+    best_ = two_view_solver_base::find_via_ransac(std::vector<problem_view>{own_}, max_num_iter, recompute).front();
+}
+
+inline Mat33_t solve::homography_solver::get_best_H_21() const { return adapters::to_mat33(best_.M_21); }
+
+inline solve::fundamental_solver::fundamental_solver(const std::vector<cv::KeyPoint>& undist_keypts_1,
+                                                     const std::vector<cv::KeyPoint>& undist_keypts_2,
+                                                     const std::vector<std::pair<int, int>>& matches_12, const float sigma)
+    : fundamental_solver(sigma) {
+    adapters::two_view_problem(undist_keypts_1, undist_keypts_2, matches_12, own_keypts_1_, own_keypts_2_, own_matches_, own_);
+}
+
+inline void solve::fundamental_solver::find_via_ransac(const unsigned int max_num_iter, const bool recompute) {
+    best_ = two_view_solver_base::find_via_ransac(std::vector<problem_view>{own_}, max_num_iter, recompute).front();
+}
+
+inline Mat33_t solve::fundamental_solver::get_best_F_21() const { return adapters::to_mat33(best_.M_21); }
 
 }  // namespace openvslam

@@ -7,6 +7,7 @@
 //   openvslam::solve::sim3_solver                         (src/openvslam/solve/sim3_solver.h)
 //   openvslam::solve::pnp_solver                          (src/openvslam/solve/pnp_solver.h)
 //   openvslam::solve::essential_solver                    (src/openvslam/solve/essential_solver.h)
+//   openvslam::solve::homography_solver / fundamental_solver (src/openvslam/solve/{homography,fundamental}_solver.h)
 // [file names as recalled in SURVEY.md 8(a); /root/reference holds no source, so no line numbers].
 //
 // The reference's methods take cv::Mat / cv::KeyPoint / Eigen / data::frame / data::keyframe.  None of
@@ -792,6 +793,128 @@ private:
     problem_view own_{};                                   // the reference constructor's flattened matches
     std::vector<double> own_bearings_1_, own_bearings_2_;
     solution best_{};
+};
+
+//! The batched find_via_ransac shared by homography_solver and fundamental_solver (the same arguments, one entry point each).
+class two_view_solver_base {
+public:
+    //! One problem on array views (see include/ovs_b200.h, ovs_homography_solve_ransac_host).
+    struct problem_view {
+        int num_keypts_1 = 0, num_keypts_2 = 0;
+        const ovs_keypoint* keypts_1 = nullptr;           // all undistorted keypoints of view 1 (only pt is read)
+        const ovs_keypoint* keypts_2 = nullptr;           // the same of view 2
+        int num_matches = 0;
+        const std::int32_t* matches_12 = nullptr;         // 2 per match: idx_1, idx_2
+        std::uint64_t seed = 0;
+    };
+    struct solution {
+        bool valid = false;
+        double M_21[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};     // row-major H_21 or F_21
+        unsigned int num_inliers = 0;
+        int best_iter = -1;
+        double best_score = 0.0;
+        std::vector<std::uint8_t> is_inlier;
+    };
+    using entry_t = int (*)(ovs_matcher*, int, const std::int32_t*, const ovs_keypoint*, const std::int32_t*, const ovs_keypoint*,
+                            const std::int32_t*, const std::int32_t*, float, int, int, const std::uint64_t*, double*, std::uint8_t*,
+                            std::int32_t*, std::int32_t*, double*, std::uint8_t*);
+
+    two_view_solver_base(entry_t entry, const float sigma, const int device) : entry_(entry), sigma_(sigma) {
+        detail::check(ovs_matcher_create(device, &h_));
+    }
+    ~two_view_solver_base() { ovs_matcher_destroy(h_); }
+    two_view_solver_base(const two_view_solver_base&) = delete;
+    two_view_solver_base& operator=(const two_view_solver_base&) = delete;
+
+    //! find_via_ransac(max_num_iter, recompute) for every problem, one GPU call
+    std::vector<solution> find_via_ransac(const std::vector<problem_view>& problems, const unsigned int max_num_iter,
+                                          const bool recompute = true) const {
+        const int B = static_cast<int>(problems.size());
+        std::vector<std::int32_t> o1(static_cast<std::size_t>(B) + 1, 0), o2(o1), om(o1);
+        for (int b = 0; b < B; ++b) {
+            o1[b + 1] = o1[b] + problems[b].num_keypts_1;
+            o2[b + 1] = o2[b] + problems[b].num_keypts_2;
+            om[b + 1] = om[b] + problems[b].num_matches;
+        }
+        std::vector<ovs_keypoint> k1(std::max(o1[B], 1)), k2(std::max(o2[B], 1));
+        std::vector<std::int32_t> mt(2 * static_cast<std::size_t>(std::max(om[B], 1)));
+        std::vector<std::uint64_t> seeds(std::max(B, 1));
+        for (int b = 0; b < B; ++b) {
+            const problem_view& p = problems[b];
+            seeds[b] = p.seed;
+            if (p.num_keypts_1) std::memcpy(&k1[o1[b]], p.keypts_1, sizeof(ovs_keypoint) * p.num_keypts_1);
+            if (p.num_keypts_2) std::memcpy(&k2[o2[b]], p.keypts_2, sizeof(ovs_keypoint) * p.num_keypts_2);
+            if (p.num_matches) std::memcpy(&mt[2 * static_cast<std::size_t>(om[b])], p.matches_12, 8 * static_cast<std::size_t>(p.num_matches));
+        }
+        std::vector<double> M(9 * static_cast<std::size_t>(std::max(B, 1))), score(std::max(B, 1));
+        std::vector<std::uint8_t> valid(std::max(B, 1)), flags(std::max(om[B], 1));
+        std::vector<std::int32_t> num(std::max(B, 1)), best(std::max(B, 1));
+        detail::check(entry_(h_, B, o1.data(), k1.data(), o2.data(), k2.data(), om.data(), mt.data(), sigma_, static_cast<int>(max_num_iter),
+                     recompute ? 1 : 0, seeds.data(), M.data(), valid.data(), num.data(), best.data(), score.data(), flags.data()));
+        std::vector<solution> out(B);
+        for (int b = 0; b < B; ++b) {
+            out[b].valid = valid[b] != 0;
+            std::memcpy(out[b].M_21, &M[9 * static_cast<std::size_t>(b)], 9 * sizeof(double));
+            out[b].num_inliers = static_cast<unsigned int>(num[b]);
+            out[b].best_iter = best[b];
+            out[b].best_score = score[b];
+            out[b].is_inlier.assign(flags.begin() + om[b], flags.begin() + om[b + 1]);
+        }
+        return out;
+    }
+
+    //! the last find_via_ransac(max_num_iter, recompute) of a solver built with the reference's constructor
+    const solution& best_solution() const { return best_; }
+
+protected:
+    entry_t entry_;
+    float sigma_;
+    ovs_matcher* h_ = nullptr;
+    problem_view own_{};                                   // the reference constructor's problem
+    std::vector<ovs_keypoint> own_keypts_1_, own_keypts_2_;
+    std::vector<std::int32_t> own_matches_;
+    solution best_{};
+};
+
+//! solve::homography_solver (perspective map initialisation): RANSAC over the normalised 8-point DLT on keypoint matches, with an
+//! optional refit on all inliers.  The reference builds one solver per pair of views; here find_via_ransac(problems, max_num_iter,
+//! recompute) solves a whole batch in one call, and the reference's constructor / find_via_ransac(max_num_iter, recompute) /
+//! getters are in adapters.hpp.  H_21 maps view 1 to view 2: p2 ~ H_21 p1.
+class homography_solver : public two_view_solver_base {
+public:
+    explicit homography_solver(const float sigma = 1.0f, const int device = 0)
+        : two_view_solver_base(&ovs_homography_solve_ransac_host, sigma, device) {}
+#ifdef OVS_B200_WITH_REFERENCE_TYPES
+    //! The reference's signatures (solve/homography_solver.h); bodies in adapters.hpp.  The sampler is seeded with a splitmix64
+    //! hash of the input bits (the batched call takes explicit seeds).
+    homography_solver(const std::vector<cv::KeyPoint>& undist_keypts_1, const std::vector<cv::KeyPoint>& undist_keypts_2,
+                      const std::vector<std::pair<int, int>>& matches_12, const float sigma);
+    void find_via_ransac(const unsigned int max_num_iter, const bool recompute = true);
+    bool solution_is_valid() const { return best_.valid; }
+    float get_best_score() const { return static_cast<float>(best_.best_score); }
+    Mat33_t get_best_H_21() const;
+    std::vector<bool> get_inlier_matches() const { return std::vector<bool>(best_.is_inlier.begin(), best_.is_inlier.end()); }
+#endif
+    using two_view_solver_base::find_via_ransac;
+};
+
+//! solve::fundamental_solver (perspective map initialisation): RANSAC over the normalised eight-point algorithm with a rank-2
+//! projection; the same interface as homography_solver.  p2^T F_21 p1 = 0.
+class fundamental_solver : public two_view_solver_base {
+public:
+    explicit fundamental_solver(const float sigma = 1.0f, const int device = 0)
+        : two_view_solver_base(&ovs_fundamental_solve_ransac_host, sigma, device) {}
+#ifdef OVS_B200_WITH_REFERENCE_TYPES
+    //! The reference's signatures (solve/fundamental_solver.h); bodies in adapters.hpp.
+    fundamental_solver(const std::vector<cv::KeyPoint>& undist_keypts_1, const std::vector<cv::KeyPoint>& undist_keypts_2,
+                       const std::vector<std::pair<int, int>>& matches_12, const float sigma);
+    void find_via_ransac(const unsigned int max_num_iter, const bool recompute = true);
+    bool solution_is_valid() const { return best_.valid; }
+    float get_best_score() const { return static_cast<float>(best_.best_score); }
+    Mat33_t get_best_F_21() const;
+    std::vector<bool> get_inlier_matches() const { return std::vector<bool>(best_.is_inlier.begin(), best_.is_inlier.end()); }
+#endif
+    using two_view_solver_base::find_via_ransac;
 };
 
 }  // namespace solve

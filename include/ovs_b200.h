@@ -206,6 +206,35 @@ int ovs_robust_brute_force_match_device(ovs_matcher* h, const uint8_t* d_desc_fr
 int ovs_essential_solve_ransac_host(ovs_matcher* h, int B, const int32_t* match_offsets, const double* bearings_1, const double* bearings_2,
                                     int max_num_iter, int recompute, const uint64_t* seeds, double* E_21, uint8_t* valid,
                                     int32_t* num_inliers, int32_t* best_iter, double* best_score, uint8_t* inlier_out);
+/* solve::homography_solver(undist_keypts_1, undist_keypts_2, matches_12, sigma).find_via_ransac(max_num_iter, recompute) and
+ * solve::fundamental_solver(...) the same way (solve/{homography,fundamental}_solver.cc): the two solvers perspective map
+ * initialisation runs on each frame (it passes sigma = 1.0 and recompute = true), for B independent problems in one call.
+ * Problem b owns the keypoints keypt_offsets_1[b] .. keypt_offsets_1[b + 1] - 1 of keypts_1 (ALL of view 1's undistorted
+ * keypoints: undist_keypts_.data() can be passed; only pt is read), the same of keypts_2 through keypt_offsets_2, and the matches
+ * match_offsets[b] .. match_offsets[b + 1] - 1 of matches_12 (2 per match: idx_1, idx_2, indices into the problem's own keypoints).
+ * Every offset array starts at 0 and is non-decreasing.  seeds[B]: the sampler's seed per problem (a problem gives the same
+ * result alone or inside a batch).  Each view is normalised over all of its keypoints; hypotheses are solved on 8 matches.
+ * Per problem: H_21[b*9] / F_21[b*9] row-major (p2 ~ H_21 p1, p2^T F_21 p1 = 0, pixel coordinates; the entry of largest magnitude
+ * positive; zero when no hypothesis scored above 0), valid[b] = solution_is_valid() (best score > 0 and at least 8 inliers),
+ * num_inliers[b] = the number of inlier flags set, best_iter[b] = the best hypothesis (-1: none), best_score[b] = get_best_score()
+ * (after the recompute, when one ran), inlier_out[m] = get_inlier_matches().  Fewer than 8 matches: no hypothesis runs and the
+ * problem is invalid.  With recompute, a valid problem is solved again on all inliers and its flags, count and score are re-checked
+ * (valid keeps its value).  The conventions (normalisation, minimal solves, the inlier tests and score, their summation orders) are
+ * in DESIGN.md section 5.  B outside 0 .. 65535, invalid offsets, a match index outside its problem's keypoints, a keypoint
+ * coordinate that is not finite, sigma <= 0 (or not finite) or a negative max_num_iter return OVS_ERR_INVALID_ARG before any
+ * launch; B == 0 or no match at all returns without a launch.  Otherwise the call is four launches (one with max_num_iter == 0),
+ * one copy each way and one wait.  The solve has its own buffers on the handle: the brute-force and essential entry points are
+ * unaffected by it. */
+int ovs_homography_solve_ransac_host(ovs_matcher* h, int B, const int32_t* keypt_offsets_1, const ovs_keypoint* keypts_1,
+                                     const int32_t* keypt_offsets_2, const ovs_keypoint* keypts_2, const int32_t* match_offsets,
+                                     const int32_t* matches_12, float sigma, int max_num_iter, int recompute, const uint64_t* seeds,
+                                     double* H_21, uint8_t* valid, int32_t* num_inliers, int32_t* best_iter, double* best_score,
+                                     uint8_t* inlier_out);
+int ovs_fundamental_solve_ransac_host(ovs_matcher* h, int B, const int32_t* keypt_offsets_1, const ovs_keypoint* keypts_1,
+                                      const int32_t* keypt_offsets_2, const ovs_keypoint* keypts_2, const int32_t* match_offsets,
+                                      const int32_t* matches_12, float sigma, int max_num_iter, int recompute, const uint64_t* seeds,
+                                      double* F_21, uint8_t* valid, int32_t* num_inliers, int32_t* best_iter, double* best_score,
+                                      uint8_t* inlier_out);
 /* match::robust::match_frame_and_keyframe(frm, keyfrm, matched_lms_in_frm) (match/robust.cc), the tracker's robust-match fallback:
  * ovs_robust_brute_force_match_host (the same pairs, bit for bit), then the essential solver on them with recompute off
  * (the reference calls find_via_ransac(50, false); pass max_num_iter = 50).  bearings_frm[n1*3] = frm.bearings_,

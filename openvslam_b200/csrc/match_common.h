@@ -23,6 +23,9 @@ struct ovs_matcher {
     // the essential solver's own arenas (essential_ransac.cu): a solve leaves the brute-force buffers above untouched
     uint8_t* d_ess = nullptr; size_t d_ess_cap = 0;
     uint8_t* h_ess = nullptr; size_t h_ess_cap = 0;     // pinned
+    // the homography / fundamental-matrix solvers' own arenas (two_view_ransac.cu)
+    uint8_t* d_tv = nullptr; size_t d_tv_cap = 0;
+    uint8_t* h_tv = nullptr; size_t h_tv_cap = 0;       // pinned
     cudaEvent_t ev[2]{};
     float last_kernel_us = 0.f;
     int num_requeries = 0;   // GPU re-queries issued by the greedy replays so far (diagnostic)

@@ -1,9 +1,9 @@
-"""Host-side mirror of openvslam::solve::sim3_solver, solve::pnp_solver and solve::essential_solver
-(src/openvslam/solve/{sim3,pnp,essential}_solver.h; names as in SURVEY.md 8a) over the C ABI of libovs_b200.so: loop detection's
-Sim3 RANSAC, relocalisation's PnP RANSAC and the tracker's essential-matrix RANSAC, each solved on the GPU for a whole batch of
-problems in one call.  The reference constructs one solver per problem; here each problem is a `problem` of flat arrays (see
-include/ovs_b200.h, ovs_sim3_solve_ransac_host / ovs_pnp_solve_ransac_host / ovs_essential_solve_ransac_host, for the
-field-by-field mapping)."""
+"""Host-side mirror of openvslam::solve::sim3_solver, solve::pnp_solver, solve::essential_solver, solve::homography_solver and
+solve::fundamental_solver (src/openvslam/solve/*_solver.h; names as in SURVEY.md 8a) over the C ABI of libovs_b200.so: loop
+detection's Sim3 RANSAC, relocalisation's PnP RANSAC, the tracker's essential-matrix RANSAC and perspective map initialisation's
+homography and fundamental-matrix RANSAC, each solved on the GPU for a whole batch of problems in one call.  The reference
+constructs one solver per problem; here each problem is a `problem` of flat arrays (see include/ovs_b200.h,
+ovs_*_solve_ransac_host, for the field-by-field mapping)."""
 import ctypes as C
 
 import numpy as np
@@ -153,3 +153,77 @@ class essential_solver(_matcher_handle):
                                                               vp(E), vp(valid), vp(ninl), vp(best), vp(score), vp(flags)))
         return [dict(valid=bool(valid[b]), E_21=E[b].reshape(3, 3).copy(), num_inliers=int(ninl[b]), best_iter=int(best[b]),
                      best_score=float(score[b]), inliers=flags[off[b]:off[b + 1]].astype(bool)) for b in range(B)]
+
+
+# cv::KeyPoint / ovs_keypoint (28 bytes): the two-view solvers read pt only
+_KEYPOINT = np.dtype([("x", "<f4"), ("y", "<f4"), ("size", "<f4"), ("angle", "<f4"), ("response", "<f4"), ("octave", "<i4"),
+                      ("class_id", "<i4")])
+
+
+class _two_view_solver(_matcher_handle):
+    _entry = None
+    _key = None
+
+    def __init__(self, sigma=1.0, device=0):
+        super().__init__(device)
+        self.sigma_ = float(sigma)
+
+    def find_via_ransac(self, problems, max_num_iter, recompute=True, seeds=None):
+        name = type(self).__name__
+        B = len(problems)
+        kp1, kp2, mt = [], [], []
+        for p in problems:
+            k1 = np.asarray(p["keypts_1"], np.float32); k2 = np.asarray(p["keypts_2"], np.float32)
+            m = np.asarray(p["matches_12"]).reshape(-1, 2) if np.asarray(p["matches_12"]).size else np.zeros((0, 2), np.int32)
+            if k1.size % 2 or k2.size % 2:
+                raise ValueError(name + ": keypts_1 / keypts_2 need (n, 2) each")
+            kp1.append(k1.reshape(-1, 2)); kp2.append(k2.reshape(-1, 2)); mt.append(m.astype(np.int32))
+
+        def offsets(arrs):
+            off = np.zeros(B + 1, np.int32)
+            off[1:] = np.cumsum([len(a) for a in arrs])
+            return off
+        koff1, koff2, moff = offsets(kp1), offsets(kp2), offsets(mt)
+        N = int(moff[-1])
+        seeds = np.arange(B, dtype=np.uint64) if seeds is None else np.asarray(seeds, np.uint64).reshape(-1)
+        if len(seeds) != B:
+            raise ValueError(name + ": one seed per problem")
+
+        def keypoints(arrs):
+            xy = np.concatenate(arrs) if B and sum(len(a) for a in arrs) else np.zeros((0, 2), np.float32)
+            out = np.zeros(max(len(xy), 1), _KEYPOINT)
+            out["x"][:len(xy)] = xy[:, 0]; out["y"][:len(xy)] = xy[:, 1]
+            return out
+        k1, k2 = keypoints(kp1), keypoints(kp2)
+        m, pm = _p(np.concatenate(mt) if N else np.zeros((1, 2), np.int32), np.int32)
+        o1, po1 = _p(koff1, np.int32); o2, po2 = _p(koff2, np.int32); om, pom = _p(moff, np.int32)
+        seeds_, pseed = _p(seeds if B else np.zeros(1, np.uint64), np.uint64)
+        M = np.zeros((max(B, 1), 9)); valid = np.zeros(max(B, 1), np.uint8); score = np.zeros(max(B, 1))
+        ninl = np.zeros(max(B, 1), np.int32); best = np.zeros(max(B, 1), np.int32); flags = np.zeros(max(N, 1), np.uint8)
+        vp = lambda a: a.ctypes.data_as(C.c_void_p)
+        _lib.check(getattr(_lib.lib(), self._entry)(self._h, B, po1, vp(k1), po2, vp(k2), pom, pm, C.c_float(self.sigma_), int(max_num_iter),
+                                                    int(bool(recompute)), pseed, vp(M), vp(valid), vp(ninl), vp(best), vp(score), vp(flags)))
+        return [{"valid": bool(valid[b]), self._key: M[b].reshape(3, 3).copy(), "num_inliers": int(ninl[b]), "best_iter": int(best[b]),
+                 "best_score": float(score[b]), "inliers": flags[moff[b]:moff[b + 1]].astype(bool)} for b in range(B)]
+
+
+class homography_solver(_two_view_solver):
+    """openvslam::solve::homography_solver(undist_keypts_1, undist_keypts_2, matches_12, sigma), batched, on a matcher handle (its
+    own buffers: the handle's matchers and essential solver are unaffected).  Perspective map initialisation passes sigma = 1.0.
+
+    find_via_ransac(problems, max_num_iter, recompute=True, seeds=None): problems is a list of dicts with
+      keypts_1    (n1, 2) undistorted keypoints of view 1 (all of them: the normalisation runs over every keypoint),
+      keypts_2    (n2, 2) the same of view 2,
+      matches_12  (m, 2) pairs (idx_1, idx_2) into them;
+    seeds: one sampler seed per problem (default: the problem's index).  A problem gives the same result alone or in a batch.
+    Returns one dict per problem: valid (solution_is_valid()), H_21 (3, 3) (get_best_H_21(), p2 ~ H_21 p1; zero when no hypothesis
+    scored), num_inliers, best_iter (-1: none), best_score (get_best_score()), inliers (m,) bool (get_inlier_matches())."""
+    _entry = "ovs_homography_solve_ransac_host"
+    _key = "H_21"
+
+
+class fundamental_solver(_two_view_solver):
+    """openvslam::solve::fundamental_solver(undist_keypts_1, undist_keypts_2, matches_12, sigma), batched; the same interface as
+    homography_solver, with F_21 (3, 3) (get_best_F_21(), p2^T F_21 p1 = 0, rank 2) in place of H_21."""
+    _entry = "ovs_fundamental_solve_ransac_host"
+    _key = "F_21"
