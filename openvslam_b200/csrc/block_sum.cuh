@@ -1,6 +1,6 @@
 // block_sum.cuh -- the CTA-wide form of pnp_sum (pnp_math.cuh), shared by the solvers whose recompute kernels sum over every
-// inlier of a problem with one 256-thread CTA: the PnP solver's EPnP (optimize.cu, k_pnp_refine) and the essential solver's
-// eight-point A^T A (essential_ransac.cu, k_essential_refine).  Device only.
+// inlier of a problem with one 256-thread CTA: the PnP solver's EPnP (optimize.cu, k_pnp_refine) and the essential, homography
+// and fundamental-matrix solvers' A^T A (two_view_ransac.cu, k_two_view_refine).  Device only.
 #pragma once
 #include "pnp_math.cuh"
 

@@ -20,7 +20,7 @@ struct ovs_matcher {
     unsigned* d_mask = nullptr; size_t d_mask_cap = 0;
     unsigned* h_keys = nullptr; size_t h_keys_cap = 0;  // pinned
     uint8_t* h_stage = nullptr; size_t h_stage_cap = 0; // pinned
-    // the essential solver's own arenas (essential_ransac.cu): a solve leaves the brute-force buffers above untouched
+    // the essential solver's own arenas (two_view_ransac.cu): a solve leaves the brute-force buffers above untouched
     uint8_t* d_ess = nullptr; size_t d_ess_cap = 0;
     uint8_t* h_ess = nullptr; size_t h_ess_cap = 0;     // pinned
     // the homography / fundamental-matrix solvers' own arenas (two_view_ransac.cu)

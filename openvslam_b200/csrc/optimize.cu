@@ -48,10 +48,12 @@
 #include "block_sum.cuh"
 #include "ovs_common.h"
 #include "pnp_math.cuh"
+#include "ransac.cuh"
 #include "sim3_math.cuh"
 
 namespace {
 
+using ovs::Arena;
 using ovs::CameraD;
 
 constexpr int kMaxReducedDimBig = 6000;  // 1000 free keyframes: beyond this the dense (n + 1) x n x 4 systems alone are > 1 GB
@@ -2273,16 +2275,6 @@ struct ovs_optimizer {
 
 namespace {
 
-struct Arena {
-    uint8_t* base; size_t off, cap;
-    template <typename T> T* take(size_t n) {
-        off = (off + 255) / 256 * 256;
-        T* p = reinterpret_cast<T*>(base + off);
-        off += n * sizeof(T);
-        return p;
-    }
-};
-
 int ensure_arenas(ovs_optimizer* h, size_t dbytes, size_t hbytes) {
     // grow with a quarter of slack: a map's local window changes size from call to call, and every cudaFree / cudaMalloc stalls
     // all streams of the device
@@ -2333,7 +2325,7 @@ extern "C" int ovs_pose_optimize_host(ovs_optimizer* h, const ovs_camera* cam, i
     const size_t dbytes = hbytes + N * 24 + N + 4096;
     int rc = ensure_arenas(h, dbytes, hbytes);
     if (rc != OVS_OK) return rc;
-    Arena H{h->h_arena, 0, h->h_cap}, D{h->d_arena, 0, h->d_cap};
+    Arena H{h->h_arena, 0}, D{h->d_arena, 0};
     double* hp = H.take<double>(3 * N); float* hxy = H.take<float>(2 * N); float* hxr = H.take<float>(N); float* hw = H.take<float>(N);
     double* hpose = H.take<double>(12); double* hstats = H.take<double>(16); uint8_t* hout = H.take<uint8_t>(N);
     const size_t in_bytes = H.off;
@@ -2635,7 +2627,7 @@ extern "C" int ovs_transform_optimize_host(ovs_optimizer* h, const ovs_camera* c
     const size_t dbytes = hbytes + N * 32 + N + 4096;
     int rc = ensure_arenas(h, dbytes, hbytes);
     if (rc != OVS_OK) return rc;
-    Arena H{h->h_arena, 0, h->h_cap}, D{h->d_arena, 0, h->d_cap};
+    Arena H{h->h_arena, 0}, D{h->d_arena, 0};
     double* hp1 = H.take<double>(3 * N); float* hxy1 = H.take<float>(2 * N); float* hw1 = H.take<float>(N);
     double* hp2 = H.take<double>(3 * N); float* hxy2 = H.take<float>(2 * N); float* hw2 = H.take<float>(N);
     double* hS = H.take<double>(13); double* hstats = H.take<double>(16); uint8_t* hout = H.take<uint8_t>(N);
@@ -2770,14 +2762,9 @@ __global__ void __launch_bounds__(kRansacThreads) k_sim3_ransac(RansacArgs A) {
         ransac_hypothesis(A, b, o, n, k, S12, S21);
         ovs::sim3_scaled_rotation(S12, sR12);
         ovs::sim3_scaled_rotation(S21, sR21);
-        unsigned cnt = 0;
-        for (int base = 0; base < n; base += 32) {
-            const int i = base + lane;
-            const bool in = i < n && ransac_pair(A, c1, c2, sR12, S12, sR21, S21, (size_t)(o + i));
-            cnt += __popc(__ballot_sync(0xffffffffu, in));
-        }
+        const unsigned cnt = ovs::warp_count(n, lane, [&](int i) { return ransac_pair(A, c1, c2, sR12, S12, sR21, S21, (size_t)(o + i)); });
         if (lane == 0 && cnt > 0) {
-            atomicMax(&A.key[b], ((unsigned long long)cnt << 32) | (unsigned long long)(~(unsigned)k));
+            atomicMax(&A.key[b], ovs::best_key(cnt, k));
             __threadfence();
         }
     }
@@ -2790,9 +2777,8 @@ __global__ void __launch_bounds__(kRansacThreads) k_sim3_ransac(RansacArgs A) {
     __syncthreads();
     if (!s_last) return;
     __threadfence();
-    const unsigned long long key = atomicOr(&A.key[b], 0ull);
-    const unsigned cnt = (unsigned)(key >> 32);
-    const int best = cnt > 0 ? (int)(~(unsigned)(key & 0xffffffffull)) : -1;
+    unsigned cnt;
+    const int best = ovs::best_of_key(atomicOr(&A.key[b], 0ull), &cnt);
     double S12[13], S21[13];
     if (best >= 0) {
         double sR12[9], sR21[9];
@@ -2825,13 +2811,15 @@ extern "C" int ovs_sim3_solve_ransac_host(ovs_optimizer* h, int B, const int32_t
     if (B == 0) return OVS_OK;
     OVS_REQUIRE(pair_offsets && cam_1 && pose_1w && cam_2 && pose_2w && seeds && sim3_12 && valid && num_inliers && best_iter,
                 OVS_ERR_INVALID_ARG, "null argument");
-    OVS_REQUIRE(pair_offsets[0] == 0, OVS_ERR_INVALID_ARG, "pair_offsets[0] must be 0");
-    for (int b = 0; b < B; ++b) {
-        OVS_REQUIRE(pair_offsets[b + 1] >= pair_offsets[b], OVS_ERR_INVALID_ARG, "pair_offsets must be non-decreasing (problem %d)", b);
-        OVS_REQUIRE((cam_1[b].model == ovs::kCamPerspective || cam_1[b].model == ovs::kCamEquirectangular) &&
-                    (cam_2[b].model == ovs::kCamPerspective || cam_2[b].model == ovs::kCamEquirectangular),
-                    OVS_ERR_INVALID_ARG, "unknown camera model (problem %d)", b);
-    }
+    int rc;
+    for (int b = 0; b < B; ++b)
+        if (!((cam_1[b].model == ovs::kCamPerspective || cam_1[b].model == ovs::kCamEquirectangular) &&
+              (cam_2[b].model == ovs::kCamPerspective || cam_2[b].model == ovs::kCamEquirectangular))) {
+            // problem by problem, the offsets up to problem b are checked before its cameras
+            if ((rc = ovs::check_offsets(pair_offsets, b + 1, "pair_offsets")) != OVS_OK) return rc;
+            OVS_REQUIRE(false, OVS_ERR_INVALID_ARG, "unknown camera model (problem %d)", b);
+        }
+    if ((rc = ovs::check_offsets(pair_offsets, B, "pair_offsets")) != OVS_OK) return rc;
     const int n_all = pair_offsets[B];
     OVS_REQUIRE(n_all == 0 || (pos_w_1 && sigma_sq_1 && pos_w_2 && sigma_sq_2 && inlier_out), OVS_ERR_INVALID_ARG, "null argument");
     for (int i = 0; i < n_all; ++i)
@@ -2849,47 +2837,36 @@ extern "C" int ovs_sim3_solve_ransac_host(ovs_optimizer* h, int B, const int32_t
     invalidate_plan(h);
     if (h->pending) { OVS_CUDA_CHECK(ovs::sync_stream(h->stream)); h->pending = false; }
     const size_t N = (size_t)n_all, NB = (size_t)B;
-    const size_t in_bytes_max = 256 * 12 + (NB + 1) * 4 + NB * 2 * sizeof(CameraD) + NB * 2 * 96 + N * 2 * (24 + 4) + NB * (8 + 8 + 4);
-    const size_t out_bytes_max = 256 * 5 + NB * (13 * 8 + 4 + 4 + 1) + N;
-    const size_t hbytes = in_bytes_max + out_bytes_max;
-    const size_t dbytes = hbytes + 256 * 6 + N * 2 * (24 + 16 + 4) + 4096;
-    int rc = ensure_arenas(h, dbytes, hbytes);
-    if (rc != OVS_OK) return rc;
-    Arena H{h->h_arena, 0, h->h_cap}, D{h->d_arena, 0, h->d_cap};
-    // inputs: the same carving sequence in both arenas, so one contiguous copy moves them
-    int* hoff = H.take<int>(NB + 1); CameraD* hc1 = H.take<CameraD>(NB); CameraD* hc2 = H.take<CameraD>(NB);
-    double* hp1 = H.take<double>(12 * NB); double* hp2 = H.take<double>(12 * NB);
-    double* hw1 = H.take<double>(3 * N); float* hs1 = H.take<float>(N); double* hw2 = H.take<double>(3 * N); float* hs2 = H.take<float>(N);
-    uint64_t* hseed = H.take<uint64_t>(NB); unsigned long long* hkey = H.take<unsigned long long>(NB); unsigned* hdone = H.take<unsigned>(NB);
-    const size_t in_bytes = H.off;
-    // outputs: one contiguous copy back
-    double* hS = H.take<double>(13 * NB);
-    const size_t out_begin = (size_t)((uint8_t*)hS - h->h_arena);
-    int* hnum = H.take<int>(NB); int* hbest = H.take<int>(NB); uint8_t* hvalid = H.take<uint8_t>(NB); uint8_t* hflags = H.take<uint8_t>(N);
-    const size_t out_end = H.off;
     RansacArgs A;
     A.B = B; A.N = n_all; A.fix_scale = fix_scale ? 1 : 0; A.min_num_inliers = min_num_inliers; A.max_num_iter = max_num_iter;
-    A.off = D.take<int>(NB + 1); A.cam1 = D.take<CameraD>(NB); A.cam2 = D.take<CameraD>(NB);
-    A.pose1 = D.take<double>(12 * NB); A.pose2 = D.take<double>(12 * NB);
-    A.pw1 = D.take<double>(3 * N); A.sig1 = D.take<float>(N); A.pw2 = D.take<double>(3 * N); A.sig2 = D.take<float>(N);
-    A.seed = D.take<uint64_t>(NB); A.key = D.take<unsigned long long>(NB); A.done = D.take<unsigned>(NB);
-    A.sim3 = D.take<double>(13 * NB); A.num_inliers = D.take<int>(NB); A.best_iter = D.take<int>(NB); A.valid = D.take<uint8_t>(NB);
-    A.inlier = D.take<uint8_t>(N);
-    A.pc1 = D.take<double>(3 * N); A.pc2 = D.take<double>(3 * N); A.rp1 = D.take<double>(2 * N); A.rp2 = D.take<double>(2 * N);
-    A.bd1 = D.take<float>(N); A.bd2 = D.take<float>(N);
+    int* hoff; CameraD *hc1, *hc2; double *hp1, *hp2, *hw1, *hw2; float *hs1, *hs2; uint64_t* hseed; unsigned long long* hkey; unsigned* hdone;
+    double* hS; int *hnum, *hbest; uint8_t *hvalid, *hflags;
+    ovs::Staging S;
+    rc = ovs::stage(S, h->h_arena, h->d_arena, [&](size_t hbytes, size_t dbytes) { return ensure_arenas(h, dbytes, hbytes); },
+                    [&](ovs::Staging& S) {
+        A.off = S.in(hoff, NB + 1); A.cam1 = S.in(hc1, NB); A.cam2 = S.in(hc2, NB);
+        A.pose1 = S.in(hp1, 12 * NB); A.pose2 = S.in(hp2, 12 * NB);
+        A.pw1 = S.in(hw1, 3 * N); A.sig1 = S.in(hs1, N); A.pw2 = S.in(hw2, 3 * N); A.sig2 = S.in(hs2, N);
+        A.seed = S.in(hseed, NB); A.key = S.in(hkey, NB); A.done = S.in(hdone, NB);
+        A.sim3 = S.out(hS, 13 * NB); A.num_inliers = S.out(hnum, NB); A.best_iter = S.out(hbest, NB); A.valid = S.out(hvalid, NB);
+        A.inlier = S.out(hflags, N);
+        A.pc1 = S.dev<double>(3 * N); A.pc2 = S.dev<double>(3 * N); A.rp1 = S.dev<double>(2 * N); A.rp2 = S.dev<double>(2 * N);
+        A.bd1 = S.dev<float>(N); A.bd2 = S.dev<float>(N);
+    });
+    if (rc != OVS_OK) return rc;
     memcpy(hoff, pair_offsets, 4 * (NB + 1));
     for (int b = 0; b < B; ++b) { hc1[b] = to_cam(&cam_1[b]); hc2[b] = to_cam(&cam_2[b]); }
     memcpy(hp1, pose_1w, 96 * NB); memcpy(hp2, pose_2w, 96 * NB);
     memcpy(hw1, pos_w_1, 24 * N); memcpy(hs1, sigma_sq_1, 4 * N); memcpy(hw2, pos_w_2, 24 * N); memcpy(hs2, sigma_sq_2, 4 * N);
     memcpy(hseed, seeds, 8 * NB); memset(hkey, 0, 8 * NB); memset(hdone, 0, 4 * NB);
     cudaStream_t st = h->stream;
-    OVS_CUDA_CHECK(cudaMemcpyAsync(h->d_arena, h->h_arena, in_bytes, cudaMemcpyHostToDevice, st));
+    OVS_CUDA_CHECK(S.upload(st));
     k_sim3_ransac_prep<<<(n_all + kRansacPrepThreads - 1) / kRansacPrepThreads, kRansacPrepThreads, 0, st>>>(A);
     OVS_LAUNCH_CHECK();
     const int hyp_blocks = max_num_iter > 0 ? (max_num_iter + kRansacWarps - 1) / kRansacWarps : 1;
     k_sim3_ransac<<<dim3(hyp_blocks, B), kRansacThreads, 0, st>>>(A);
     OVS_LAUNCH_CHECK();
-    OVS_CUDA_CHECK(cudaMemcpyAsync(h->h_arena + out_begin, h->d_arena + out_begin, out_end - out_begin, cudaMemcpyDeviceToHost, st));
+    OVS_CUDA_CHECK(S.download(st));
     OVS_CUDA_CHECK(ovs::sync_stream(st));
     memcpy(sim3_12, hS, 13 * 8 * NB);
     memcpy(num_inliers, hnum, 4 * NB); memcpy(best_iter, hbest, 4 * NB); memcpy(valid, hvalid, NB);
@@ -2953,13 +2930,8 @@ __global__ void __launch_bounds__(kPnpThreads) k_pnp_ransac(PnpArgs A) {
     const double* hp = A.hyp + 12 * ((size_t)b * A.H + k);
     double pose[12];
     for (int m = 0; m < 12; ++m) pose[m] = hp[m];
-    unsigned cnt = 0;
-    for (int base = 0; base < n; base += 32) {
-        const int i = base + lane;
-        const bool in = i < n && pnp_corr(A, pose, (size_t)(o + i));
-        cnt += __popc(__ballot_sync(0xffffffffu, in));
-    }
-    if (lane == 0 && cnt > 0) atomicMax(&A.key[b], ((unsigned long long)cnt << 32) | (unsigned long long)(~(unsigned)k));
+    const unsigned cnt = ovs::warp_count(n, lane, [&](int i) { return pnp_corr(A, pose, (size_t)(o + i)); });
+    if (lane == 0 && cnt > 0) atomicMax(&A.key[b], ovs::best_key(cnt, k));
 }
 
 // pnp_sum across the CTA (block_sum.cuh): same bits as PnpSeqSum.
@@ -2971,12 +2943,11 @@ __global__ void __launch_bounds__(kPnpRefineThreads) k_pnp_refine(PnpArgs A) {
     __shared__ double s_red[kPnpChunk * kPnpRefineThreads];
     __shared__ double s_res[78];
     __shared__ int s_warp[kPnpRefineThreads / 32];
-    const int b = blockIdx.x, t = threadIdx.x, lane = t & 31, warp = t >> 5;
+    const int b = blockIdx.x, t = threadIdx.x;
     const int o = A.off[b], n = A.off[b + 1] - o;
     const bool runs = pnp_runs(A, n);
-    const unsigned long long key = A.key[b];
-    const unsigned cnt = (unsigned)(key >> 32);
-    const int best = cnt > 0 ? (int)(~(unsigned)(key & 0xffffffffull)) : -1;
+    unsigned cnt;
+    const int best = ovs::best_of_key(A.key[b], &cnt);
     double pose[12];
     if (best >= 0) {
         const double* hp = A.hyp + 12 * ((size_t)b * A.H + best);
@@ -2988,20 +2959,7 @@ __global__ void __launch_bounds__(kPnpRefineThreads) k_pnp_refine(PnpArgs A) {
     const bool valid = runs && (int)cnt >= A.min_num_inliers;
     int num = (int)cnt;
     if (valid && A.recompute && best >= 0 && (int)cnt >= ovs::kPnpMinSet) {
-        int running = 0;
-        for (int base = 0; base < n; base += kPnpRefineThreads) {   // compaction in index order
-            const int i = base + t;
-            const bool f = i < n && pnp_corr(A, pose, (size_t)(o + i));
-            const unsigned bal = __ballot_sync(0xffffffffu, f);
-            if (lane == 0) s_warp[warp] = __popc(bal);
-            __syncthreads();
-            int before = running;
-            for (int w = 0; w < warp; ++w) before += s_warp[w];
-            if (f) A.cidx[o + before + __popc(bal & ((1u << lane) - 1u))] = i;
-            for (int w = 0; w < kPnpRefineThreads / 32; ++w) running += s_warp[w];
-            __syncthreads();
-        }
-        __syncthreads();
+        ovs::cta_compact<kPnpRefineThreads>(n, A.cidx + o, s_warp, [&](int i) { return pnp_corr(A, pose, (size_t)(o + i)); });
         const ovs::PnpPoints P{A.pw + 3 * (size_t)o, A.bear + 3 * (size_t)o, A.cidx + o, (int)cnt};
         double np[12];
         ovs::epnp_pose(P, PnpBlockSum{(int)cnt, s_red, s_res}, np);
@@ -3033,9 +2991,8 @@ extern "C" int ovs_pnp_solve_ransac_host(ovs_optimizer* h, int B, const int32_t*
     OVS_REQUIRE(min_num_inliers >= 0 && max_num_iter >= 0, OVS_ERR_INVALID_ARG, "min_num_inliers and max_num_iter must not be negative");
     if (B == 0) return OVS_OK;
     OVS_REQUIRE(corr_offsets && seeds && pose_cw && valid && num_inliers && best_iter, OVS_ERR_INVALID_ARG, "null argument");
-    OVS_REQUIRE(corr_offsets[0] == 0, OVS_ERR_INVALID_ARG, "corr_offsets[0] must be 0");
-    for (int b = 0; b < B; ++b)
-        OVS_REQUIRE(corr_offsets[b + 1] >= corr_offsets[b], OVS_ERR_INVALID_ARG, "corr_offsets must be non-decreasing (problem %d)", b);
+    int rc;
+    if ((rc = ovs::check_offsets(corr_offsets, B, "corr_offsets")) != OVS_OK) return rc;
     const int n_all = corr_offsets[B];
     OVS_REQUIRE(n_all == 0 || (bearings && pos_w && scale_factor && inlier_out), OVS_ERR_INVALID_ARG, "null argument");
     for (int i = 0; i < n_all; ++i) {
@@ -3061,36 +3018,26 @@ extern "C" int ovs_pnp_solve_ransac_host(ovs_optimizer* h, int B, const int32_t*
     invalidate_plan(h);
     if (h->pending) { OVS_CUDA_CHECK(ovs::sync_stream(h->stream)); h->pending = false; }
     const size_t N = (size_t)n_all, NB = (size_t)B, H = (size_t)max_num_iter;
-    const size_t in_bytes_max = 256 * 7 + (NB + 1) * 4 + N * (24 + 24 + 4) + NB * (8 + 8);
-    const size_t out_bytes_max = 256 * 5 + NB * (12 * 8 + 4 + 4 + 1) + N;
-    const size_t hbytes = in_bytes_max + out_bytes_max;
-    const size_t dbytes = hbytes + 256 * 3 + N * (8 + 4) + NB * H * 96 + 4096;
-    int rc = ensure_arenas(h, dbytes, hbytes);
-    if (rc != OVS_OK) return rc;
-    Arena Hh{h->h_arena, 0, h->h_cap}, D{h->d_arena, 0, h->d_cap};
-    // inputs: the same carving sequence in both arenas, so one contiguous copy moves them
-    int* hoff = Hh.take<int>(NB + 1);
-    double* hbear = Hh.take<double>(3 * N); double* hpw = Hh.take<double>(3 * N); float* hsf = Hh.take<float>(N);
-    uint64_t* hseed = Hh.take<uint64_t>(NB); unsigned long long* hkey = Hh.take<unsigned long long>(NB);
-    const size_t in_bytes = Hh.off;
-    // outputs: one contiguous copy back
-    double* hpose = Hh.take<double>(12 * NB);
-    const size_t out_begin = (size_t)((uint8_t*)hpose - h->h_arena);
-    int* hnum = Hh.take<int>(NB); int* hbest = Hh.take<int>(NB); uint8_t* hvalid = Hh.take<uint8_t>(NB); uint8_t* hflags = Hh.take<uint8_t>(N);
-    const size_t out_end = Hh.off;
     PnpArgs A;
     A.B = B; A.N = n_all; A.H = max_num_iter; A.min_num_inliers = min_num_inliers; A.recompute = recompute ? 1 : 0;
-    A.off = D.take<int>(NB + 1);
-    A.bear = D.take<double>(3 * N); A.pw = D.take<double>(3 * N); A.sf = D.take<float>(N);
-    A.seed = D.take<uint64_t>(NB); A.key = D.take<unsigned long long>(NB);
-    A.pose = D.take<double>(12 * NB); A.num_inliers = D.take<int>(NB); A.best_iter = D.take<int>(NB); A.valid = D.take<uint8_t>(NB);
-    A.inlier = D.take<uint8_t>(N);
-    A.bound = D.take<double>(N); A.cidx = D.take<int>(N); A.hyp = D.take<double>(12 * NB * H);
+    int* hoff; double *hbear, *hpw; float* hsf; uint64_t* hseed; unsigned long long* hkey;
+    double* hpose; int *hnum, *hbest; uint8_t *hvalid, *hflags;
+    ovs::Staging S;
+    rc = ovs::stage(S, h->h_arena, h->d_arena, [&](size_t hbytes, size_t dbytes) { return ensure_arenas(h, dbytes, hbytes); },
+                    [&](ovs::Staging& S) {
+        A.off = S.in(hoff, NB + 1);
+        A.bear = S.in(hbear, 3 * N); A.pw = S.in(hpw, 3 * N); A.sf = S.in(hsf, N);
+        A.seed = S.in(hseed, NB); A.key = S.in(hkey, NB);
+        A.pose = S.out(hpose, 12 * NB); A.num_inliers = S.out(hnum, NB); A.best_iter = S.out(hbest, NB); A.valid = S.out(hvalid, NB);
+        A.inlier = S.out(hflags, N);
+        A.bound = S.dev<double>(N); A.cidx = S.dev<int>(N); A.hyp = S.dev<double>(12 * NB * H);
+    });
+    if (rc != OVS_OK) return rc;
     memcpy(hoff, corr_offsets, 4 * (NB + 1));
     memcpy(hbear, bearings, 24 * N); memcpy(hpw, pos_w, 24 * N); memcpy(hsf, scale_factor, 4 * N);
     memcpy(hseed, seeds, 8 * NB); memset(hkey, 0, 8 * NB);
     cudaStream_t st = h->stream;
-    OVS_CUDA_CHECK(cudaMemcpyAsync(h->d_arena, h->h_arena, in_bytes, cudaMemcpyHostToDevice, st));
+    OVS_CUDA_CHECK(S.upload(st));
     const size_t hyp_threads = std::max(N, NB * H);
     k_pnp_hypotheses<<<(unsigned)((hyp_threads + kPnpHypThreads - 1) / kPnpHypThreads), kPnpHypThreads, 0, st>>>(A);
     OVS_LAUNCH_CHECK();
@@ -3100,7 +3047,7 @@ extern "C" int ovs_pnp_solve_ransac_host(ovs_optimizer* h, int B, const int32_t*
     }
     k_pnp_refine<<<B, kPnpRefineThreads, 0, st>>>(A);
     OVS_LAUNCH_CHECK();
-    OVS_CUDA_CHECK(cudaMemcpyAsync(h->h_arena + out_begin, h->d_arena + out_begin, out_end - out_begin, cudaMemcpyDeviceToHost, st));
+    OVS_CUDA_CHECK(S.download(st));
     OVS_CUDA_CHECK(ovs::sync_stream(st));
     memcpy(pose_cw, hpose, 12 * 8 * NB);
     memcpy(num_inliers, hnum, 4 * NB); memcpy(best_iter, hbest, 4 * NB); memcpy(valid, hvalid, NB);
@@ -3221,12 +3168,12 @@ int prepare_impl(ovs_optimizer* h, const ovs_camera* cam, int setup_is_mono, int
         pl.dfail = D.take<int>(kSpec); pl.dmaxdiag = D.take<double>(2); pl.dclk = D.take<long long>(192); pl.dnchunks = D.take<int>(2);
     };
     {
-        Arena H0{nullptr, 0, 0}, D0{nullptr, 0, 0};
+        Arena H0{nullptr, 0}, D0{nullptr, 0};
         carve1(H0, D0);
         const int rc = ensure_arenas(h, D0.off + 256, H0.off + 256);
         if (rc != OVS_OK) return rc;
     }
-    Arena H{h->h_arena, 0, h->h_cap}, D{h->d_arena, 0, h->d_cap};
+    Arena H{h->h_arena, 0}, D{h->d_arena, 0};
     carve1(H, D);
     pl.exec_cap = exec_cap;
     h->pending = true;
@@ -3299,12 +3246,12 @@ int prepare_impl(ovs_optimizer* h, const ovs_camera* cam, int setup_is_mono, int
         pl.dspart = W.take<double>(kSpec * pl.spart_stride); pl.dppart = W.take<double>(27 * max_dchunks);
     };
     {
-        Arena W0{nullptr, 0, 0};
+        Arena W0{nullptr, 0};
         carve2(W0);
         const int rc = ensure_work(h, W0.off + 256);
         if (rc != OVS_OK) return rc;
     }
-    Arena W{h->d_work, 0, h->w_cap};
+    Arena W{h->d_work, 0};
     carve2(W);
     pl.max_chunks = (int)max_chunks; pl.max_dchunks = (int)max_dchunks;
     OVS_CUDA_CHECK(cudaMemsetAsync(pl.dsegb, 0, 4 * (size_t)npairs, st));
@@ -4239,21 +4186,21 @@ extern "C" int ovs_graph_optimize_host(ovs_optimizer* h, int K, double* sim3_cw,
         dfail = D.take<int>(kSpec); dmaxdiag = D.take<double>(2);
     };
     {
-        Arena H0{nullptr, 0, 0}, D0{nullptr, 0, 0};
+        Arena H0{nullptr, 0}, D0{nullptr, 0};
         carve(H0, D0);
         int rc = ensure_arenas(h, D0.off + 256, H0.off + 256);
         if (rc != OVS_OK) return rc;
         if (run_lm) {
-            Arena W0{nullptr, 0, 0};
+            Arena W0{nullptr, 0};
             W0.take<double>(kSpec * ds.S_stride); W0.take<double>(kSpec * (size_t)nsys); W0.take<double>(kSpec * ds.invL_stride);
             rc = ensure_work(h, W0.off + 256);
             if (rc != OVS_OK) return rc;
         }
     }
-    Arena H{h->h_arena, 0, h->h_cap}, D{h->d_arena, 0, h->d_cap};
+    Arena H{h->h_arena, 0}, D{h->d_arena, 0};
     carve(H, D);
     if (run_lm) {
-        Arena W{h->d_work, 0, h->w_cap};
+        Arena W{h->d_work, 0};
         ds.S = W.take<double>(kSpec * ds.S_stride); ds.x = W.take<double>(kSpec * (size_t)nsys); ds.invL = W.take<double>(kSpec * ds.invL_stride);
         ds.fail = dfail; ds.clk = nullptr;
     }

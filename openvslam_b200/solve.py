@@ -5,12 +5,44 @@ homography and fundamental-matrix RANSAC, each solved on the GPU for a whole bat
 constructs one solver per problem; here each problem is a `problem` of flat arrays (see include/ovs_b200.h,
 ovs_*_solve_ransac_host, for the field-by-field mapping)."""
 import ctypes as C
+import itertools
+import types
 
 import numpy as np
 
 from . import _lib
 from .match import _matcher_handle
-from .optimize import Camera, _optimizer_handle, _p
+from .optimize import Camera, _optimizer_handle
+
+
+def _offsets(counts):
+    """(B + 1,) int32 offsets of B problems with these item counts"""
+    return np.fromiter(itertools.accumulate(counts, initial=0), np.int32, len(counts) + 1)
+
+
+def _batch(name, B, seeds, items, width):
+    """What a batched solver passes to the C ABI for B problems.
+
+    items: {kind: (B per-problem arrays, row shape, dtype)}.  Each kind gives off[kind], its (B + 1,) int32 offsets, and
+    cat[kind], the arrays as rows of that shape concatenated in problem order (one zero row when there is none, so that there
+    is a pointer to pass).  seeds: one per problem (default: the problem's index).  The outputs, zeroed, for at least one
+    problem: model (B, width), valid, num_inliers, best_iter and best_score per problem, flags per item of the first kind."""
+    off, cat = {}, {}
+    for kind, (arrays, row, dt) in items.items():
+        rows = [np.asarray(a, dt).reshape((-1,) + row) for a in arrays]
+        off[kind] = _offsets([len(r) for r in rows])
+        cat[kind] = np.concatenate(rows) if off[kind][-1] else np.zeros((1,) + row, dt)
+    seeds = np.arange(B, dtype=np.uint64) if seeds is None else np.ascontiguousarray(seeds, np.uint64).reshape(-1)
+    if len(seeds) != B:
+        raise ValueError(name + ": one seed per problem")
+    N, Bo = int(off[next(iter(items))][-1]), max(B, 1)
+    return types.SimpleNamespace(off=off, cat=cat, seeds=seeds if B else np.zeros(1, np.uint64), model=np.zeros((Bo, width)),
+                                 valid=np.zeros(Bo, np.uint8), num_inliers=np.zeros(Bo, np.int32), best_iter=np.zeros(Bo, np.int32),
+                                 best_score=np.zeros(Bo), flags=np.zeros(max(N, 1), np.uint8))
+
+
+def _vp(a):
+    return a.ctypes.data_as(C.c_void_p)
 
 
 class sim3_solver(_optimizer_handle):
@@ -32,39 +64,24 @@ class sim3_solver(_optimizer_handle):
 
     def find_via_ransac(self, problems, max_num_iter=200, seeds=None):
         B = len(problems)
-        counts = []
         for p in problems:
             n = len(np.asarray(p["sigma_sq_1"]).reshape(-1))
             if not (np.asarray(p["pos_w_1"]).size == np.asarray(p["pos_w_2"]).size == 3 * n and np.asarray(p["sigma_sq_2"]).size == n):
                 raise ValueError("sim3_solver: pos_w_1 / pos_w_2 need (n, 3) and sigma_sq_1 / sigma_sq_2 n entries")
-            counts.append(n)
-        off = np.zeros(B + 1, np.int32)
-        off[1:] = np.cumsum(counts)
-        N = int(off[-1])
-        seeds = np.arange(B, dtype=np.uint64) if seeds is None else np.asarray(seeds, np.uint64).reshape(-1)
-        if len(seeds) != B:
-            raise ValueError("sim3_solver: one seed per problem")
-        cams_1 = (Camera * max(B, 1))(*[p["cam_1"] for p in problems])
-        cams_2 = (Camera * max(B, 1))(*[p["cam_2"] for p in problems])
-
-        def cat(key, width, dt):
-            if N == 0:
-                return np.zeros((1, width) if width > 1 else 1, dt)
-            return np.concatenate([np.asarray(p[key], dt).reshape(-1, width) if width > 1 else np.asarray(p[key], dt).reshape(-1)
-                                   for p in problems])
-        pose1, pp1 = _p(np.concatenate([np.asarray(p["pose_1w"], np.float64).reshape(12) for p in problems]) if B else np.zeros(12), np.float64)
-        pose2, pp2 = _p(np.concatenate([np.asarray(p["pose_2w"], np.float64).reshape(12) for p in problems]) if B else np.zeros(12), np.float64)
-        w1, pw1 = _p(cat("pos_w_1", 3, np.float64), np.float64); s1, ps1 = _p(cat("sigma_sq_1", 1, np.float32), np.float32)
-        w2, pw2 = _p(cat("pos_w_2", 3, np.float64), np.float64); s2, ps2 = _p(cat("sigma_sq_2", 1, np.float32), np.float32)
-        off_, po = _p(off, np.int32); seeds_, pseed = _p(seeds if B else np.zeros(1, np.uint64), np.uint64)
-        S = np.zeros((max(B, 1), 13)); valid = np.zeros(max(B, 1), np.uint8)
-        ninl = np.zeros(max(B, 1), np.int32); best = np.zeros(max(B, 1), np.int32); flags = np.zeros(max(N, 1), np.uint8)
-        vp = lambda a: a.ctypes.data_as(C.c_void_p)
-        _lib.check(_lib.lib().ovs_sim3_solve_ransac_host(self._h, B, po, cams_1, pp1, cams_2, pp2, pw1, ps1, pw2, ps2, int(self.fix_scale_),
-                                                         self.min_num_inliers_, int(max_num_iter), pseed, vp(S), vp(valid), vp(ninl), vp(best),
-                                                         vp(flags)))
-        return [dict(valid=bool(valid[b]), sim3_12=S[b].copy(), num_inliers=int(ninl[b]), best_iter=int(best[b]),
-                     inliers=flags[off[b]:off[b + 1]].astype(bool)) for b in range(B)]
+        col = lambda key: [p[key] for p in problems]
+        t = _batch("sim3_solver", B, seeds, {"pos_w_1": (col("pos_w_1"), (3,), np.float64), "sigma_sq_1": (col("sigma_sq_1"), (), np.float32),
+                                             "pos_w_2": (col("pos_w_2"), (3,), np.float64), "sigma_sq_2": (col("sigma_sq_2"), (), np.float32)}, 13)
+        cams_1 = (Camera * max(B, 1))(*col("cam_1"))
+        cams_2 = (Camera * max(B, 1))(*col("cam_2"))
+        pose1, pose2 = (np.concatenate([np.asarray(p[k], np.float64).reshape(12) for p in problems]) if B else np.zeros(12)
+                        for k in ("pose_1w", "pose_2w"))
+        c, off = t.cat, t.off["pos_w_1"]
+        _lib.check(_lib.lib().ovs_sim3_solve_ransac_host(self._h, B, _vp(off), cams_1, _vp(pose1), cams_2, _vp(pose2),
+                                                         _vp(c["pos_w_1"]), _vp(c["sigma_sq_1"]), _vp(c["pos_w_2"]), _vp(c["sigma_sq_2"]),
+                                                         int(self.fix_scale_), self.min_num_inliers_, int(max_num_iter), _vp(t.seeds),
+                                                         _vp(t.model), _vp(t.valid), _vp(t.num_inliers), _vp(t.best_iter), _vp(t.flags)))
+        return [dict(valid=bool(t.valid[b]), sim3_12=t.model[b].copy(), num_inliers=int(t.num_inliers[b]), best_iter=int(t.best_iter[b]),
+                     inliers=t.flags[off[b]:off[b + 1]].astype(bool)) for b in range(B)]
 
 
 class pnp_solver(_optimizer_handle):
@@ -84,34 +101,19 @@ class pnp_solver(_optimizer_handle):
 
     def find_via_ransac(self, problems, max_num_iter=30, recompute=True, seeds=None):
         B = len(problems)
-        counts = []
         for p in problems:
             n = len(np.asarray(p["scale_factor"]).reshape(-1))
             if not (np.asarray(p["bearings"]).size == np.asarray(p["pos_w"]).size == 3 * n):
                 raise ValueError("pnp_solver: bearings / pos_w need (n, 3) and scale_factor n entries")
-            counts.append(n)
-        off = np.zeros(B + 1, np.int32)
-        off[1:] = np.cumsum(counts)
-        N = int(off[-1])
-        seeds = np.arange(B, dtype=np.uint64) if seeds is None else np.asarray(seeds, np.uint64).reshape(-1)
-        if len(seeds) != B:
-            raise ValueError("pnp_solver: one seed per problem")
-
-        def cat(key, width, dt):
-            if N == 0:
-                return np.zeros((1, width) if width > 1 else 1, dt)
-            return np.concatenate([np.asarray(p[key], dt).reshape(-1, width) if width > 1 else np.asarray(p[key], dt).reshape(-1)
-                                   for p in problems])
-        b, pb = _p(cat("bearings", 3, np.float64), np.float64); w, pw = _p(cat("pos_w", 3, np.float64), np.float64)
-        s, ps = _p(cat("scale_factor", 1, np.float32), np.float32)
-        off_, po = _p(off, np.int32); seeds_, pseed = _p(seeds if B else np.zeros(1, np.uint64), np.uint64)
-        pose = np.zeros((max(B, 1), 12)); valid = np.zeros(max(B, 1), np.uint8)
-        ninl = np.zeros(max(B, 1), np.int32); best = np.zeros(max(B, 1), np.int32); flags = np.zeros(max(N, 1), np.uint8)
-        vp = lambda a: a.ctypes.data_as(C.c_void_p)
-        _lib.check(_lib.lib().ovs_pnp_solve_ransac_host(self._h, B, po, pb, pw, ps, self.min_num_inliers_, int(max_num_iter),
-                                                        int(bool(recompute)), pseed, vp(pose), vp(valid), vp(ninl), vp(best), vp(flags)))
-        return [dict(valid=bool(valid[b]), pose_cw=pose[b].copy(), num_inliers=int(ninl[b]), best_iter=int(best[b]),
-                     inliers=flags[off[b]:off[b + 1]].astype(bool)) for b in range(B)]
+        col = lambda key: [p[key] for p in problems]
+        t = _batch("pnp_solver", B, seeds, {"bearings": (col("bearings"), (3,), np.float64), "pos_w": (col("pos_w"), (3,), np.float64),
+                                            "scale_factor": (col("scale_factor"), (), np.float32)}, 12)
+        c, off = t.cat, t.off["bearings"]
+        _lib.check(_lib.lib().ovs_pnp_solve_ransac_host(self._h, B, _vp(off), _vp(c["bearings"]), _vp(c["pos_w"]), _vp(c["scale_factor"]),
+                                                        self.min_num_inliers_, int(max_num_iter), int(bool(recompute)), _vp(t.seeds),
+                                                        _vp(t.model), _vp(t.valid), _vp(t.num_inliers), _vp(t.best_iter), _vp(t.flags)))
+        return [dict(valid=bool(t.valid[b]), pose_cw=t.model[b].copy(), num_inliers=int(t.num_inliers[b]), best_iter=int(t.best_iter[b]),
+                     inliers=t.flags[off[b]:off[b + 1]].astype(bool)) for b in range(B)]
 
 
 class essential_solver(_matcher_handle):
@@ -127,32 +129,18 @@ class essential_solver(_matcher_handle):
 
     def find_via_ransac(self, problems, max_num_iter, recompute=True, seeds=None):
         B = len(problems)
-        counts = []
         for p in problems:
             n = np.asarray(p["bearings_1"]).size // 3
             if not (np.asarray(p["bearings_1"]).size == np.asarray(p["bearings_2"]).size == 3 * n):
                 raise ValueError("essential_solver: bearings_1 / bearings_2 need (n, 3) each")
-            counts.append(n)
-        off = np.zeros(B + 1, np.int32)
-        off[1:] = np.cumsum(counts)
-        N = int(off[-1])
-        seeds = np.arange(B, dtype=np.uint64) if seeds is None else np.asarray(seeds, np.uint64).reshape(-1)
-        if len(seeds) != B:
-            raise ValueError("essential_solver: one seed per problem")
-
-        def cat(key):
-            if N == 0:
-                return np.zeros((1, 3))
-            return np.concatenate([np.asarray(p[key], np.float64).reshape(-1, 3) for p in problems])
-        b1, pb1 = _p(cat("bearings_1"), np.float64); b2, pb2 = _p(cat("bearings_2"), np.float64)
-        off_, po = _p(off, np.int32); seeds_, pseed = _p(seeds if B else np.zeros(1, np.uint64), np.uint64)
-        E = np.zeros((max(B, 1), 9)); valid = np.zeros(max(B, 1), np.uint8); score = np.zeros(max(B, 1))
-        ninl = np.zeros(max(B, 1), np.int32); best = np.zeros(max(B, 1), np.int32); flags = np.zeros(max(N, 1), np.uint8)
-        vp = lambda a: a.ctypes.data_as(C.c_void_p)
-        _lib.check(_lib.lib().ovs_essential_solve_ransac_host(self._h, B, po, pb1, pb2, int(max_num_iter), int(bool(recompute)), pseed,
-                                                              vp(E), vp(valid), vp(ninl), vp(best), vp(score), vp(flags)))
-        return [dict(valid=bool(valid[b]), E_21=E[b].reshape(3, 3).copy(), num_inliers=int(ninl[b]), best_iter=int(best[b]),
-                     best_score=float(score[b]), inliers=flags[off[b]:off[b + 1]].astype(bool)) for b in range(B)]
+        t = _batch("essential_solver", B, seeds, {k: ([p[k] for p in problems], (3,), np.float64) for k in ("bearings_1", "bearings_2")}, 9)
+        off = t.off["bearings_1"]
+        _lib.check(_lib.lib().ovs_essential_solve_ransac_host(self._h, B, _vp(off), _vp(t.cat["bearings_1"]), _vp(t.cat["bearings_2"]),
+                                                              int(max_num_iter), int(bool(recompute)), _vp(t.seeds), _vp(t.model), _vp(t.valid),
+                                                              _vp(t.num_inliers), _vp(t.best_iter), _vp(t.best_score), _vp(t.flags)))
+        return [dict(valid=bool(t.valid[b]), E_21=t.model[b].reshape(3, 3).copy(), num_inliers=int(t.num_inliers[b]),
+                     best_iter=int(t.best_iter[b]), best_score=float(t.best_score[b]), inliers=t.flags[off[b]:off[b + 1]].astype(bool))
+                for b in range(B)]
 
 
 # cv::KeyPoint / ovs_keypoint (28 bytes): the two-view solvers read pt only
@@ -171,40 +159,27 @@ class _two_view_solver(_matcher_handle):
     def find_via_ransac(self, problems, max_num_iter, recompute=True, seeds=None):
         name = type(self).__name__
         B = len(problems)
-        kp1, kp2, mt = [], [], []
         for p in problems:
-            k1 = np.asarray(p["keypts_1"], np.float32); k2 = np.asarray(p["keypts_2"], np.float32)
-            m = np.asarray(p["matches_12"]).reshape(-1, 2) if np.asarray(p["matches_12"]).size else np.zeros((0, 2), np.int32)
-            if k1.size % 2 or k2.size % 2:
+            if np.size(p["keypts_1"]) % 2 or np.size(p["keypts_2"]) % 2:
                 raise ValueError(name + ": keypts_1 / keypts_2 need (n, 2) each")
-            kp1.append(k1.reshape(-1, 2)); kp2.append(k2.reshape(-1, 2)); mt.append(m.astype(np.int32))
+        t = _batch(name, B, seeds, {"matches_12": ([p["matches_12"] for p in problems], (2,), np.int32)}, 9)
 
-        def offsets(arrs):
-            off = np.zeros(B + 1, np.int32)
-            off[1:] = np.cumsum([len(a) for a in arrs])
-            return off
-        koff1, koff2, moff = offsets(kp1), offsets(kp2), offsets(mt)
-        N = int(moff[-1])
-        seeds = np.arange(B, dtype=np.uint64) if seeds is None else np.asarray(seeds, np.uint64).reshape(-1)
-        if len(seeds) != B:
-            raise ValueError(name + ": one seed per problem")
-
-        def keypoints(arrs):
-            xy = np.concatenate(arrs) if B and sum(len(a) for a in arrs) else np.zeros((0, 2), np.float32)
-            out = np.zeros(max(len(xy), 1), _KEYPOINT)
-            out["x"][:len(xy)] = xy[:, 0]; out["y"][:len(xy)] = xy[:, 1]
-            return out
-        k1, k2 = keypoints(kp1), keypoints(kp2)
-        m, pm = _p(np.concatenate(mt) if N else np.zeros((1, 2), np.int32), np.int32)
-        o1, po1 = _p(koff1, np.int32); o2, po2 = _p(koff2, np.int32); om, pom = _p(moff, np.int32)
-        seeds_, pseed = _p(seeds if B else np.zeros(1, np.uint64), np.uint64)
-        M = np.zeros((max(B, 1), 9)); valid = np.zeros(max(B, 1), np.uint8); score = np.zeros(max(B, 1))
-        ninl = np.zeros(max(B, 1), np.int32); best = np.zeros(max(B, 1), np.int32); flags = np.zeros(max(N, 1), np.uint8)
-        vp = lambda a: a.ctypes.data_as(C.c_void_p)
-        _lib.check(getattr(_lib.lib(), self._entry)(self._h, B, po1, vp(k1), po2, vp(k2), pom, pm, C.c_float(self.sigma_), int(max_num_iter),
-                                                    int(bool(recompute)), pseed, vp(M), vp(valid), vp(ninl), vp(best), vp(score), vp(flags)))
-        return [{"valid": bool(valid[b]), self._key: M[b].reshape(3, 3).copy(), "num_inliers": int(ninl[b]), "best_iter": int(best[b]),
-                 "best_score": float(score[b]), "inliers": flags[moff[b]:moff[b + 1]].astype(bool)} for b in range(B)]
+        def keypoints(key):
+            # the records are filled from each view's x, y, so the float copy of all keypoints is never formed
+            arrs = [np.asarray(p[key], np.float32).reshape(-1, 2) for p in problems]
+            off = _offsets([len(a) for a in arrs])
+            out = np.zeros(max(int(off[-1]), 1), _KEYPOINT)
+            for a, o in zip(arrs, off):
+                out["x"][o:o + len(a)] = a[:, 0]; out["y"][o:o + len(a)] = a[:, 1]
+            return off, out
+        (o1, k1), (o2, k2), moff = keypoints("keypts_1"), keypoints("keypts_2"), t.off["matches_12"]
+        _lib.check(getattr(_lib.lib(), self._entry)(self._h, B, _vp(o1), _vp(k1), _vp(o2), _vp(k2), _vp(moff),
+                                                    _vp(t.cat["matches_12"]), C.c_float(self.sigma_), int(max_num_iter), int(bool(recompute)),
+                                                    _vp(t.seeds), _vp(t.model), _vp(t.valid), _vp(t.num_inliers), _vp(t.best_iter),
+                                                    _vp(t.best_score), _vp(t.flags)))
+        return [{"valid": bool(t.valid[b]), self._key: t.model[b].reshape(3, 3).copy(), "num_inliers": int(t.num_inliers[b]),
+                 "best_iter": int(t.best_iter[b]), "best_score": float(t.best_score[b]), "inliers": t.flags[moff[b]:moff[b + 1]].astype(bool)}
+                for b in range(B)]
 
 
 class homography_solver(_two_view_solver):

@@ -1,5 +1,5 @@
-"""solve::essential_solver and match::robust::match_frame_and_keyframe on the GPU (k_essential_hypotheses + k_essential_score +
-k_essential_refine: three launches per batch) against the oracle (oracle/essential_solver_oracle.c) and ground truth.  The kernels
+"""solve::essential_solver and match::robust::match_frame_and_keyframe on the GPU (k_two_view_hypotheses + k_two_view_score +
+k_two_view_refine instantiated for EssentialModel: three launches per batch) against the oracle (oracle/essential_solver_oracle.c) and ground truth.  The kernels
 give every hypothesis one thread for the eight-point E and then a warp whose lanes take the matches with a stride of 32, put 4
 hypotheses in a CTA, and recompute with one 256-thread CTA per problem whose sums take 256 strided partials; the sizes below sit
 around those strides."""
@@ -104,6 +104,20 @@ def test_batch_equals_single_calls_and_oracle(es, recompute, max_iter):
         n = len(p["bearings_1"])
         if n < 8 or max_iter == 0:
             assert not g[b]["valid"] and g[b]["best_iter"] == -1 and not g[b]["E_21"].any()
+
+
+@pytest.mark.parametrize("view", ["strided", "reversed"])
+def test_seeds_given_as_a_view_equal_their_contiguous_copy(view):
+    """seeds may be any 1-D array: a strided or reversed view gives the result of its values, not of the memory it starts at"""
+    probs = [ep.problem(300, model=m, wrong=0.4, noise=1e-3, seed=60 + k) for k, m in enumerate(["perspective", "equirectangular"] * 2)]
+    base = np.arange(100, 100 + 2 * len(probs), dtype=np.uint64)
+    seeds = base[::2] if view == "strided" else base[len(probs):][::-1]
+    g = _solve(probs, 50, True, seeds)
+    for x, y in zip(g, _solve(probs, 50, True, np.array(seeds))):
+        _same(x, y)
+    if view == "strided":   # the seeds make a difference here: reading the view's memory as if contiguous would be seen
+        assert any(x["best_iter"] != y["best_iter"] or not np.array_equal(x["inliers"], y["inliers"])
+                   for x, y in zip(g, _solve(probs, 50, True, base[:len(probs)])))
 
 
 def test_repeated_calls_are_bit_identical():
