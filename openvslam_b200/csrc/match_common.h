@@ -1,8 +1,10 @@
-// match_common.h -- the matcher handle shared by match_bruteforce.cu and match_window.cu.
+// match_common.h -- the matcher handle shared by match_bruteforce.cu, match_window.cu and two_view_ransac.cu.  Its arenas
+// grow and are carved through staging.h.
 #pragma once
 #include <algorithm>
 #include <vector>
 #include "ovs_common.h"
+#include "staging.h"
 
 // device buffer of a released frame index, kept for the next ovs_frame_index_create* (one per frame in a tracking loop:
 // cudaMalloc / cudaFree per frame would serialise every stream of the device)
@@ -31,27 +33,3 @@ struct ovs_matcher {
     int num_requeries = 0;   // GPU re-queries issued by the greedy replays so far (diagnostic)
     std::vector<ovs_index_buf> index_pool;
 };
-
-namespace ovs {
-
-template <typename T>
-int grow_dev(T** p, size_t* cap, size_t need) {
-    if (need <= *cap) return OVS_OK;
-    cudaFree(*p); *p = nullptr; *cap = 0;
-    // a quarter of slack: the number of keypoints creeps from frame to frame, and every cudaFree / cudaMalloc stalls all streams of the device
-    const size_t n = std::max(need + need / 4, (size_t)4096);
-    OVS_CUDA_CHECK(cudaMalloc(p, n * sizeof(T)));
-    *cap = n;
-    return OVS_OK;
-}
-template <typename T>
-int grow_host(T** p, size_t* cap, size_t need) {
-    if (need <= *cap) return OVS_OK;
-    cudaFreeHost(*p); *p = nullptr; *cap = 0;
-    const size_t n = std::max(need + need / 4, (size_t)4096);
-    OVS_CUDA_CHECK(cudaHostAlloc(p, n * sizeof(T), cudaHostAllocDefault));
-    *cap = n;
-    return OVS_OK;
-}
-
-}  // namespace ovs

@@ -277,29 +277,27 @@ int window_topk(ovs_frame_index* f, int nq, const float* ref_xy, const float* ma
     ovs_matcher* m = f->m;
     cudaStream_t st = m->stream;
     const size_t N = (size_t)nq;
-    const size_t bytes = N * (8 + 4 + 4 + 4 + 4 + 32) + 512;
-    int rc;
-    if ((rc = ovs::grow_host(&m->h_stage, &m->h_stage_cap, bytes)) != OVS_OK) return rc;
-    if ((rc = ovs::grow_dev(&m->d_q, &m->d_q_cap, bytes)) != OVS_OK) return rc;
+    WindowQueries Q;
+    uint8_t* hdesc; float2* href; float *hm, *hxr; int *hlo, *hhi; float* dxr;
+    ovs::Staging S;
+    int rc = ovs::stage(S, m->h_stage, m->h_stage_cap, m->d_q, m->d_q_cap, [&](ovs::Staging& S) {
+        Q.desc = (const uint4*)S.in(hdesc, 32 * N); Q.ref = S.in(href, N); Q.margin = S.in(hm, N);
+        Q.min_level = S.in(hlo, N); Q.max_level = S.in(hhi, N); dxr = S.in(hxr, N);
+    });
+    if (rc != OVS_OK) return rc;
     if ((rc = ovs::grow_dev(&m->d_keys, &m->d_keys_cap, (N + 1) * kTopK)) != OVS_OK) return rc;
     if ((rc = ovs::grow_host(&m->h_keys, &m->h_keys_cap, (N + 1) * kTopK)) != OVS_OK) return rc;
-    // carve: desc (32 N, 16-aligned first), ref (8 N), margin, min, max, xr (4 N each)
-    size_t off = 0;
-    auto carve = [&](size_t b) { const size_t o = off; off += (b + 15) / 16 * 16; return o; };
-    const size_t o_desc = carve(32 * N), o_ref = carve(8 * N), o_m = carve(4 * N), o_lo = carve(4 * N), o_hi = carve(4 * N), o_xr = carve(4 * N);
-    memcpy(m->h_stage + o_desc, qdesc, 32 * N); memcpy(m->h_stage + o_ref, ref_xy, 8 * N); memcpy(m->h_stage + o_m, margin, 4 * N);
-    memcpy(m->h_stage + o_lo, min_level, 4 * N); memcpy(m->h_stage + o_hi, max_level, 4 * N);
-    if (xr_q) memcpy(m->h_stage + o_xr, xr_q, 4 * N);
-    OVS_CUDA_CHECK(cudaMemcpyAsync(m->d_q, m->h_stage, off, cudaMemcpyHostToDevice, st));
+    memcpy(hdesc, qdesc, 32 * N); memcpy(href, ref_xy, 8 * N); memcpy(hm, margin, 4 * N);
+    memcpy(hlo, min_level, 4 * N); memcpy(hhi, max_level, 4 * N);
+    if (xr_q) memcpy(hxr, xr_q, 4 * N);
+    OVS_CUDA_CHECK(S.upload(st));
     if (cap_rank_order) OVS_CUDA_CHECK(cudaMemcpyAsync(f->d_cap, cap_rank_order, 2 * (size_t)std::max(f->nranked, 1), cudaMemcpyHostToDevice, st));
     WindowFrame F;
     F.min_x = f->grid.min_x; F.min_y = f->grid.min_y; F.inv_w = f->grid.inv_cell_width; F.inv_h = f->grid.inv_cell_height;
     F.cols = f->grid.num_grid_cols; F.rows = f->grid.num_grid_rows;
     F.x = f->d_x; F.y = f->d_y; F.xr = f->has_xr ? f->d_xr : nullptr; F.oct = f->d_oct; F.desc = f->d_desc;
     F.cell_start = f->d_cell_start; F.cap = cap_rank_order ? f->d_cap : nullptr;
-    WindowQueries Q;
-    Q.nq = nq; Q.desc = (const uint4*)(m->d_q + o_desc); Q.ref = (const float2*)(m->d_q + o_ref); Q.margin = (const float*)(m->d_q + o_m);
-    Q.min_level = (const int*)(m->d_q + o_lo); Q.max_level = (const int*)(m->d_q + o_hi); Q.xr = xr_q ? (const float*)(m->d_q + o_xr) : nullptr;
+    Q.nq = nq; Q.xr = xr_q ? dxr : nullptr;
     Q.fuse_gate = fuse_inv_sigma_sq ? 1 : 0;
     for (int l = 0; l < 16; ++l) Q.inv_sigma_sq[l] = (fuse_inv_sigma_sq && l < fuse_levels) ? fuse_inv_sigma_sq[l] : 0.0f;
     OVS_CUDA_CHECK(cudaEventRecord(m->ev[0], st));
@@ -367,9 +365,14 @@ std::vector<int> rank_keypoints(ovs_frame_index* f) {
 }
 
 bool alloc_index_arrays(ovs_frame_index* f, size_t R, int ncells) {
-    auto up = [](size_t b) { return (b + 255) / 256 * 256; };
-    const size_t o_desc = 0, o_x = o_desc + up(R * 32), o_y = o_x + up(R * 4), o_xr = o_y + up(R * 4), o_rank = o_xr + up(R * 4),
-                 o_cell = o_rank + up(R * 4), o_cap = o_cell + up((size_t)(ncells + 1) * 4), o_oct = o_cap + up(R * 2), need = o_oct + up(R);
+    auto carve = [&](ovs::Arena& A) {
+        f->d_desc = A.take<uint4>(2 * R); f->d_x = A.take<float>(R); f->d_y = A.take<float>(R); f->d_xr = A.take<float>(R);
+        f->d_rank = A.take<int>(R); f->d_cell_start = A.take<int>((size_t)ncells + 1); f->d_cap = A.take<unsigned short>(R);
+        f->d_oct = A.take<signed char>(R);
+    };
+    ovs::Arena A{nullptr, 0};
+    carve(A);
+    const size_t need = A.off;
     ovs_matcher* m = f->m;
     int pick = -1;
     for (int i = 0; i < (int)m->index_pool.size(); ++i)
@@ -382,10 +385,8 @@ bool alloc_index_arrays(ovs_frame_index* f, size_t R, int ncells) {
         if (cudaMalloc(&f->buf.base, cap) != cudaSuccess) { f->buf = ovs_index_buf(); return false; }
         f->buf.cap = cap;
     }
-    uint8_t* b = f->buf.base;
-    f->d_desc = reinterpret_cast<uint4*>(b + o_desc); f->d_x = reinterpret_cast<float*>(b + o_x); f->d_y = reinterpret_cast<float*>(b + o_y);
-    f->d_xr = reinterpret_cast<float*>(b + o_xr); f->d_rank = reinterpret_cast<int*>(b + o_rank); f->d_cell_start = reinterpret_cast<int*>(b + o_cell);
-    f->d_cap = reinterpret_cast<unsigned short*>(b + o_cap); f->d_oct = reinterpret_cast<signed char*>(b + o_oct);
+    A = ovs::Arena{f->buf.base, 0};
+    carve(A);
     return true;
 }
 
@@ -461,10 +462,14 @@ extern "C" int ovs_frame_index_create_device(ovs_matcher* m, int n, const ovs_ke
     OVS_CUDA_CHECK(cudaSetDevice(m->device));
     cudaStream_t st = m->stream;
     const size_t N = (size_t)std::max(n, 1);
-    int rc = ovs::grow_host(&m->h_stage, &m->h_stage_cap, N * (sizeof(ovs_keypoint) + 4) + 64);
+    ovs_keypoint* hk; float* hxr;
+    auto carve = [&](ovs::Arena& H) { hk = H.take<ovs_keypoint>(N); hxr = H.take<float>(N); };
+    ovs::Arena H{nullptr, 0};
+    carve(H);
+    const int rc = ovs::grow_host(&m->h_stage, &m->h_stage_cap, H.off);
     if (rc != OVS_OK) return rc;
-    ovs_keypoint* hk = reinterpret_cast<ovs_keypoint*>(m->h_stage);
-    float* hxr = reinterpret_cast<float*>(m->h_stage + N * sizeof(ovs_keypoint));
+    H = ovs::Arena{m->h_stage, 0};
+    carve(H);
     if (n) OVS_CUDA_CHECK(cudaMemcpyAsync(hk, d_keypts, (size_t)n * sizeof(ovs_keypoint), cudaMemcpyDeviceToHost, st));
     if (n && d_x_right) OVS_CUDA_CHECK(cudaMemcpyAsync(hxr, d_x_right, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
     OVS_CUDA_CHECK(ovs::sync_stream(st));
@@ -940,38 +945,34 @@ extern "C" int ovs_stereo_compute_host(ovs_matcher* m, const ovs_extractor* left
     for (int i = 0; i < n_left; ++i) OVS_REQUIRE(loct[i] >= 0 && loct[i] < L, OVS_ERR_INVALID_ARG, "left octave out of range");
     for (int i = 0; i < n_right; ++i) OVS_REQUIRE(roct[i] >= 0 && roct[i] < L, OVS_ERR_INVALID_ARG, "right octave out of range");
     const size_t NL = (size_t)n_left, NR = (size_t)n_right;
-    size_t off = 0;
-    auto carve = [&](size_t b) { const size_t o = off; off += (b + 15) / 16 * 16; return o; };
-    const size_t o_ld = carve(32 * NL), o_rd = carve(32 * NR), o_lx = carve(4 * NL), o_ly = carve(4 * NL), o_lo = carve(4 * NL),
-                 o_rx = carve(4 * NR), o_ry = carve(4 * NR), o_ro = carve(4 * NR);
-    const size_t in_bytes = off;
-    const size_t o_best = carve(4 * NL), o_xr = carve(4 * NL), o_dp = carve(4 * NL), o_co = carve(4 * NL);
-    if ((rc = ovs::grow_host(&m->h_stage, &m->h_stage_cap, off)) != OVS_OK) return rc;
-    if ((rc = ovs::grow_dev(&m->d_t, &m->d_t_cap, off)) != OVS_OK) return rc;
-    uint8_t* hs = m->h_stage; uint8_t* ds = m->d_t;
-    memcpy(hs + o_ld, ldesc, 32 * NL); memcpy(hs + o_rd, rdesc, 32 * NR);
-    memcpy(hs + o_lx, lx, 4 * NL); memcpy(hs + o_ly, ly, 4 * NL); memcpy(hs + o_lo, loct, 4 * NL);
-    memcpy(hs + o_rx, rx, 4 * NR); memcpy(hs + o_ry, ry, 4 * NR); memcpy(hs + o_ro, roct, 4 * NR);
+    uint8_t *hld, *hrd; float *hlx, *hly, *hrx, *hry, *hxr, *hdp, *dxr, *ddp; int *hlo, *hro; unsigned *hco, *dco, *dbest;
+    ovs::Staging S;
+    rc = ovs::stage(S, m->h_stage, m->h_stage_cap, m->d_t, m->d_t_cap, [&](ovs::Staging& S) {
+        A.ldesc = (const uint4*)S.in(hld, 32 * NL); A.rdesc = (const uint4*)S.in(hrd, 32 * NR);
+        A.lx = S.in(hlx, NL); A.ly = S.in(hly, NL); A.loct = S.in(hlo, NL); A.rx = S.in(hrx, NR); A.ry = S.in(hry, NR); A.roct = S.in(hro, NR);
+        dxr = S.out(hxr, NL); ddp = S.out(hdp, NL); dco = S.out(hco, NL);
+        dbest = S.dev<unsigned>(NL);
+    });
+    if (rc != OVS_OK) return rc;
+    memcpy(hld, ldesc, 32 * NL); memcpy(hrd, rdesc, 32 * NR);
+    memcpy(hlx, lx, 4 * NL); memcpy(hly, ly, 4 * NL); memcpy(hlo, loct, 4 * NL);
+    memcpy(hrx, rx, 4 * NR); memcpy(hry, ry, 4 * NR); memcpy(hro, roct, 4 * NR);
     cudaStream_t st = m->stream;
-    OVS_CUDA_CHECK(cudaMemcpyAsync(ds, hs, in_bytes, cudaMemcpyHostToDevice, st));
+    OVS_CUDA_CHECK(S.upload(st));
     A.n_left = n_left; A.n_right = n_right;
-    A.ldesc = (const uint4*)(ds + o_ld); A.rdesc = (const uint4*)(ds + o_rd);
-    A.lx = (const float*)(ds + o_lx); A.ly = (const float*)(ds + o_ly); A.loct = (const int*)(ds + o_lo);
-    A.rx = (const float*)(ds + o_rx); A.ry = (const float*)(ds + o_ry); A.roct = (const int*)(ds + o_ro);
     A.min_disp = 0.0f; A.max_disp = focal_x_baseline / true_baseline;
     A.hamm_thr = (OVS_HAMMING_DIST_THR_HIGH + OVS_HAMMING_DIST_THR_LOW) / 2;
     A.rows0 = A.ph[0]; A.focal_x_baseline = focal_x_baseline;
     OVS_CUDA_CHECK(cudaEventRecord(m->ev[0], st));
-    k_stereo_match<<<(n_left + 127) / 128, 128, 0, st>>>(A, (unsigned*)(ds + o_best));
+    k_stereo_match<<<(n_left + 127) / 128, 128, 0, st>>>(A, dbest);
     OVS_LAUNCH_CHECK();
-    k_stereo_subpixel<<<(n_left + 3) / 4, 128, 0, st>>>(A, (const unsigned*)(ds + o_best), (float*)(ds + o_xr), (float*)(ds + o_dp), (unsigned*)(ds + o_co));
+    k_stereo_subpixel<<<(n_left + 3) / 4, 128, 0, st>>>(A, dbest, dxr, ddp, dco);
     OVS_LAUNCH_CHECK();
     OVS_CUDA_CHECK(cudaEventRecord(m->ev[1], st));
-    OVS_CUDA_CHECK(cudaMemcpyAsync(hs + o_xr, ds + o_xr, (o_co + 4 * NL) - o_xr, cudaMemcpyDeviceToHost, st));
+    OVS_CUDA_CHECK(S.download(st));
     OVS_CUDA_CHECK(ovs::sync_stream(st));
     float ms = 0; cudaEventElapsedTime(&ms, m->ev[0], m->ev[1]);
     m->last_kernel_us = ms * 1000.f;
-    const float* hxr = (const float*)(hs + o_xr); const float* hdp = (const float*)(hs + o_dp); const unsigned* hco = (const unsigned*)(hs + o_co);
     // median test on the SAD of the accepted matches (sorted (correlation, idx_left) pairs)
     std::vector<std::pair<unsigned, int>> corr;
     for (int i = 0; i < n_left; ++i) {
@@ -1126,39 +1127,36 @@ extern "C" int ovs_robust_match_for_triangulation_host(ovs_matcher* m, int n1, c
             seg[k] = make_int2((int)lo, (int)hi);
         }
     }
-    // staging layout (host pinned / device), widest alignment first:
-    // [qdesc 32Q][tdesc 32R][qbearing 24Q][tbearing 24R][qseg 8Q][qscale 4Q][qstereo Q][tstereo R][taken R]
-    const size_t o_qd = 0, o_td = o_qd + 32 * (size_t)Q, o_qb = o_td + 32 * (size_t)R, o_tb = o_qb + 24 * (size_t)Q, o_sg = o_tb + 24 * (size_t)R,
-                 o_qs = o_sg + 8 * (size_t)Q, o_q8 = o_qs + 4 * (size_t)Q, o_t8 = o_q8 + (size_t)Q, in_total = ((o_t8 + (size_t)R + 15) / 16) * 16,
-                 o_tk = in_total, total = ((o_tk + (size_t)R + 15) / 16) * 16;
-    int rc;
-    if ((rc = ovs::grow_host(&m->h_stage, &m->h_stage_cap, total)) != OVS_OK) return rc;
-    if ((rc = ovs::grow_dev(&m->d_q, &m->d_q_cap, total)) != OVS_OK) return rc;
+    const size_t sQ = (size_t)Q, sR = (size_t)R;
+    TriArgs A{};
+    uint8_t *hqd, *htd, *hq8, *ht8, *taken, *dtaken; double *hqb, *htb; int2* hsg; float* hqs;
+    ovs::Staging S;
+    int rc = ovs::stage(S, m->h_stage, m->h_stage_cap, m->d_q, m->d_q_cap, [&](ovs::Staging& S) {
+        A.qdesc = (const uint4*)S.in(hqd, 32 * sQ); A.tdesc = (const uint4*)S.in(htd, 32 * sR);
+        A.qbearing = S.in(hqb, 3 * sQ); A.tbearing = S.in(htb, 3 * sR); A.qseg = S.in(hsg, sQ); A.qscale = S.in(hqs, sQ);
+        A.qstereo = S.in(hq8, sQ); A.tstereo = S.in(ht8, sR);
+        dtaken = S.out(taken, sR);   // uploaded a node's slice at a time by the re-queries
+    });
+    if (rc != OVS_OK) return rc;
     if ((rc = ovs::grow_dev(&m->d_keys, &m->d_keys_cap, (size_t)(Q + 1) * kTriK)) != OVS_OK) return rc;
     if ((rc = ovs::grow_host(&m->h_keys, &m->h_keys_cap, (size_t)(Q + 1) * kTriK)) != OVS_OK) return rc;
-    uint8_t* hs = m->h_stage;
     for (int k = 0; k < Q; ++k) {
         const int i = q1[k];
-        memcpy(hs + o_qd + 32 * (size_t)k, desc_1 + 32 * (size_t)i, 32);
-        memcpy(hs + o_qb + 24 * (size_t)k, bearing_1 + 3 * (size_t)i, 24);
-        reinterpret_cast<float*>(hs + o_qs)[k] = scale_factors_1[octave_1[i]];
-        reinterpret_cast<int2*>(hs + o_sg)[k] = seg[k];
-        hs[o_q8 + k] = is_stereo_1 ? is_stereo_1[i] : 0;
+        memcpy(hqd + 32 * (size_t)k, desc_1 + 32 * (size_t)i, 32);
+        memcpy(hqb + 3 * (size_t)k, bearing_1 + 3 * (size_t)i, 24);
+        hqs[k] = scale_factors_1[octave_1[i]];
+        hsg[k] = seg[k];
+        hq8[k] = is_stereo_1 ? is_stereo_1[i] : 0;
     }
     for (int r = 0; r < R; ++r) {
         const int i = rank2[r];
-        memcpy(hs + o_td + 32 * (size_t)r, desc_2 + 32 * (size_t)i, 32);
-        memcpy(hs + o_tb + 24 * (size_t)r, bearing_2 + 3 * (size_t)i, 24);
-        hs[o_t8 + r] = is_stereo_2 ? is_stereo_2[i] : 0;
+        memcpy(htd + 32 * (size_t)r, desc_2 + 32 * (size_t)i, 32);
+        memcpy(htb + 3 * (size_t)r, bearing_2 + 3 * (size_t)i, 24);
+        ht8[r] = is_stereo_2 ? is_stereo_2[i] : 0;
     }
     cudaStream_t st = m->stream;
-    uint8_t* ds = m->d_q;
-    OVS_CUDA_CHECK(cudaMemcpyAsync(ds, hs, in_total, cudaMemcpyHostToDevice, st));
-    TriArgs A{};
-    A.nq = Q; A.qdesc = reinterpret_cast<const uint4*>(ds + o_qd); A.tdesc = reinterpret_cast<const uint4*>(ds + o_td);
-    A.qbearing = reinterpret_cast<const double*>(ds + o_qb); A.tbearing = reinterpret_cast<const double*>(ds + o_tb);
-    A.qscale = reinterpret_cast<const float*>(ds + o_qs); A.qseg = reinterpret_cast<const int2*>(ds + o_sg);
-    A.qstereo = ds + o_q8; A.tstereo = ds + o_t8;
+    OVS_CUDA_CHECK(S.upload(st));
+    A.nq = Q;
     for (int k = 0; k < 9; ++k) A.E[k] = E_12[k];
     for (int k = 0; k < 3; ++k) A.epipole[k] = epipole_in_2[k];
     OVS_CUDA_CHECK(cudaEventRecord(m->ev[0], st));
@@ -1171,7 +1169,6 @@ extern "C" int ovs_robust_match_for_triangulation_host(ovs_matcher* m, int n1, c
     m->last_kernel_us = ms * 1000.f;
     // sequential replay: a keyframe-2 keypoint goes to its first taker (the flags live in the pinned staging area so that
     // a re-query can upload the slice of a node)
-    uint8_t* const taken = hs + o_tk;
     memset(taken, 0, (size_t)R);
     std::vector<float> deltas; std::vector<int> delta_idx;
     int num = 0;
@@ -1190,9 +1187,9 @@ extern "C" int ovs_robust_match_for_triangulation_host(ovs_matcher* m, int n1, c
             // of the same node to have claimed them).  The replay is sequential, so it waits for the answer.
             ++m->num_requeries;
             const size_t len = (size_t)(seg[k].y - seg[k].x);
-            OVS_CUDA_CHECK(cudaMemcpyAsync(ds + o_tk + seg[k].x, taken + seg[k].x, len, cudaMemcpyHostToDevice, st));
+            OVS_CUDA_CHECK(cudaMemcpyAsync(dtaken + seg[k].x, taken + seg[k].x, len, cudaMemcpyHostToDevice, st));
             TriArgs B = A;
-            B.q0 = k; B.nq = k + 1; B.out_shift = Q - k; B.taken = ds + o_tk;
+            B.q0 = k; B.nq = k + 1; B.out_shift = Q - k; B.taken = dtaken;
             k_triangulation_topk<<<1, 128, 0, st>>>(B, m->d_keys);
             OVS_LAUNCH_CHECK();
             OVS_CUDA_CHECK(cudaMemcpyAsync(m->h_keys + (size_t)Q * kTriK, m->d_keys + (size_t)Q * kTriK, kTriK * 4, cudaMemcpyDeviceToHost, st));
@@ -1302,26 +1299,24 @@ int bow_core(ovs_matcher* m, int na, const uint8_t* desc_a, const uint8_t* valid
             seg[k] = make_int2((int)lo, (int)hi);
         }
     }
-    // staging (host pinned / device): [qdesc 32Q][tdesc 32R][qseg 8Q] | [taken R]
-    const size_t o_qd = 0, o_td = o_qd + 32 * (size_t)Q, o_sg = o_td + 32 * (size_t)R, in_total = ((o_sg + 8 * (size_t)Q + 15) / 16) * 16,
-                 o_tk = in_total, total = ((o_tk + (size_t)R + 15) / 16) * 16;
-    int rc;
-    if ((rc = ovs::grow_host(&m->h_stage, &m->h_stage_cap, total)) != OVS_OK) return rc;
-    if ((rc = ovs::grow_dev(&m->d_q, &m->d_q_cap, total)) != OVS_OK) return rc;
+    NodeArgs A{};
+    uint8_t *hqd, *htd, *taken, *dtaken; int2* hsg;
+    ovs::Staging S;
+    int rc = ovs::stage(S, m->h_stage, m->h_stage_cap, m->d_q, m->d_q_cap, [&](ovs::Staging& S) {
+        A.qdesc = (const uint4*)S.in(hqd, 32 * (size_t)Q); A.tdesc = (const uint4*)S.in(htd, 32 * (size_t)R); A.qseg = S.in(hsg, (size_t)Q);
+        dtaken = S.out(taken, (size_t)R);   // uploaded a node's slice at a time by the re-queries
+    });
+    if (rc != OVS_OK) return rc;
     if ((rc = ovs::grow_dev(&m->d_keys, &m->d_keys_cap, (size_t)(Q + 1) * kNodeK)) != OVS_OK) return rc;
     if ((rc = ovs::grow_host(&m->h_keys, &m->h_keys_cap, (size_t)(Q + 1) * kNodeK)) != OVS_OK) return rc;
-    uint8_t* hs = m->h_stage;
     for (int k = 0; k < Q; ++k) {
-        memcpy(hs + o_qd + 32 * (size_t)k, desc_a + 32 * (size_t)qa[k], 32);
-        reinterpret_cast<int2*>(hs + o_sg)[k] = seg[k];
+        memcpy(hqd + 32 * (size_t)k, desc_a + 32 * (size_t)qa[k], 32);
+        hsg[k] = seg[k];
     }
-    for (int r = 0; r < R; ++r) memcpy(hs + o_td + 32 * (size_t)r, desc_b + 32 * (size_t)rankb[r], 32);
+    for (int r = 0; r < R; ++r) memcpy(htd + 32 * (size_t)r, desc_b + 32 * (size_t)rankb[r], 32);
     cudaStream_t st = m->stream;
-    uint8_t* ds = m->d_q;
-    OVS_CUDA_CHECK(cudaMemcpyAsync(ds, hs, in_total, cudaMemcpyHostToDevice, st));
-    NodeArgs A{};
-    A.nq = Q; A.qdesc = reinterpret_cast<const uint4*>(ds + o_qd); A.tdesc = reinterpret_cast<const uint4*>(ds + o_td);
-    A.qseg = reinterpret_cast<const int2*>(ds + o_sg);
+    OVS_CUDA_CHECK(S.upload(st));
+    A.nq = Q;
     OVS_CUDA_CHECK(cudaEventRecord(m->ev[0], st));
     k_node_topk<<<(Q + 3) / 4, 128, 0, st>>>(A, m->d_keys);
     OVS_LAUNCH_CHECK();
@@ -1334,7 +1329,6 @@ int bow_core(ovs_matcher* m, int na, const uint8_t* desc_a, const uint8_t* valid
     int d_star = OVS_HAMMING_DIST_THR_LOW + 1;
     while (d_star < OVS_MAX_HAMMING_DIST && lowe_ratio * (float)(unsigned)d_star < (float)OVS_HAMMING_DIST_THR_LOW) ++d_star;
     ++d_star;
-    uint8_t* const taken = hs + o_tk;
     memset(taken, 0, (size_t)R);
     for (int k = 0; k < Q; ++k) {
         unsigned keys[kNodeK];
@@ -1363,9 +1357,9 @@ int bow_core(ovs_matcher* m, int na, const uint8_t* desc_a, const uint8_t* valid
             if (!decided) {
                 ++m->num_requeries;
                 const size_t len = (size_t)(seg[k].y - seg[k].x);
-                OVS_CUDA_CHECK(cudaMemcpyAsync(ds + o_tk + seg[k].x, taken + seg[k].x, len, cudaMemcpyHostToDevice, st));
+                OVS_CUDA_CHECK(cudaMemcpyAsync(dtaken + seg[k].x, taken + seg[k].x, len, cudaMemcpyHostToDevice, st));
                 NodeArgs B = A;
-                B.q0 = k; B.nq = k + 1; B.out_shift = Q - k; B.taken = ds + o_tk;
+                B.q0 = k; B.nq = k + 1; B.out_shift = Q - k; B.taken = dtaken;
                 k_node_topk<<<1, 128, 0, st>>>(B, m->d_keys);
                 OVS_LAUNCH_CHECK();
                 OVS_CUDA_CHECK(cudaMemcpyAsync(m->h_keys + (size_t)Q * kNodeK, m->d_keys + (size_t)Q * kNodeK, kNodeK * 4, cudaMemcpyDeviceToHost, st));

@@ -50,6 +50,7 @@
 #include "pnp_math.cuh"
 #include "ransac.cuh"
 #include "sim3_math.cuh"
+#include "staging.h"
 
 namespace {
 
@@ -2275,24 +2276,6 @@ struct ovs_optimizer {
 
 namespace {
 
-int ensure_arenas(ovs_optimizer* h, size_t dbytes, size_t hbytes) {
-    // grow with a quarter of slack: a map's local window changes size from call to call, and every cudaFree / cudaMalloc stalls
-    // all streams of the device
-    if (dbytes > h->d_cap) {
-        cudaFree(h->d_arena); h->d_arena = nullptr; h->d_cap = 0;
-        dbytes += dbytes / 4;
-        OVS_CUDA_CHECK(cudaMalloc(&h->d_arena, dbytes));
-        h->d_cap = dbytes;
-    }
-    if (hbytes > h->h_cap) {
-        cudaFreeHost(h->h_arena); h->h_arena = nullptr; h->h_cap = 0;
-        hbytes += hbytes / 4;
-        OVS_CUDA_CHECK(cudaHostAlloc(&h->h_arena, hbytes, cudaHostAllocDefault));
-        h->h_cap = hbytes;
-    }
-    return OVS_OK;
-}
-
 CameraD to_cam(const ovs_camera* c) {
     CameraD d;
     d.model = c->model; d.fx = c->fx; d.fy = c->fy; d.cx = c->cx; d.cy = c->cy; d.fb = c->focal_x_baseline; d.cols = c->cols; d.rows = c->rows;
@@ -2321,38 +2304,30 @@ extern "C" int ovs_pose_optimize_host(ovs_optimizer* h, const ovs_camera* cam, i
     invalidate_plan(h);
     if (h->pending) { OVS_CUDA_CHECK(ovs::sync_stream(h->stream)); h->pending = false; }
     const size_t N = (size_t)n;
-    const size_t hbytes = 256 * 8 + N * (24 + 8 + 4 + 4 + 1) + 12 * 8 + 16 * 8;
-    const size_t dbytes = hbytes + N * 24 + N + 4096;
-    int rc = ensure_arenas(h, dbytes, hbytes);
+    PoseOptArgs A;
+    double *hp, *hpose, *hstats, *derr; float *hxy, *hxr, *hw; uint8_t *hout, *dlevel;
+    ovs::Staging S;
+    const int rc = ovs::stage(S, h->h_arena, h->h_cap, h->d_arena, h->d_cap, [&](ovs::Staging& S) {
+        A.pts_w = S.in(hp, 3 * N); A.obs_xy = (const float2*)S.in(hxy, 2 * N); A.obs_xr = S.in(hxr, N); A.inv_sigma_sq = S.in(hw, N);
+        A.pose = S.io(hpose, 12); A.stats = S.io(hstats, 16); A.outlier = S.out(hout, N);
+        derr = S.dev<double>(3 * N); dlevel = S.dev<uint8_t>(N);
+    });
     if (rc != OVS_OK) return rc;
-    Arena H{h->h_arena, 0}, D{h->d_arena, 0};
-    double* hp = H.take<double>(3 * N); float* hxy = H.take<float>(2 * N); float* hxr = H.take<float>(N); float* hw = H.take<float>(N);
-    double* hpose = H.take<double>(12); double* hstats = H.take<double>(16); uint8_t* hout = H.take<uint8_t>(N);
-    const size_t in_bytes = H.off;
-    double* dp = D.take<double>(3 * N); float* dxy = D.take<float>(2 * N); float* dxr = D.take<float>(N); float* dw = D.take<float>(N);
-    double* dpose = D.take<double>(12); double* dstats = D.take<double>(16); uint8_t* dout = D.take<uint8_t>(N);
-    double* derr = D.take<double>(3 * N); uint8_t* dlevel = D.take<uint8_t>(N);
     memcpy(hp, pts_w, 24 * N); memcpy(hxy, obs_xy, 8 * N); memcpy(hw, inv_sigma_sq, 4 * N);
     if (obs_x_right) memcpy(hxr, obs_x_right, 4 * N); else for (size_t i = 0; i < N; ++i) hxr[i] = -1.0f;
     memcpy(hpose, pose_cw, 96);
     memset(hstats, 0, 128);
     cudaStream_t st = h->stream;
-    // both arenas were carved with the same sequence, so one contiguous copy moves all inputs
-    OVS_CUDA_CHECK(cudaMemcpyAsync(h->d_arena, h->h_arena, in_bytes, cudaMemcpyHostToDevice, st));
-    PoseOptArgs A;
-    A.cam = to_cam(cam); A.n = n; A.pts_w = dp; A.obs_xy = (const float2*)dxy; A.obs_xr = dxr; A.inv_sigma_sq = dw;
-    A.pose = dpose; A.outlier = dout; A.num_trials = num_trials; A.num_each_iter = num_each_iter;
+    OVS_CUDA_CHECK(S.upload(st));
+    A.cam = to_cam(cam); A.n = n; A.num_trials = num_trials; A.num_each_iter = num_each_iter;
     const float chi_sq_2D = 5.99146f, chi_sq_3D = 7.81473f;
     A.delta = (double)(setup_is_mono ? sqrtf(chi_sq_2D) : sqrtf(chi_sq_3D));
     A.chi2_2d = (double)chi_sq_2D; A.chi2_3d = (double)chi_sq_3D;
-    A.stats = dstats;
     OVS_CUDA_CHECK(cudaEventRecord(h->ev[0], st));
     k_pose_optimize<<<kPoseCluster, kPoseThreads, 0, st>>>(A, derr, dlevel);
     OVS_LAUNCH_CHECK();
     OVS_CUDA_CHECK(cudaEventRecord(h->ev[1], st));
-    OVS_CUDA_CHECK(cudaMemcpyAsync(hpose, dpose, 96, cudaMemcpyDeviceToHost, st));
-    OVS_CUDA_CHECK(cudaMemcpyAsync(hstats, dstats, 128, cudaMemcpyDeviceToHost, st));
-    OVS_CUDA_CHECK(cudaMemcpyAsync(hout, dout, N, cudaMemcpyDeviceToHost, st));
+    OVS_CUDA_CHECK(S.download(st));
     OVS_CUDA_CHECK(ovs::sync_stream(st));
     memcpy(pose_cw, hpose, 96);
     memcpy(outlier_flags, hout, N);
@@ -2623,41 +2598,32 @@ extern "C" int ovs_transform_optimize_host(ovs_optimizer* h, const ovs_camera* c
     invalidate_plan(h);
     if (h->pending) { OVS_CUDA_CHECK(ovs::sync_stream(h->stream)); h->pending = false; }
     const size_t N = (size_t)n;
-    const size_t hbytes = 256 * 12 + N * 2 * (24 + 8 + 4) + N + 13 * 8 + 16 * 8;   // 256: alignment of each take
-    const size_t dbytes = hbytes + N * 32 + N + 4096;
-    int rc = ensure_arenas(h, dbytes, hbytes);
+    Sim3OptArgs A;
+    double *hp1, *hp2, *hS, *hstats, *derr; float *hxy1, *hw1, *hxy2, *hw2; uint8_t *hout, *dlevel;
+    ovs::Staging S;
+    const int rc = ovs::stage(S, h->h_arena, h->h_cap, h->d_arena, h->d_cap, [&](ovs::Staging& S) {
+        A.pw1 = S.in(hp1, 3 * N); A.xy1 = (const float2*)S.in(hxy1, 2 * N); A.w1 = S.in(hw1, N);
+        A.pw2 = S.in(hp2, 3 * N); A.xy2 = (const float2*)S.in(hxy2, 2 * N); A.w2 = S.in(hw2, N);
+        A.sim3 = S.io(hS, 13); A.stats = S.io(hstats, 16); A.inlier = S.out(hout, N);
+        derr = S.dev<double>(4 * N); dlevel = S.dev<uint8_t>(N);
+    });
     if (rc != OVS_OK) return rc;
-    Arena H{h->h_arena, 0}, D{h->d_arena, 0};
-    double* hp1 = H.take<double>(3 * N); float* hxy1 = H.take<float>(2 * N); float* hw1 = H.take<float>(N);
-    double* hp2 = H.take<double>(3 * N); float* hxy2 = H.take<float>(2 * N); float* hw2 = H.take<float>(N);
-    double* hS = H.take<double>(13); double* hstats = H.take<double>(16); uint8_t* hout = H.take<uint8_t>(N);
-    const size_t in_bytes = H.off;
-    double* dp1 = D.take<double>(3 * N); float* dxy1 = D.take<float>(2 * N); float* dw1 = D.take<float>(N);
-    double* dp2 = D.take<double>(3 * N); float* dxy2 = D.take<float>(2 * N); float* dw2 = D.take<float>(N);
-    double* dS = D.take<double>(13); double* dstats = D.take<double>(16); uint8_t* dout = D.take<uint8_t>(N);
-    double* derr = D.take<double>(4 * N); uint8_t* dlevel = D.take<uint8_t>(N);
     memcpy(hp1, pos_w_1, 24 * N); memcpy(hxy1, obs_xy_1, 8 * N); memcpy(hw1, inv_sigma_sq_1, 4 * N);
     memcpy(hp2, pos_w_2, 24 * N); memcpy(hxy2, obs_xy_2, 8 * N); memcpy(hw2, inv_sigma_sq_2, 4 * N);
     memcpy(hS, sim3_12, 13 * 8);
     memset(hstats, 0, 128);
     cudaStream_t st = h->stream;
-    // both arenas were carved with the same sequence, so one contiguous copy moves all inputs
-    OVS_CUDA_CHECK(cudaMemcpyAsync(h->d_arena, h->h_arena, in_bytes, cudaMemcpyHostToDevice, st));
-    Sim3OptArgs A;
+    OVS_CUDA_CHECK(S.upload(st));
     A.cam1 = to_cam(cam_1); A.cam2 = to_cam(cam_2);
     memcpy(A.pose1, pose_1w, 96); memcpy(A.pose2, pose_2w, 96);
     A.n = n;
-    A.pw1 = dp1; A.xy1 = (const float2*)dxy1; A.w1 = dw1; A.pw2 = dp2; A.xy2 = (const float2*)dxy2; A.w2 = dw2;
-    A.sim3 = dS; A.inlier = dout; A.fix_scale = fix_scale ? 1 : 0; A.num_first_iter = num_first_iter; A.num_iter = num_iter;
+    A.fix_scale = fix_scale ? 1 : 0; A.num_first_iter = num_first_iter; A.num_iter = num_iter;
     A.delta = (double)sqrtf(chi_sq); A.chi_sq = (double)chi_sq;
-    A.stats = dstats;
     OVS_CUDA_CHECK(cudaEventRecord(h->ev[0], st));
     k_sim3_optimize<<<kSim3Cluster, kSim3Threads, 0, st>>>(A, derr, dlevel);
     OVS_LAUNCH_CHECK();
     OVS_CUDA_CHECK(cudaEventRecord(h->ev[1], st));
-    OVS_CUDA_CHECK(cudaMemcpyAsync(hS, dS, 13 * 8, cudaMemcpyDeviceToHost, st));
-    OVS_CUDA_CHECK(cudaMemcpyAsync(hstats, dstats, 128, cudaMemcpyDeviceToHost, st));
-    OVS_CUDA_CHECK(cudaMemcpyAsync(hout, dout, N, cudaMemcpyDeviceToHost, st));
+    OVS_CUDA_CHECK(S.download(st));
     OVS_CUDA_CHECK(ovs::sync_stream(st));
     memcpy(sim3_12, hS, 13 * 8);     // the device wrote it back only on success: otherwise these are the input bits
     memcpy(inlier_out, hout, N);
@@ -2842,8 +2808,7 @@ extern "C" int ovs_sim3_solve_ransac_host(ovs_optimizer* h, int B, const int32_t
     int* hoff; CameraD *hc1, *hc2; double *hp1, *hp2, *hw1, *hw2; float *hs1, *hs2; uint64_t* hseed; unsigned long long* hkey; unsigned* hdone;
     double* hS; int *hnum, *hbest; uint8_t *hvalid, *hflags;
     ovs::Staging S;
-    rc = ovs::stage(S, h->h_arena, h->d_arena, [&](size_t hbytes, size_t dbytes) { return ensure_arenas(h, dbytes, hbytes); },
-                    [&](ovs::Staging& S) {
+    rc = ovs::stage(S, h->h_arena, h->h_cap, h->d_arena, h->d_cap, [&](ovs::Staging& S) {
         A.off = S.in(hoff, NB + 1); A.cam1 = S.in(hc1, NB); A.cam2 = S.in(hc2, NB);
         A.pose1 = S.in(hp1, 12 * NB); A.pose2 = S.in(hp2, 12 * NB);
         A.pw1 = S.in(hw1, 3 * N); A.sig1 = S.in(hs1, N); A.pw2 = S.in(hw2, 3 * N); A.sig2 = S.in(hs2, N);
@@ -3023,8 +2988,7 @@ extern "C" int ovs_pnp_solve_ransac_host(ovs_optimizer* h, int B, const int32_t*
     int* hoff; double *hbear, *hpw; float* hsf; uint64_t* hseed; unsigned long long* hkey;
     double* hpose; int *hnum, *hbest; uint8_t *hvalid, *hflags;
     ovs::Staging S;
-    rc = ovs::stage(S, h->h_arena, h->d_arena, [&](size_t hbytes, size_t dbytes) { return ensure_arenas(h, dbytes, hbytes); },
-                    [&](ovs::Staging& S) {
+    rc = ovs::stage(S, h->h_arena, h->h_cap, h->d_arena, h->d_cap, [&](ovs::Staging& S) {
         A.off = S.in(hoff, NB + 1);
         A.bear = S.in(hbear, 3 * N); A.pw = S.in(hpw, 3 * N); A.sf = S.in(hsf, N);
         A.seed = S.in(hseed, NB); A.key = S.in(hkey, NB);
@@ -3116,16 +3080,6 @@ struct BaInputs {   // all host pointers, or all device pointers (obs_x_right ma
     const float* obs_xy; const float* obs_x_right; const float* inv_sigma_sq;
 };
 
-int ensure_work(ovs_optimizer* h, size_t bytes) {
-    if (bytes > h->w_cap) {
-        cudaFree(h->d_work); h->d_work = nullptr; h->w_cap = 0;
-        bytes += bytes / 4;
-        OVS_CUDA_CHECK(cudaMalloc(&h->d_work, bytes));
-        h->w_cap = bytes;
-    }
-    return OVS_OK;
-}
-
 // prepare = upload (or device-to-device copy) of the graph, bookkeeping kernels, ONE small read-back (the counts that size
 // the work buffers; it also carries the validation verdict), co-observation lists and chunk tables.  Returns with the
 // remaining work enqueued.
@@ -3147,34 +3101,22 @@ int prepare_impl(ovs_optimizer* h, const ovs_camera* cam, int setup_is_mono, int
     double* hposes; double* hpoints; int *hkf, *hlm; float *hxy, *hxr, *hw; uint8_t* hfixed; uint8_t* hout; long long* hcounts;
     double* dposes_in; double* dpoints_in; int *dkf, *dlm; float *dxy, *dxr, *dw; uint8_t* dfixed;
     int *dfree, *dlmf, *dpoff; long long* dcounts;
-    size_t in_bytes = 0;
-    auto carve1 = [&](Arena& H, Arena& D) {
-        // inputs (same carving order on both sides -> one contiguous upload)
-        hposes = H.take<double>(12 * sK); hpoints = H.take<double>(3 * sL);
-        hkf = H.take<int>(sM); hlm = H.take<int>(sM); hxy = H.take<float>(2 * sM); hxr = H.take<float>(sM); hw = H.take<float>(sM);
-        hfixed = H.take<uint8_t>(sK);
-        in_bytes = H.off;
-        hout = H.take<uint8_t>(sM); pl.hctl = H.take<LmCtl>(1); pl.hexec = H.take<int>(exec_cap); hcounts = H.take<long long>(8);
-        dposes_in = D.take<double>(12 * sK); dpoints_in = D.take<double>(3 * sL);
-        dkf = D.take<int>(sM); dlm = D.take<int>(sM); dxy = D.take<float>(2 * sM); dxr = D.take<float>(sM); dw = D.take<float>(sM);
-        dfixed = D.take<uint8_t>(sK);
-        dfree = D.take<int>(sK); dlmf = D.take<int>(sL + 1); dpoff = D.take<int>(sL + 1); dcounts = D.take<long long>(8);
-        pl.dout = D.take<uint8_t>(sM); pl.dctl = D.take<LmCtl>(1); pl.dexec = D.take<int>(exec_cap);
-        pl.dposes_ring = D.take<double>((kSpec + 1) * 12 * sK); pl.dpoints_ring = D.take<double>((kSpec + 1) * 3 * sL);
-        pl.dlevel = D.take<uint8_t>(sM); pl.derr = D.take<double>(kSpec * 3 * sM);
-        pl.dlblocks = D.take<int4>((size_t)nlseg * kLbSegCap); pl.dnlblocks = D.take<int>(nlseg);
-        pl.dHll = D.take<double>(6 * sL); pl.dbl = D.take<double>(3 * sL);
-        pl.dpchi = D.take<double>(kSpec * (size_t)nb_obs); pl.dpscale = D.take<double>(kSpec * (size_t)nb_upd);
-        pl.dfail = D.take<int>(kSpec); pl.dmaxdiag = D.take<double>(2); pl.dclk = D.take<long long>(192); pl.dnchunks = D.take<int>(2);
-    };
-    {
-        Arena H0{nullptr, 0}, D0{nullptr, 0};
-        carve1(H0, D0);
-        const int rc = ensure_arenas(h, D0.off + 256, H0.off + 256);
-        if (rc != OVS_OK) return rc;
-    }
-    Arena H{h->h_arena, 0}, D{h->d_arena, 0};
-    carve1(H, D);
+    ovs::Staging S;
+    int rc = ovs::stage(S, h->h_arena, h->h_cap, h->d_arena, h->d_cap, [&](ovs::Staging& S) {
+        dposes_in = S.in(hposes, 12 * sK); dpoints_in = S.in(hpoints, 3 * sL);
+        dkf = S.in(hkf, sM); dlm = S.in(hlm, sM); dxy = S.in(hxy, 2 * sM); dxr = S.in(hxr, sM); dw = S.in(hw, sM);
+        dfixed = S.in(hfixed, sK);
+        // each read back by its own copy: the flags by fetch, the control block and solver slots by run, the counts below
+        pl.dout = S.out(hout, sM); pl.dctl = S.out(pl.hctl, 1); pl.dexec = S.out(pl.hexec, exec_cap); dcounts = S.out(hcounts, 8);
+        dfree = S.dev<int>(sK); dlmf = S.dev<int>(sL + 1); dpoff = S.dev<int>(sL + 1);
+        pl.dposes_ring = S.dev<double>((kSpec + 1) * 12 * sK); pl.dpoints_ring = S.dev<double>((kSpec + 1) * 3 * sL);
+        pl.dlevel = S.dev<uint8_t>(sM); pl.derr = S.dev<double>(kSpec * 3 * sM);
+        pl.dlblocks = S.dev<int4>((size_t)nlseg * kLbSegCap); pl.dnlblocks = S.dev<int>(nlseg);
+        pl.dHll = S.dev<double>(6 * sL); pl.dbl = S.dev<double>(3 * sL);
+        pl.dpchi = S.dev<double>(kSpec * (size_t)nb_obs); pl.dpscale = S.dev<double>(kSpec * (size_t)nb_upd);
+        pl.dfail = S.dev<int>(kSpec); pl.dmaxdiag = S.dev<double>(2); pl.dclk = S.dev<long long>(192); pl.dnchunks = S.dev<int>(2);
+    });
+    if (rc != OVS_OK) return rc;
     pl.exec_cap = exec_cap;
     h->pending = true;
     if (!on_device) {
@@ -3182,7 +3124,7 @@ int prepare_impl(ovs_optimizer* h, const ovs_camera* cam, int setup_is_mono, int
         memcpy(hkf, in.obs_kf, 4 * sM); memcpy(hlm, in.obs_lm, 4 * sM); memcpy(hxy, in.obs_xy, 8 * sM); memcpy(hw, in.inv_sigma_sq, 4 * sM);
         if (in.obs_x_right) memcpy(hxr, in.obs_x_right, 4 * sM); else for (size_t i = 0; i < sM; ++i) hxr[i] = -1.0f;
         memcpy(hfixed, in.fixed, sK);
-        OVS_CUDA_CHECK(cudaMemcpyAsync(h->d_arena, h->h_arena, in_bytes, cudaMemcpyHostToDevice, st));
+        OVS_CUDA_CHECK(S.upload(st));
     } else {
         const cudaMemcpyKind dd = cudaMemcpyDeviceToDevice;
         OVS_CUDA_CHECK(cudaMemcpyAsync(dposes_in, in.poses, 96 * sK, dd, st)); OVS_CUDA_CHECK(cudaMemcpyAsync(dpoints_in, in.points, 24 * sL, dd, st));
@@ -3229,7 +3171,7 @@ int prepare_impl(ovs_optimizer* h, const ovs_camera* cam, int setup_is_mono, int
     const size_t max_chunks = sE / 128 + (size_t)npairs + 8;                     // ceil(len / 128) summed over the pairs
     const size_t max_dchunks = (size_t)nfree_edges / 128 + (size_t)nfree + 8;   // the same over the diagonal pairs
     unsigned *dkeys, *dkeys2; unsigned long long *dvals, *dvals2; int4* dprec; int* dsort;
-    auto carve2 = [&](Arena& W) {
+    auto carve_work = [&](Arena& W) {
         pl.drec = W.take<double>(rec_doubles);
         pl.dpab = W.take<int2>(npairs); pl.ddiag = W.take<int>(nfree);
         pl.dHpp = W.take<double>(21 * (size_t)nfree); pl.dbp = W.take<double>(6 * (size_t)nfree);
@@ -3245,14 +3187,11 @@ int prepare_impl(ovs_optimizer* h, const ovs_camera* cam, int setup_is_mono, int
         pl.spart_stride = 42 * max_chunks;
         pl.dspart = W.take<double>(kSpec * pl.spart_stride); pl.dppart = W.take<double>(27 * max_dchunks);
     };
-    {
-        Arena W0{nullptr, 0};
-        carve2(W0);
-        const int rc = ensure_work(h, W0.off + 256);
-        if (rc != OVS_OK) return rc;
-    }
-    Arena W{h->d_work, 0};
-    carve2(W);
+    Arena W{nullptr, 0};
+    carve_work(W);
+    if ((rc = ovs::grow_dev(&h->d_work, &h->w_cap, W.off)) != OVS_OK) return rc;
+    W = Arena{h->d_work, 0};
+    carve_work(W);
     pl.max_chunks = (int)max_chunks; pl.max_dchunks = (int)max_dchunks;
     OVS_CUDA_CHECK(cudaMemsetAsync(pl.dsegb, 0, 4 * (size_t)npairs, st));
     OVS_CUDA_CHECK(cudaMemsetAsync(pl.dsege, 0, 4 * (size_t)npairs, st));
@@ -4163,45 +4102,33 @@ extern "C" int ovs_graph_optimize_host(ovs_optimizer* h, int K, double* sim3_cw,
     double *dS_in, *dmeas, *dlm, *dS_out, *dpose, *dlm_out, *dring, *dblk, *dbvec, *dpchi, *dpscale, *dmaxdiag;
     int *dfree, *dei, *dej, *dref, *dsegb, *dsege, *dsort, *dfail, *dexec; LmCtl* dctl;
     unsigned *dkeys, *dkeys2; unsigned long long *dvals, *dvals2;
-    size_t in_bytes = 0;
-    auto carve = [&](Arena& H, Arena& D) {
-        // inputs: the same carving order on both sides -> one contiguous upload
-        hS = H.take<double>(13 * sK); hfree = H.take<int>(sK); hei = H.take<int>(sE); hej = H.take<int>(sE); hmeas = H.take<double>(13 * sE);
-        hlm = H.take<double>(3 * sL); href = H.take<int>(sL);
-        in_bytes = H.off;
-        hS_out = H.take<double>(13 * sK); hpose = H.take<double>(12 * sK); hlm_out = H.take<double>(3 * sL);
-        hctl = H.take<LmCtl>(1); hexec = H.take<int>(exec_cap);
-        dS_in = D.take<double>(13 * sK); dfree = D.take<int>(sK); dei = D.take<int>(sE); dej = D.take<int>(sE); dmeas = D.take<double>(13 * sE);
-        dlm = D.take<double>(3 * sL); dref = D.take<int>(sL);
-        dS_out = D.take<double>(13 * sK); dpose = D.take<double>(12 * sK); dlm_out = D.take<double>(3 * sL);
-        dctl = D.take<LmCtl>(1); dexec = D.take<int>(exec_cap);
-        dring = D.take<double>((kSpec + 1) * 13 * sK);
-        dblk = D.take<double>(kPgBlk * sE);
-        dkeys = D.take<unsigned>(nent); dkeys2 = D.take<unsigned>(nent);
-        dvals = D.take<unsigned long long>(nent); dvals2 = D.take<unsigned long long>(nent);
-        dsort = D.take<int>(sort_scratch_ints((long long)std::max<size_t>(nent, 1)));
-        dsegb = D.take<int>((size_t)npairs + 1); dsege = D.take<int>((size_t)npairs + 1);
-        dbvec = D.take<double>((size_t)std::max(n, 1));
-        dpchi = D.take<double>(kSpec * (size_t)std::max(nb_edge, 1)); dpscale = D.take<double>(kSpec * (size_t)nb_vert);
-        dfail = D.take<int>(kSpec); dmaxdiag = D.take<double>(2);
-    };
-    {
-        Arena H0{nullptr, 0}, D0{nullptr, 0};
-        carve(H0, D0);
-        int rc = ensure_arenas(h, D0.off + 256, H0.off + 256);
-        if (rc != OVS_OK) return rc;
-        if (run_lm) {
-            Arena W0{nullptr, 0};
-            W0.take<double>(kSpec * ds.S_stride); W0.take<double>(kSpec * (size_t)nsys); W0.take<double>(kSpec * ds.invL_stride);
-            rc = ensure_work(h, W0.off + 256);
-            if (rc != OVS_OK) return rc;
-        }
-    }
-    Arena H{h->h_arena, 0}, D{h->d_arena, 0};
-    carve(H, D);
+    ovs::Staging S;
+    int rc = ovs::stage(S, h->h_arena, h->h_cap, h->d_arena, h->d_cap, [&](ovs::Staging& S) {
+        dS_in = S.in(hS, 13 * sK); dfree = S.in(hfree, sK); dei = S.in(hei, sE); dej = S.in(hej, sE); dmeas = S.in(hmeas, 13 * sE);
+        dlm = S.in(hlm, 3 * sL); dref = S.in(href, sL);
+        // each read back by its own copy
+        dS_out = S.out(hS_out, 13 * sK); dpose = S.out(hpose, 12 * sK); dlm_out = S.out(hlm_out, 3 * sL);
+        dctl = S.out(hctl, 1); dexec = S.out(hexec, exec_cap);
+        dring = S.dev<double>((kSpec + 1) * 13 * sK);
+        dblk = S.dev<double>(kPgBlk * sE);
+        dkeys = S.dev<unsigned>(nent); dkeys2 = S.dev<unsigned>(nent);
+        dvals = S.dev<unsigned long long>(nent); dvals2 = S.dev<unsigned long long>(nent);
+        dsort = S.dev<int>(sort_scratch_ints((long long)std::max<size_t>(nent, 1)));
+        dsegb = S.dev<int>((size_t)npairs + 1); dsege = S.dev<int>((size_t)npairs + 1);
+        dbvec = S.dev<double>((size_t)std::max(n, 1));
+        dpchi = S.dev<double>(kSpec * (size_t)std::max(nb_edge, 1)); dpscale = S.dev<double>(kSpec * (size_t)nb_vert);
+        dfail = S.dev<int>(kSpec); dmaxdiag = S.dev<double>(2);
+    });
+    if (rc != OVS_OK) return rc;
     if (run_lm) {
-        Arena W{h->d_work, 0};
-        ds.S = W.take<double>(kSpec * ds.S_stride); ds.x = W.take<double>(kSpec * (size_t)nsys); ds.invL = W.take<double>(kSpec * ds.invL_stride);
+        auto carve_work = [&](Arena& W) {
+            ds.S = W.take<double>(kSpec * ds.S_stride); ds.x = W.take<double>(kSpec * (size_t)nsys); ds.invL = W.take<double>(kSpec * ds.invL_stride);
+        };
+        Arena W{nullptr, 0};
+        carve_work(W);
+        if ((rc = ovs::grow_dev(&h->d_work, &h->w_cap, W.off)) != OVS_OK) return rc;
+        W = Arena{h->d_work, 0};
+        carve_work(W);
         ds.fail = dfail; ds.clk = nullptr;
     }
     memcpy(hS, sim3_cw, 104 * sK);
@@ -4214,7 +4141,7 @@ extern "C" int ovs_graph_optimize_host(ovs_optimizer* h, int K, double* sim3_cw,
     h->h_mirror[0] = 0; h->h_mirror[1] = 0; h->h_mirror[2] = 0;
     volatile int* const mirror = (volatile int*)h->d_mirror;
     OVS_CUDA_CHECK(cudaEventRecord(h->ev[0], st));
-    OVS_CUDA_CHECK(cudaMemcpyAsync(h->d_arena, h->h_arena, in_bytes, cudaMemcpyHostToDevice, st));
+    OVS_CUDA_CHECK(S.upload(st));
     OVS_CUDA_CHECK(cudaMemcpyAsync(dring, dS_in, 104 * sK, cudaMemcpyDeviceToDevice, st));
     PgDev P;
     P.K = K; P.E = E; P.nfree = nfree; P.n = nsys; P.fix_scale = fix_scale ? 1 : 0;
@@ -4229,7 +4156,7 @@ extern "C" int ovs_graph_optimize_host(ovs_optimizer* h, int K, double* sim3_cw,
         int end_bit = 1;
         while ((1u << end_bit) <= sentinel) ++end_bit;
         unsigned* ksorted = nullptr; unsigned long long* vsorted = nullptr;
-        int rc = sort_pairs(st, dkeys, dkeys2, dvals, dvals2, (int)nent, end_bit, dsort, &ksorted, &vsorted);
+        rc = sort_pairs(st, dkeys, dkeys2, dvals, dvals2, (int)nent, end_bit, dsort, &ksorted, &vsorted);
         if (rc != OVS_OK) return rc;
         OVS_CUDA_CHECK(cudaMemsetAsync(dsegb, 0, 4 * ((size_t)npairs + 1), st));
         OVS_CUDA_CHECK(cudaMemsetAsync(dsege, 0, 4 * ((size_t)npairs + 1), st));

@@ -1,6 +1,7 @@
 // ransac.cuh -- the building blocks of the batched RANSAC solvers: Sim3 and PnP (optimize.cu) and the essential, homography and
 // fundamental-matrix solvers (two_view_ransac.cu).  Device: the warp-per-hypothesis inlier count and lane-order score, the
-// best-hypothesis key and the CTA-wide index-order compaction.  Host: the offsets check and the staging of a solve's buffers.
+// best-hypothesis key and the CTA-wide index-order compaction.  Host: the offsets check (a solve's buffers are staged through
+// staging.h).
 #pragma once
 #include <cstddef>
 #include <cstdint>
@@ -73,65 +74,6 @@ inline int check_offsets(const int32_t* off, int B, const char* what) {
     OVS_REQUIRE(off[0] == 0, OVS_ERR_INVALID_ARG, "%s[0] must be 0", what);
     for (int b = 0; b < B; ++b)
         OVS_REQUIRE(off[b + 1] >= off[b], OVS_ERR_INVALID_ARG, "%s must be non-decreasing (problem %d)", what, b);
-    return OVS_OK;
-}
-
-// Buffers carved one after another from a byte arena, each aligned to 256 bytes.  With a null base the carve only counts:
-// `off` is then the size the arena needs.
-struct Arena {
-    uint8_t* base; size_t off;
-    template <typename T> T* take(size_t n) {
-        off = (off + 255) / 256 * 256;
-        T* p = reinterpret_cast<T*>(base + off);
-        off += n * sizeof(T);
-        return p;
-    }
-};
-
-// The buffers of one batched solve, carved from a pinned host arena and a device arena together.  Each input and output is
-// named once and gets the same offset in both arenas, so the inputs go up in one copy and the outputs come back in another.
-// Carve the inputs first, then the outputs, then the device-only scratch: `ordered` turns false when a take breaks that order
-// (an input after an output would move the end of the inputs past outputs, and the copy back would miss them).
-struct Staging {
-    Arena h{nullptr, 0}, d{nullptr, 0};
-    size_t in_end = 0;                               // bytes of the inputs
-    int phase = 0;                                   // 0 inputs, 1 outputs, 2 device scratch
-    bool ordered = true;
-    template <typename T> T* in(T*& host, size_t n) {
-        ordered = ordered && phase == 0;
-        host = h.take<T>(n);
-        in_end = h.off;
-        return d.take<T>(n);
-    }
-    template <typename T> T* out(T*& host, size_t n) {
-        ordered = ordered && phase <= 1;
-        phase = 1;
-        host = h.take<T>(n);
-        return d.take<T>(n);
-    }
-    template <typename T> T* dev(size_t n) {
-        phase = 2;
-        return d.take<T>(n);
-    }
-    size_t out_begin() const { return (in_end + 255) / 256 * 256; }
-    cudaError_t upload(cudaStream_t st) const { return cudaMemcpyAsync(d.base, h.base, in_end, cudaMemcpyHostToDevice, st); }
-    cudaError_t download(cudaStream_t st) const {
-        const size_t b = out_begin();
-        return cudaMemcpyAsync(h.base + b, d.base + b, h.off - b, cudaMemcpyDeviceToHost, st);
-    }
-};
-
-// Sizes the arenas by running carve(S) on null bases, has grow(host_bytes, device_bytes) make room (it may move hbase and
-// dbase), then carves them for real into S.  A carve out of order is refused before anything is allocated.
-template <class Grow, class Carve>
-int stage(Staging& S, uint8_t*& hbase, uint8_t*& dbase, Grow grow, Carve carve) {
-    S = Staging{};
-    carve(S);
-    OVS_REQUIRE(S.ordered, OVS_ERR_UNSUPPORTED, "staging carved out of order (inputs, then outputs, then device scratch)");
-    const int rc = grow(S.h.off, S.d.off);
-    if (rc != OVS_OK) return rc;
-    S = Staging{{hbase, 0}, {dbase, 0}};
-    carve(S);
     return OVS_OK;
 }
 

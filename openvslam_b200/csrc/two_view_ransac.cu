@@ -280,10 +280,7 @@ int essential_run(ovs_matcher* h, int B, const int32_t* off, const int32_t* pair
     Results r;
     ovs::Staging S;
     OVS_CUDA_CHECK(cudaSetDevice(h->device));
-    int rc = ovs::stage(S, h->h_ess, h->d_ess, [&](size_t hbytes, size_t dbytes) {
-        const int e = ovs::grow_dev(&h->d_ess, &h->d_ess_cap, dbytes);
-        return e != OVS_OK ? e : ovs::grow_host(&h->h_ess, &h->h_ess_cap, hbytes);
-    }, [&](ovs::Staging& S) {
+    int rc = ovs::stage(S, h->h_ess, h->h_ess_cap, h->d_ess, h->d_ess_cap, [&](ovs::Staging& S) {
         A.off = S.in(hoff, NB + 1); A.seed = S.in(hseed, NB);
         A.model.pairs = pairs ? S.in(hpairs, np) : nullptr;
         if (bear.on_device) { A.model.bear_1 = bear.b1; A.model.bear_2 = bear.b2; }
@@ -315,10 +312,7 @@ int two_view_run(ovs_matcher* h, int B, const int32_t* koff_1, const ovs_keypoin
     Results r;
     ovs::Staging S;
     OVS_CUDA_CHECK(cudaSetDevice(h->device));
-    int rc = ovs::stage(S, h->h_tv, h->d_tv, [&](size_t hbytes, size_t dbytes) {
-        const int e = ovs::grow_dev(&h->d_tv, &h->d_tv_cap, dbytes);
-        return e != OVS_OK ? e : ovs::grow_host(&h->h_tv, &h->h_tv_cap, hbytes);
-    }, [&](ovs::Staging& S) {
+    int rc = ovs::stage(S, h->h_tv, h->h_tv_cap, h->d_tv, h->d_tv_cap, [&](ovs::Staging& S) {
         TwoViewModel<Model>& m = A.model;
         A.off = S.in(hmoff, NB + 1); m.koff_1 = S.in(hk1, NB + 1); m.koff_2 = S.in(hk2, NB + 1);
         A.seed = S.in(hseed, NB); m.pairs = S.in(hpairs, 2 * N);
