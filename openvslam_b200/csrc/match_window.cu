@@ -334,6 +334,7 @@ Resolved resolve(const ovs_frame_index* f, const unsigned* keys, Valid valid) {
 // Re-runs one query with a distance cap per keypoint (cap[idx]: candidate valid iff d < cap[idx]).
 int requery(ovs_frame_index* f, const float* ref_xy, float margin, int min_level, int max_level, const float* xr_q,
             const uint8_t* qdesc, const std::vector<unsigned short>& cap_by_idx, unsigned* keys_out) {
+    ++f->m->num_requeries;
     std::vector<unsigned short> cap((size_t)std::max(f->nranked, 1));
     for (int r = 0; r < f->nranked; ++r) cap[r] = cap_by_idx[f->rank_to_idx[r]];
     int rc = window_topk(f, 1, ref_xy, &margin, &min_level, &max_level, xr_q, qdesc, cap.data());
@@ -857,6 +858,12 @@ extern "C" int ovs_area_match_in_consistent_area_host(ovs_frame_index* f2, int n
         lo[q] = octave_1[i]; hi[q] = octave_1[i];
         memcpy(&qd[32 * (size_t)q], desc_1 + 32 * (size_t)i, 32);
     }
+    // the area matcher has no x_right test: a stereo frame's index searches here as a monocular one (restored on return)
+    struct NoXr {
+        ovs_frame_index* f; bool saved;
+        ~NoXr() { f->has_xr = saved; }
+    } no_xr{f, f->has_xr};
+    f->has_xr = false;
     int rc = window_topk(f, nq, ref.data(), mg.data(), lo.data(), hi.data(), nullptr, qd.data(), nullptr);
     if (rc != OVS_OK) return rc;
     std::vector<unsigned> keys(f->m->h_keys, f->m->h_keys + (size_t)nq * kTopK);

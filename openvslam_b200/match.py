@@ -13,10 +13,16 @@ MAX_HAMMING_DIST = 256
 class _matcher_handle:
     def __init__(self, device=0):
         self._h = C.c_void_p()
+        self._indexes = set()      # handles of the frame indexes built on this matcher and not yet destroyed
         _lib.check(_lib.lib().ovs_matcher_create(int(device), C.byref(self._h)))
 
     def close(self):
         if getattr(self, "_h", None):
+            # an index uses its matcher until it is destroyed, and the garbage collector may finalize a matcher before
+            # the indexes that refer to it: destroy those first
+            for h in getattr(self, "_indexes", ()):
+                _lib.lib().ovs_frame_index_destroy(C.c_void_p(h))
+            self._indexes = set()
             _lib.lib().ovs_matcher_destroy(self._h)
             self._h = None
 
@@ -182,6 +188,7 @@ class frame_index:
         self.grid = grid
         self._h = C.c_void_p()
         _lib.check(_lib.lib().ovs_frame_index_create(matcher._h, self.n, px, py, po, pa, pxr, pd, C.byref(grid), C.byref(self._h)))
+        matcher._indexes.add(self._h.value)
 
     @classmethod
     def from_device(cls, matcher, n, d_keypts_ptr, d_desc_ptr, grid, d_x_right_ptr=None):
@@ -193,11 +200,15 @@ class frame_index:
         self._h = C.c_void_p()
         _lib.check(_lib.lib().ovs_frame_index_create_device(matcher._h, self.n, C.c_void_p(d_keypts_ptr), C.c_void_p(d_desc_ptr),
                                                              C.c_void_p(d_x_right_ptr) if d_x_right_ptr else None, C.byref(grid), C.byref(self._h)))
+        matcher._indexes.add(self._h.value)
         return self
 
     def close(self):
         if getattr(self, "_h", None):
-            _lib.lib().ovs_frame_index_destroy(self._h)
+            live = self._m._indexes
+            if self._h.value in live:      # else the matcher was closed first and destroyed this index with it
+                live.discard(self._h.value)
+                _lib.lib().ovs_frame_index_destroy(self._h)
             self._h = None
 
     def __del__(self):

@@ -5,6 +5,7 @@ import numpy as np
 import pytest
 
 from openvslam_b200 import synth
+import window_match_reference as R
 
 pytestmark = pytest.mark.gpu
 
@@ -172,10 +173,21 @@ def test_greedy_requery_paths(oracle):
     lmd = base[rng.integers(0, 6, nl)].copy()
     reproj = np.stack([rng.uniform(100, 400, nl), rng.uniform(100, 300, nl)], 1).astype(np.float32)
     lvl = rng.integers(0, 3, nl).astype(np.int32)
+    fr = R.Frame(x, y, octv, ang, None, desc, R.Grid(0, 752, 0, 480))
+    before = mt.num_requeries()
     n1, m1 = mt.match_frame_and_landmarks(fi, sf, reproj, None, lvl, lmd, None, None, 40.0)
     o1, om1 = oracle.projection_match_frame_and_landmarks(fo, sf, reproj, None, lvl, lmd, None, None, 40.0, 0.95)
-    assert n1 == o1 and np.array_equal(m1, om1)
-    n2, m2 = mt.match_current_and_last_frames(fi, sf, 8, np.ones(nl, np.uint8), reproj, None, lvl, rng.uniform(0, 360, nl).astype(np.float32), lmd, None, 40.0)
+    r1, rm1, _ = R.match_frame_and_landmarks(fr, sf, reproj, None, lvl, lmd, None, None, 40.0, 0.95)
+    assert n1 == o1 == r1 and np.array_equal(m1, om1) and np.array_equal(m1, rm1)
+    assert mt.num_requeries() > before
+    usable = np.ones(nl, np.uint8)
+    last_angle = rng.uniform(0, 360, nl).astype(np.float32)
+    before = mt.num_requeries()
+    n2, m2 = mt.match_current_and_last_frames(fi, sf, 8, usable, reproj, None, lvl, last_angle, lmd, None, 40.0)
+    o2, om2 = oracle.projection_match_current_and_last(fo, sf, 8, usable, reproj, None, lvl, last_angle, lmd, None, 40.0, False, False, True)
+    r2, rm2, _ = R.match_current_and_last_frames(fr, sf, 8, usable, reproj, None, lvl, last_angle, lmd, None, 40.0)
+    assert n2 == o2 == r2 and np.array_equal(m2, om2) and np.array_equal(m2, rm2) and n2 > 0
+    assert mt.num_requeries() > before
     fi.close(); mt.close()
 
 
