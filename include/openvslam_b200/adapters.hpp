@@ -18,6 +18,8 @@
 //   solve::homography_solver / solve::fundamental_solver(const std::vector<cv::KeyPoint>&, const std::vector<cv::KeyPoint>&,
 //     const std::vector<std::pair<int, int>>&, float), find_via_ransac(unsigned, bool), solution_is_valid(), get_best_score(),
 //     get_best_H_21() / get_best_F_21(), get_inlier_matches()                    (solve/{homography,fundamental}_solver.h)
+//   the compute step of mapping_module::create_new_landmarks over data::keyframe (module/mapping_module.cc): match_for_triangulation
+//     and two_view_triangulator::triangulate for every neighbour, as module::two_view_triangulator::create_new_landmarks
 //
 // Include it INSTEAD of openvslam_b200.hpp in a translation unit that can see the reference's headers (here: the stand-ins
 // under tests/cpp/standin, which declare the members used below with the names recalled in SURVEY.md section 2 / 8b;
@@ -33,6 +35,8 @@
 #endif
 
 #include <algorithm>
+#include <array>
+#include <cmath>
 #include <cstring>
 #include <map>
 #include <mutex>
@@ -514,5 +518,88 @@ inline void solve::fundamental_solver::find_via_ransac(const unsigned int max_nu
 }
 
 inline Mat33_t solve::fundamental_solver::get_best_F_21() const { return adapters::to_mat33(best_.M_21); }
+
+// ------------------------------------------------------------------ module::two_view_triangulator / create_new_landmarks
+namespace adapters {
+//! A keyframe's own vectors as an ovs_keyframe_view (owns the flattened copies): undist_keypts_ (cv::KeyPoint is layout-compatible
+//! with ovs_keypoint), bearings_, stereo_x_right_ / depths_ (left out when the keyframe has no stereo keypoint), descriptors_, the
+//! landmark flags (get_landmarks()[i] != nullptr), bow_feat_vec_ inverted into node ids, the scale tables, the pose and the camera.
+//! true_baseline is focal_x_baseline_ / fx_, the value the reference's perspective-family camera constructors store.
+struct keyframe_arrays {
+    std::vector<ovs_keypoint> keypts;
+    std::vector<double> bearings;
+    std::vector<float> x_right, depths;
+    std::vector<std::uint8_t> desc, has_landmark;
+    std::vector<std::int32_t> bow_node;
+    ovs_keyframe_view view{};
+    template <class Keyframe>
+    explicit keyframe_arrays(Keyframe* k) {
+        static_assert(sizeof(cv::KeyPoint) == sizeof(ovs_keypoint), "cv::KeyPoint layout changed");
+        const std::size_t n = k->undist_keypts_.size();
+        keypts.resize(n);
+        if (n) std::memcpy(keypts.data(), k->undist_keypts_.data(), sizeof(ovs_keypoint) * n);
+        bearings = flat_bearings(k->bearings_);
+        const bool stereo = k->stereo_x_right_.size() == n && k->depths_.size() == n &&
+                            std::any_of(k->stereo_x_right_.begin(), k->stereo_x_right_.end(), [](float x) { return 0.0f <= x; });
+        if (stereo) { x_right.assign(k->stereo_x_right_.begin(), k->stereo_x_right_.end()); depths.assign(k->depths_.begin(), k->depths_.end()); }
+        desc.resize(32 * n);
+        for (std::size_t i = 0; i < n; ++i) std::memcpy(&desc[32 * i], k->descriptors_.ptr(static_cast<int>(i)), 32);   // rows may be strided
+        const auto lms = k->get_landmarks();
+        has_landmark.assign(n, 0);
+        for (std::size_t i = 0; i < n && i < lms.size(); ++i) has_landmark[i] = lms[i] != nullptr;
+        bow_node.assign(n, -1);
+        for (const auto& node : k->bow_feat_vec_)
+            for (const auto idx : node.second)
+                if (static_cast<std::size_t>(idx) < n) bow_node[idx] = static_cast<std::int32_t>(node.first);
+        to_Rt(k->get_cam_pose(), view.pose_cw);
+        view.camera = to_camera(k->camera_);
+        view.true_baseline = view.camera.fx != 0.0 ? view.camera.focal_x_baseline / view.camera.fx : 0.0;
+        view.scale_factor = k->scale_factor_;
+        view.num_scale_levels = static_cast<std::int32_t>(k->scale_factors_.size());
+        view.scale_factors = k->scale_factors_.data(); view.level_sigma_sq = k->level_sigma_sq_.data();
+        view.num_keypts = static_cast<std::int32_t>(n);
+        view.undist_keypts = keypts.data(); view.bearings = bearings.data();
+        view.stereo_x_right = stereo ? x_right.data() : nullptr; view.depths = stereo ? depths.data() : nullptr;
+        view.descriptors = desc.data(); view.has_landmark = has_landmark.data(); view.bow_node = bow_node.data();
+    }
+};
+
+//! E_12 = [t_12]x R_12 with R_12 = R_1w R_2w^T, t_12 = t_1w - R_12 t_2w (the reference's essential_solver::create_E_21 with the two
+//! keyframes swapped), and the epipole: keyframe 1's centre c_1 = -R_1w^T t_1w as a unit bearing of keyframe 2, R_2w c_1 + t_2w.
+inline void e12_and_epipole(const double* P1, const double* P2, std::array<double, 9>& E, std::array<double, 3>& epipole) {
+    double R12[9], t12[3], c1[3];
+    for (int r = 0; r < 3; ++r)
+        for (int c = 0; c < 3; ++c) R12[3 * r + c] = P1[3 * r] * P2[3 * c] + P1[3 * r + 1] * P2[3 * c + 1] + P1[3 * r + 2] * P2[3 * c + 2];
+    for (int r = 0; r < 3; ++r) t12[r] = P1[9 + r] - (R12[3 * r] * P2[9] + R12[3 * r + 1] * P2[10] + R12[3 * r + 2] * P2[11]);
+    const double tx[9] = {0, -t12[2], t12[1], t12[2], 0, -t12[0], -t12[1], t12[0], 0};
+    for (int r = 0; r < 3; ++r)
+        for (int c = 0; c < 3; ++c) E[3 * r + c] = tx[3 * r] * R12[c] + tx[3 * r + 1] * R12[3 + c] + tx[3 * r + 2] * R12[6 + c];
+    for (int r = 0; r < 3; ++r) c1[r] = -(P1[r] * P1[9] + P1[3 + r] * P1[10] + P1[6 + r] * P1[11]);
+    double e[3];
+    for (int r = 0; r < 3; ++r) e[r] = P2[3 * r] * c1[0] + P2[3 * r + 1] * c1[1] + P2[3 * r + 2] * c1[2] + P2[9 + r];
+    const double nrm = std::sqrt(e[0] * e[0] + e[1] * e[1] + e[2] * e[2]);
+    for (int r = 0; r < 3; ++r) epipole[r] = e[r] / nrm;
+}
+}  // namespace adapters
+
+// create_new_landmarks on data::keyframe: the neighbours are the ones that passed the caller's baseline / depth gates, in the
+// reference's order.  Records (neighbour, idx_1, idx_2, pos_w) in creation order; making the landmarks stays with the caller.
+template <class Keyframe>
+inline std::vector<ovs_new_landmark> module::two_view_triangulator::create_new_landmarks(Keyframe* keyfrm_1,
+                                                                                         const std::vector<Keyframe*>& neighbours,
+                                                                                         const bool check_orientation) const {
+    const adapters::keyframe_arrays k1(keyfrm_1);
+    std::vector<adapters::keyframe_arrays> own;
+    own.reserve(neighbours.size());
+    std::vector<ovs_keyframe_view> views;
+    std::vector<std::array<double, 9>> E(neighbours.size());
+    std::vector<std::array<double, 3>> ep(neighbours.size());
+    for (std::size_t b = 0; b < neighbours.size(); ++b) {
+        own.emplace_back(neighbours[b]);
+        views.push_back(own.back().view);
+        adapters::e12_and_epipole(k1.view.pose_cw, own.back().view.pose_cw, E[b], ep[b]);
+    }
+    return create_new_landmarks(k1.view, views, E, ep, check_orientation);
+}
 
 }  // namespace openvslam

@@ -20,6 +20,8 @@
 // member names and return values.
 #pragma once
 
+#include <algorithm>
+#include <array>
 #include <cstdint>
 #include <cstring>
 #include <stdexcept>
@@ -918,4 +920,106 @@ public:
 };
 
 }  // namespace solve
+
+namespace module {
+
+//! module::two_view_triangulator (module/two_view_triangulator.h) on array views (ovs_keyframe_view: a keyframe's own vectors),
+//! and the compute step of mapping_module::create_new_landmarks.  Owns a matcher handle (its CUDA stream and buffers).
+class two_view_triangulator {
+public:
+    //! One keyframe pair and its pairs (idx_1, idx_2) for the batched triangulate.
+    struct problem {
+        const ovs_keyframe_view* keyfrm_1;
+        const ovs_keyframe_view* keyfrm_2;
+        std::vector<std::pair<unsigned int, unsigned int>> pairs;
+    };
+
+    explicit two_view_triangulator(const float rays_parallax_deg_thr = 1.0, const int device = 0)
+        : rays_parallax_deg_thr_(rays_parallax_deg_thr) {
+        detail::check(ovs_matcher_create(device, &h_));
+    }
+    //! The reference's constructor arguments: keyfrm_1, keyfrm_2 (the views must outlive the object), rays_parallax_deg_thr.
+    two_view_triangulator(const ovs_keyframe_view& keyfrm_1, const ovs_keyframe_view& keyfrm_2, const float rays_parallax_deg_thr,
+                          const int device = 0)
+        : two_view_triangulator(rays_parallax_deg_thr, device) {
+        keyfrm_1_ = &keyfrm_1; keyfrm_2_ = &keyfrm_2;
+    }
+    ~two_view_triangulator() { ovs_matcher_destroy(h_); }
+    two_view_triangulator(const two_view_triangulator&) = delete;
+    two_view_triangulator& operator=(const two_view_triangulator&) = delete;
+    ovs_matcher* handle() const { return h_; }
+
+    //! triangulate(idx_1, idx_2, pos_w) of the constructor's keyframe pair for every pair of the list in one GPU call:
+    //! valid[m] = the reference's return value, pos_w[3 m] = the point (zero where invalid).
+    void triangulate(const std::vector<std::pair<unsigned int, unsigned int>>& pairs, std::vector<std::uint8_t>& valid,
+                     std::vector<double>& pos_w) const {
+        if (!keyfrm_1_ || !keyfrm_2_) throw std::runtime_error("ovs_b200: two_view_triangulator built without its keyframes");
+        std::vector<std::vector<std::uint8_t>> v;
+        std::vector<std::vector<double>> p;
+        triangulate(std::vector<problem>{problem{keyfrm_1_, keyfrm_2_, pairs}}, v, p);
+        valid = std::move(v.front()); pos_w = std::move(p.front());
+    }
+    //! The same for B keyframe pairs in one GPU call; valid[b] / pos_w[b] per problem.
+    void triangulate(const std::vector<problem>& problems, std::vector<std::vector<std::uint8_t>>& valid,
+                     std::vector<std::vector<double>>& pos_w) const {
+        const std::size_t B = problems.size();
+        std::vector<ovs_keyframe_view> k1(B), k2(B);
+        std::vector<std::int32_t> off(B + 1, 0), pairs;
+        for (std::size_t b = 0; b < B; ++b) {
+            k1[b] = *problems[b].keyfrm_1; k2[b] = *problems[b].keyfrm_2;
+            for (const auto& pr : problems[b].pairs) { pairs.push_back(static_cast<std::int32_t>(pr.first)); pairs.push_back(static_cast<std::int32_t>(pr.second)); }
+            off[b + 1] = static_cast<std::int32_t>(pairs.size() / 2);
+        }
+        const std::size_t M = pairs.size() / 2;
+        std::vector<std::uint8_t> v(std::max<std::size_t>(M, 1));
+        std::vector<double> p(3 * std::max<std::size_t>(M, 1));
+        detail::check(ovs_two_view_triangulate_host(h_, static_cast<int>(B), k1.data(), k2.data(), off.data(), pairs.data(),
+                                                    rays_parallax_deg_thr_, v.data(), p.data()));
+        valid.assign(B, {}); pos_w.assign(B, {});
+        for (std::size_t b = 0; b < B; ++b) {
+            valid[b].assign(v.begin() + off[b], v.begin() + off[b + 1]);
+            pos_w[b].assign(p.begin() + 3 * static_cast<std::size_t>(off[b]), p.begin() + 3 * static_cast<std::size_t>(off[b + 1]));
+        }
+    }
+
+    //! create_new_landmarks' compute step (ovs_create_new_landmarks_host): for each neighbour in order, match_for_triangulation
+    //! with keyframe 1's landmark flags as they stand (E_12[b] row-major, epipole_in_2[b] = keyframe 1's centre as a bearing of
+    //! neighbour b), then this triangulator on its pairs.  Returns the records in creation order; creating the landmarks stays with
+    //! the caller.  Neighbour b's records depend on neighbours 0 .. b only (the prefix rule of ovs_b200.h).
+    std::vector<ovs_new_landmark> create_new_landmarks(const ovs_keyframe_view& keyfrm_1, const std::vector<ovs_keyframe_view>& neighbours,
+                                                       const std::vector<std::array<double, 9>>& E_12,
+                                                       const std::vector<std::array<double, 3>>& epipole_in_2,
+                                                       const bool check_orientation) const {
+        const std::size_t B = neighbours.size();
+        if (E_12.size() != B || epipole_in_2.size() != B) throw std::runtime_error("ovs_b200: one E_12 and one epipole per neighbour");
+        std::vector<double> E(9 * B), ep(3 * B);
+        for (std::size_t b = 0; b < B; ++b) {
+            std::copy(E_12[b].begin(), E_12[b].end(), E.begin() + 9 * b);
+            std::copy(epipole_in_2[b].begin(), epipole_in_2[b].end(), ep.begin() + 3 * b);
+        }
+        std::vector<ovs_new_landmark> out(static_cast<std::size_t>(std::max(keyfrm_1.num_keypts, 1)));
+        int n = 0;
+        detail::check(ovs_create_new_landmarks_host(h_, &keyfrm_1, static_cast<int>(B), neighbours.data(), E.data(), ep.data(),
+                                                    check_orientation ? 1 : 0, rays_parallax_deg_thr_, out.data(),
+                                                    keyfrm_1.num_keypts, &n));
+        out.resize(static_cast<std::size_t>(n));
+        return out;
+    }
+#ifdef OVS_B200_WITH_REFERENCE_TYPES
+    //! The same on the reference's keyframes (data::keyframe in the reference tree; body in adapters.hpp): flattens each keyframe,
+    //! forms E_12 and the epipole from the poses as the reference does.  A template deduced from its arguments, so it is compiled
+    //! only where it is called.
+    template <class Keyframe>
+    std::vector<ovs_new_landmark> create_new_landmarks(Keyframe* keyfrm_1, const std::vector<Keyframe*>& neighbours,
+                                                       const bool check_orientation) const;
+#endif
+
+private:
+    const float rays_parallax_deg_thr_;
+    const ovs_keyframe_view* keyfrm_1_ = nullptr;
+    const ovs_keyframe_view* keyfrm_2_ = nullptr;
+    ovs_matcher* h_ = nullptr;
+};
+
+}  // namespace module
 }  // namespace openvslam

@@ -371,6 +371,82 @@ typedef struct {
     double cols, rows;
 } ovs_camera;
 
+/* ---- local mapping: module::two_view_triangulator (module/two_view_triangulator.cc) and the compute step of
+ * mapping_module::create_new_landmarks (module/mapping_module.cc) ---- */
+
+/* What the triangulator (and, for ovs_create_new_landmarks_host, the triangulation matcher) reads of one keyframe.  The arrays
+ * are the keyframe's own vectors, so `.data()` can be passed:
+ *  pose_cw[12]: get_cam_pose() as {R row-major (9), t (3)};  camera: camera_ (perspective, or fisheye on undistorted
+ *  keypoints passed as perspective; equirectangular); true_baseline: camera_->true_baseline_ (read for stereo keypoints only);
+ *  scale_factor: scale_factor_;  scale_factors / level_sigma_sq [num_scale_levels]: scale_factors_, level_sigma_sq_;
+ *  undist_keypts[num_keypts]: undist_keypts_ (pt, octave and, for the matcher, angle are read);  bearings[num_keypts*3]: bearings_
+ *  (unit);  stereo_x_right / depths [num_keypts]: stereo_x_right_, depths_ (NULL, both: monocular; an equirectangular keyframe
+ *  has no stereo keypoint);
+ *  descriptors[num_keypts*32], has_landmark[num_keypts] (get_landmark(i) != nullptr), bow_node[num_keypts] (bow_feat_vec_
+ *  inverted, < 0 = none): read by ovs_create_new_landmarks_host only (NULL elsewhere). */
+typedef struct {
+    double pose_cw[12];
+    ovs_camera camera;
+    double true_baseline;
+    float scale_factor;
+    int32_t num_scale_levels;
+    const float* scale_factors;
+    const float* level_sigma_sq;
+    int32_t num_keypts;
+    const ovs_keypoint* undist_keypts;
+    const double* bearings;
+    const float* stereo_x_right;
+    const float* depths;
+    const uint8_t* descriptors;
+    const uint8_t* has_landmark;
+    const int32_t* bow_node;
+} ovs_keyframe_view;
+
+/* module::two_view_triangulator(keyfrm_1, keyfrm_2, rays_parallax_deg_thr).triangulate(idx_1, idx_2, pos_w) for every pair of a
+ * list, for B independent keyframe pairs in one call (create_new_landmarks passes 1.0 degree).  Problem b triangulates the pairs
+ * pair_offsets[b] .. pair_offsets[b + 1] - 1 of pairs (2 per pair: idx_1 into keyfrms_1[b], idx_2 into keyfrms_2[b]);
+ * pair_offsets[0] = 0, non-decreasing.  valid[m] = the reference's return value, pos_w[m*3] = the point (zero where invalid).
+ * The conventions (world-frame rays, the closed-form stereo parallax, the branch rule, the two-camera solve by a 4x4 Jacobi
+ * on A^T A, the stereo back-projection, the cheirality, reprojection and scale tests) are in DESIGN.md section 5.
+ * B outside 0 .. 65535, invalid offsets, an index outside its keyframe, an octave outside the scale table, a bearing that is not a
+ * finite unit vector, a stereo keypoint with a non-finite depth, an unknown camera model (or a stereo keypoint on an
+ * equirectangular camera), a non-finite pose or rays_parallax_deg_thr return OVS_ERR_INVALID_ARG, and more than 2^30 - 1 pairs in
+ * all OVS_ERR_UNSUPPORTED, before any launch; B == 0 or
+ * no pair at all returns without a launch.  Otherwise the call is one launch, one copy each way and one wait, on buffers of its
+ * own: the other entry points of the handle are unaffected. */
+int ovs_two_view_triangulate_host(ovs_matcher* h, int B, const ovs_keyframe_view* keyfrms_1, const ovs_keyframe_view* keyfrms_2,
+                                  const int32_t* pair_offsets, const int32_t* pairs, double rays_parallax_deg_thr, uint8_t* valid,
+                                  double* pos_w);
+
+/* A landmark create_new_landmarks makes: keyfrms_2[neighbour], keypoint idx_1 of keyframe 1, idx_2 of the neighbour, pos_w. */
+typedef struct {
+    int32_t neighbour, idx_1, idx_2, reserved;
+    double pos_w[3];
+} ovs_new_landmark;
+
+/* The compute step of mapping_module::create_new_landmarks: for b = 0 .. B - 1 (the neighbours in the reference's order, after
+ * the caller's baseline and depth gates), robust::match_for_triangulation(keyfrm_1, keyfrms_2[b], E_12[b*9], ...) exactly as
+ * ovs_robust_match_for_triangulation_host with the landmark flags of keyframe 1 as they stand at that neighbour, then
+ * two_view_triangulator(keyfrm_1, keyfrms_2[b], rays_parallax_deg_thr) on its pairs in idx_1 order; every valid pair becomes a
+ * record and its keyframe-1 keypoint counts as having a landmark for the neighbours after b.  epipole_in_2[b*3]: as for the
+ * matcher.  out[capacity >= keyfrm_1->num_keypts] receives the records in creation order, *num_out their count.
+ * Neighbour b's records depend on neighbours 0 .. b only: the records of the first k + 1 neighbours of a call are the records of a
+ * call with those k + 1 neighbours, so a caller that stops at the reference's keyframe_is_queued() check keeps the prefix that
+ * ends before the neighbour it stops at.
+ * Device work: ONE launch of the matcher's candidate-list kernel for every (neighbour, query) pair, ONE launch of the
+ * triangulation kernel over every listed candidate, one copy each way and one wait; then, when a record comes from a list, one
+ * gather launch, one copy each way and one wait.  A list exhausted by earlier takers costs a re-query: two launches (its list, its
+ * pair's triangulation), one copy each way and one wait.  Nothing else depends on B.  Checked before any launch:
+ *  OVS_ERR_INVALID_ARG: the keyframe checks of ovs_two_view_triangulate_host (on every keypoint of every keyframe), a missing
+ *    descriptor, landmark-flag or node array, B outside 0 .. 65535, a non-finite E_12 or epipole;
+ *  OVS_ERR_CAPACITY: capacity < keyfrm_1->num_keypts;
+ *  OVS_ERR_UNSUPPORTED: a neighbour with 65536 or more keypoints, or (B x queries + 1) x 8 candidate slots above 2^31 - 1 (queries:
+ *    the keyframe-1 keypoints without a landmark that have a node).
+ * Uses the buffers of ovs_two_view_triangulate_host. */
+int ovs_create_new_landmarks_host(ovs_matcher* h, const ovs_keyframe_view* keyfrm_1, int B, const ovs_keyframe_view* keyfrms_2,
+                                  const double* E_12, const double* epipole_in_2, int check_orientation, double rays_parallax_deg_thr,
+                                  ovs_new_landmark* out, int capacity, int* num_out);
+
 /* data::frame's constructor right after extract(): camera->undistort_keypoints(keypts_, undist_keypts_) +
  * camera->convert_keypoints_to_bearings(undist_keypts_, bearings_) (camera/perspective.cc, camera/equirectangular.cc; SURVEY 8f
  * rank 3).  Perspective: cv::undistortPoints(pts, K, dist, R = I, P = K, MAX_ITER num_iterations) -- OpenVSLAM uses 20 --

@@ -1,4 +1,5 @@
-// match_common.h -- the matcher handle shared by match_bruteforce.cu, match_window.cu and two_view_ransac.cu.  Its arenas
+// match_common.h -- the matcher handle shared by match_bruteforce.cu, match_window.cu, two_view_ransac.cu and
+// two_view_triangulate.cu.  Its arenas
 // grow and are carved through staging.h.
 #pragma once
 #include <algorithm>
@@ -28,6 +29,9 @@ struct ovs_matcher {
     // the homography / fundamental-matrix solvers' own arenas (two_view_ransac.cu)
     uint8_t* d_tv = nullptr; size_t d_tv_cap = 0;
     uint8_t* h_tv = nullptr; size_t h_tv_cap = 0;       // pinned
+    // the two-view triangulator's and create_new_landmarks' own arenas (two_view_triangulate.cu, match_window.cu)
+    uint8_t* d_tri = nullptr; size_t d_tri_cap = 0;
+    uint8_t* h_tri = nullptr; size_t h_tri_cap = 0;     // pinned
     cudaEvent_t ev[2]{};
     float last_kernel_us = 0.f;
     int num_requeries = 0;   // GPU re-queries issued by the greedy replays so far (diagnostic)

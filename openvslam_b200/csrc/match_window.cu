@@ -20,11 +20,13 @@
 // histogram, the median test of stereo) run on the host over these results.
 #include <algorithm>
 #include <cmath>
+#include <cstdint>
 #include <cstring>
 #include <new>
 #include <vector>
 
 #include "match_common.h"
+#include "two_view_triangulate.h"
 
 // ------------------------------------------------------------------------------- frame index
 struct ovs_frame_index {
@@ -1027,6 +1029,13 @@ struct TriArgs {
     // keypoints with taken[rank] != 0 are skipped, results go to slot q + out_shift
     int q0, out_shift;
     const unsigned char* taken;   // [R] or null
+    // several keyframe pairs in one launch (create_new_landmarks, k_triangulation_topk<true>): query q belongs to problem
+    // p = q / queries_per_prob and reads keyframe-1 entry q - p * queries_per_prob, its problem's E_12 (prob_E[9 p]) and
+    // epipole (prob_epipole[3 p]), and the keyframe-2 arrays (and taken) from entry prob_tbase[p] on; ranks stay per problem
+    int queries_per_prob;
+    const double* prob_E;
+    const double* prob_epipole;
+    const int* prob_tbase;
 };
 
 __device__ __forceinline__ bool epipolar_inlier(const double* E, const double b1x, const double b1y, const double b1z, const double b2x,
@@ -1042,14 +1051,29 @@ __device__ __forceinline__ bool epipolar_inlier(const double* E, const double b1
 }
 
 // one warp per query; keys = distance << 16 | (0xffff - rank): ascending order = the sequential loop's preference
+template <bool kBatched>
 __global__ void __launch_bounds__(128) k_triangulation_topk(TriArgs A, unsigned* __restrict__ keys_out) {
     const int q = A.q0 + blockIdx.x * 4 + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
     if (q >= A.nq) return;
-    const uint4 qa = A.qdesc[2 * (size_t)q], qb = A.qdesc[2 * (size_t)q + 1];
-    const double b1x = A.qbearing[3 * (size_t)q], b1y = A.qbearing[3 * (size_t)q + 1], b1z = A.qbearing[3 * (size_t)q + 2];
-    const float scale = A.qscale[q];
-    const bool stereo_1 = A.qstereo[q] != 0;
+    int qk = q;
+    const double* E = A.E;
+    const double* epipole = A.epipole;
+    const uint4* tdesc = A.tdesc;
+    const double* tbearing = A.tbearing;
+    const unsigned char* tstereo = A.tstereo;
+    const unsigned char* taken = A.taken;
+    if (kBatched) {
+        const int p = q / A.queries_per_prob, base = A.prob_tbase[p];
+        qk = q - p * A.queries_per_prob;
+        E = A.prob_E + 9 * (size_t)p; epipole = A.prob_epipole + 3 * (size_t)p;
+        tdesc += 2 * (size_t)base; tbearing += 3 * (size_t)base; tstereo += base;
+        if (taken) taken += base;
+    }
+    const uint4 qa = A.qdesc[2 * (size_t)qk], qb = A.qdesc[2 * (size_t)qk + 1];
+    const double b1x = A.qbearing[3 * (size_t)qk], b1y = A.qbearing[3 * (size_t)qk + 1], b1z = A.qbearing[3 * (size_t)qk + 2];
+    const float scale = A.qscale[qk];
+    const bool stereo_1 = A.qstereo[qk] != 0;
     const int2 seg = A.qseg[q];
     unsigned extra = 0xffffffffu;   // lane r < 8 carries entry r of the running top-8 from one chunk of candidates to the next
     for (int c0 = seg.x; c0 < seg.y; c0 += 32 * kTriK) {
@@ -1059,18 +1083,18 @@ __global__ void __launch_bounds__(128) k_triangulation_topk(TriArgs A, unsigned*
         for (int k = 0; k < kTriK; ++k) {
             mine[k] = 0xffffffffu;
             const int c = c0 + k * 32 + lane;
-            if (c < seg.y && !(A.taken && A.taken[c])) {
-                const uint4 ta = A.tdesc[2 * (size_t)c], tb = A.tdesc[2 * (size_t)c + 1];
+            if (c < seg.y && !(taken && taken[c])) {
+                const uint4 ta = tdesc[2 * (size_t)c], tb = tdesc[2 * (size_t)c + 1];
                 const int d = __popc(qa.x ^ ta.x) + __popc(qa.y ^ ta.y) + __popc(qa.z ^ ta.z) + __popc(qa.w ^ ta.w)
                               + __popc(qb.x ^ tb.x) + __popc(qb.y ^ tb.y) + __popc(qb.z ^ tb.z) + __popc(qb.w ^ tb.w);
                 if (d <= OVS_HAMMING_DIST_THR_LOW) {
-                    const double b2x = A.tbearing[3 * (size_t)c], b2y = A.tbearing[3 * (size_t)c + 1], b2z = A.tbearing[3 * (size_t)c + 2];
+                    const double b2x = tbearing[3 * (size_t)c], b2y = tbearing[3 * (size_t)c + 1], b2z = tbearing[3 * (size_t)c + 2];
                     bool ok = true;
-                    if (!stereo_1 && !A.tstereo[c]) {
-                        const double cos_dist = A.epipole[0] * b2x + A.epipole[1] * b2y + A.epipole[2] * b2z;
+                    if (!stereo_1 && !tstereo[c]) {
+                        const double cos_dist = epipole[0] * b2x + epipole[1] * b2y + epipole[2] * b2z;
                         if (0.998 < cos_dist) ok = false;
                     }
-                    if (ok && epipolar_inlier(A.E, b1x, b1y, b1z, b2x, b2y, b2z, scale)) mine[k] = ((unsigned)d << 16) | (0xffffu - (unsigned)c);
+                    if (ok && epipolar_inlier(E, b1x, b1y, b1z, b2x, b2y, b2z, scale)) mine[k] = ((unsigned)d << 16) | (0xffffu - (unsigned)c);
                 }
             }
         }
@@ -1094,6 +1118,72 @@ __global__ void __launch_bounds__(128) k_triangulation_topk(TriArgs A, unsigned*
     if (lane < kTriK) keys_out[(size_t)(q + A.out_shift) * kTriK + lane] = extra;
 }
 
+// The keypoints of a keyframe that take part (no landmark, a vocabulary node), node by node and in index order inside a node:
+// the reference's walk over the BoW feature vector.
+void tri_order(int n, const uint8_t* has_lm, const int32_t* bow_node, std::vector<int>& out) {
+    out.clear();
+    for (int i = 0; i < n; ++i) if (!has_lm[i] && bow_node[i] >= 0) out.push_back(i);
+    std::stable_sort(out.begin(), out.end(), [&](int a, int b) { return bow_node[a] < bow_node[b]; });
+}
+
+// seg[k] = the range of rank2 in the node of query q1[k]
+void tri_segments(const std::vector<int>& q1, const int32_t* bow_node_1, const std::vector<int>& rank2, const int32_t* bow_node_2, int2* seg) {
+    size_t lo = 0;
+    for (size_t k = 0; k < q1.size(); ++k) {
+        const int node = bow_node_1[q1[k]];
+        while (lo < rank2.size() && bow_node_2[rank2[lo]] < node) ++lo;
+        size_t hi = lo;
+        while (hi < rank2.size() && bow_node_2[rank2[hi]] == node) ++hi;
+        seg[k] = make_int2((int)lo, (int)hi);
+    }
+}
+
+// The sequential part of match_for_triangulation on one keyframe pair, given each query's candidate list (keys[kTriK k]): the
+// queries k = 0 .. Q - 1 (keyframe-1 keypoint q1[k], in the reference's visiting order; skipped where skip_1[q1[k]] is set, as
+// a keypoint that holds a landmark is no query) each take the first listed candidate not taken yet (taken[rank], all zero on
+// entry); a list of kTriK entries that are all taken may be truncated, so requery(k, &rank) asks the device again with the
+// taken candidates excluded.  Then the orientation histogram, if requested.  matched_idx_2_of_1[n1] (all -1 on entry) gets
+// rank2[rank] of each match; slot_of_1 (may be null) the list entry kTriK k + j it came from, or -1 - k for a re-query.
+template <class Requery>
+int tri_replay(ovs_matcher* m, int Q, const int* q1, const int* rank2, const unsigned* keys, unsigned char* taken, const uint8_t* skip_1,
+               const float* angle_1, const float* angle_2, int check_orientation, Requery&& requery, int32_t* matched_idx_2_of_1,
+               int32_t* slot_of_1, int* num_matches) {
+    std::vector<float> deltas; std::vector<int> delta_idx;
+    int num = 0;
+    for (int k = 0; k < Q; ++k) {
+        const int i1 = q1[k];
+        if (skip_1 && skip_1[i1]) continue;
+        const unsigned* lk = keys + (size_t)k * kTriK;
+        int pick = -1, seen = 0, slot = -1;
+        for (int j = 0; j < kTriK && lk[j] != 0xffffffffu; ++j) {
+            ++seen;
+            const int r = 0xffff - (int)(lk[j] & 0xffffu);
+            if (!taken[r]) { pick = r; slot = kTriK * k + j; break; }
+        }
+        if (pick < 0 && seen == kTriK) {
+            // all 8 listed candidates were taken and the list may be truncated (rare: needs 8 earlier keypoints of the same
+            // node to have claimed them).  The replay is sequential, so it waits for the answer.
+            ++m->num_requeries;
+            const int rc = requery(k, &pick);
+            if (rc != OVS_OK) return rc;
+            slot = -1 - k;
+        }
+        if (pick < 0) continue;
+        taken[pick] = 1;
+        matched_idx_2_of_1[i1] = rank2[pick];
+        if (slot_of_1) slot_of_1[i1] = slot;
+        ++num;
+        if (check_orientation) { deltas.push_back(angle_1[i1] - angle_2[rank2[pick]]); delta_idx.push_back(i1); }
+    }
+    if (check_orientation && !deltas.empty()) {
+        std::vector<uint8_t> invalid;
+        angle_checker_invalid(deltas, invalid);
+        for (size_t k = 0; k < deltas.size(); ++k) if (invalid[k]) { matched_idx_2_of_1[delta_idx[k]] = -1; --num; }
+    }
+    *num_matches = num;
+    return OVS_OK;
+}
+
 }  // namespace
 
 extern "C" int ovs_robust_match_for_triangulation_host(ovs_matcher* m, int n1, const uint8_t* desc_1, const double* bearing_1, const int32_t* octave_1,
@@ -1113,27 +1203,14 @@ extern "C" int ovs_robust_match_for_triangulation_host(ovs_matcher* m, int n1, c
     for (int i = 0; i < n1; ++i)
         OVS_REQUIRE(octave_1[i] >= 0 && octave_1[i] < num_scale_levels, OVS_ERR_INVALID_ARG, "octave %d of keypoint %d outside the scale table", octave_1[i], i);
     OVS_CUDA_CHECK(cudaSetDevice(m->device));
-    // keyframe 2: eligible keypoints (no landmark, has a node) node by node, index order inside a node
-    std::vector<int> rank2;
-    for (int i = 0; i < n2; ++i) if (!has_lm_2[i] && bow_node_2[i] >= 0) rank2.push_back(i);
-    std::stable_sort(rank2.begin(), rank2.end(), [&](int a, int b) { return bow_node_2[a] < bow_node_2[b]; });
-    // keyframe 1: queries in the order the reference visits them (node ascending, index ascending)
-    std::vector<int> q1;
-    for (int i = 0; i < n1; ++i) if (!has_lm_1[i] && bow_node_1[i] >= 0) q1.push_back(i);
-    std::stable_sort(q1.begin(), q1.end(), [&](int a, int b) { return bow_node_1[a] < bow_node_1[b]; });
+    // keyframe 2: candidates; keyframe 1: queries in the order the reference visits them
+    std::vector<int> rank2, q1;
+    tri_order(n2, has_lm_2, bow_node_2, rank2);
+    tri_order(n1, has_lm_1, bow_node_1, q1);
     const int R = (int)rank2.size(), Q = (int)q1.size();
     if (R == 0 || Q == 0) return OVS_OK;
     std::vector<int2> seg(Q);
-    {
-        size_t lo = 0;
-        for (int k = 0; k < Q; ++k) {
-            const int node = bow_node_1[q1[k]];
-            while (lo < rank2.size() && bow_node_2[rank2[lo]] < node) ++lo;
-            size_t hi = lo;
-            while (hi < rank2.size() && bow_node_2[rank2[hi]] == node) ++hi;
-            seg[k] = make_int2((int)lo, (int)hi);
-        }
-    }
+    tri_segments(q1, bow_node_1, rank2, bow_node_2, seg.data());
     const size_t sQ = (size_t)Q, sR = (size_t)R;
     TriArgs A{};
     uint8_t *hqd, *htd, *hq8, *ht8, *taken, *dtaken; double *hqb, *htb; int2* hsg; float* hqs;
@@ -1167,55 +1244,206 @@ extern "C" int ovs_robust_match_for_triangulation_host(ovs_matcher* m, int n1, c
     for (int k = 0; k < 9; ++k) A.E[k] = E_12[k];
     for (int k = 0; k < 3; ++k) A.epipole[k] = epipole_in_2[k];
     OVS_CUDA_CHECK(cudaEventRecord(m->ev[0], st));
-    k_triangulation_topk<<<(Q + 3) / 4, 128, 0, st>>>(A, m->d_keys);
+    k_triangulation_topk<false><<<(Q + 3) / 4, 128, 0, st>>>(A, m->d_keys);
     OVS_LAUNCH_CHECK();
     OVS_CUDA_CHECK(cudaEventRecord(m->ev[1], st));
     OVS_CUDA_CHECK(cudaMemcpyAsync(m->h_keys, m->d_keys, (size_t)Q * kTriK * 4, cudaMemcpyDeviceToHost, st));
     OVS_CUDA_CHECK(ovs::sync_stream(st));
     float ms = 0; cudaEventElapsedTime(&ms, m->ev[0], m->ev[1]);
     m->last_kernel_us = ms * 1000.f;
-    // sequential replay: a keyframe-2 keypoint goes to its first taker (the flags live in the pinned staging area so that
-    // a re-query can upload the slice of a node)
+    // the flags live in the pinned staging area so that a re-query can upload the slice of a node
     memset(taken, 0, (size_t)R);
-    std::vector<float> deltas; std::vector<int> delta_idx;
-    int num = 0;
+    auto requery = [&](int k, int* pick) -> int {
+        const size_t len = (size_t)(seg[k].y - seg[k].x);
+        OVS_CUDA_CHECK(cudaMemcpyAsync(dtaken + seg[k].x, taken + seg[k].x, len, cudaMemcpyHostToDevice, st));
+        TriArgs B = A;
+        B.q0 = k; B.nq = k + 1; B.out_shift = Q - k; B.taken = dtaken;
+        k_triangulation_topk<false><<<1, 128, 0, st>>>(B, m->d_keys);
+        OVS_LAUNCH_CHECK();
+        OVS_CUDA_CHECK(cudaMemcpyAsync(m->h_keys + (size_t)Q * kTriK, m->d_keys + (size_t)Q * kTriK, kTriK * 4, cudaMemcpyDeviceToHost, st));
+        OVS_CUDA_CHECK(ovs::sync_stream(st));
+        const unsigned key = m->h_keys[(size_t)Q * kTriK];
+        *pick = key != 0xffffffffu ? 0xffff - (int)(key & 0xffffu) : -1;
+        return OVS_OK;
+    };
+    return tri_replay(m, Q, q1.data(), rank2.data(), m->h_keys, taken, nullptr, angle_1, angle_2, check_orientation, requery,
+                      matched_idx_2_of_1, nullptr, num_matches);
+}
+
+// mapping_module::create_new_landmarks' compute step (ovs_b200.h): the candidate lists of every (neighbour, query) in one launch
+// and the triangulation of every listed candidate in another (a list does not depend on the other queries and a pair's
+// triangulation only on keyframe data), then the neighbour-by-neighbour replay on the host, where a keyframe-1 keypoint that got a
+// landmark from an earlier neighbour is no query any more, and one gather of the chosen points.
+extern "C" int ovs_create_new_landmarks_host(ovs_matcher* m, const ovs_keyframe_view* keyfrm_1, int B, const ovs_keyframe_view* keyfrms_2,
+                                             const double* E_12, const double* epipole_in_2, int check_orientation, double rays_parallax_deg_thr,
+                                             ovs_new_landmark* out, int capacity, int* num_out) {
+    OVS_REQUIRE(m && num_out && B >= 0 && B <= 65535, OVS_ERR_INVALID_ARG, "bad argument (B must be in 0 .. 65535)");
+    int rc;
+    double cos_thr;
+    if ((rc = ovs::tri_cos_thr(rays_parallax_deg_thr, &cos_thr)) != OVS_OK) return rc;
+    if ((rc = ovs::check_keyframe_view(keyfrm_1, true, "keyframe", 1)) != OVS_OK) return rc;
+    const ovs_keyframe_view& K1 = *keyfrm_1;
+    const int n1 = K1.num_keypts;
+    OVS_REQUIRE(capacity >= n1 && (n1 == 0 || out), OVS_ERR_CAPACITY, "capacity %d below the %d keypoints of keyframe 1", capacity, n1);
+    OVS_REQUIRE(B == 0 || (keyfrms_2 && E_12 && epipole_in_2), OVS_ERR_INVALID_ARG, "null argument");
+    for (int i = 0; i < n1; ++i)
+        if ((rc = ovs::check_tri_keypt(K1, i, "keyframe", 1)) != OVS_OK) return rc;
+    for (int b = 0; b < B; ++b) {
+        const ovs_keyframe_view& K2 = keyfrms_2[b];
+        if ((rc = ovs::check_keyframe_view(&K2, true, "neighbour", b)) != OVS_OK) return rc;
+        OVS_REQUIRE(K2.num_keypts < 65536, OVS_ERR_UNSUPPORTED, "neighbour %d has more than 65535 keypoints", b);
+        for (int i = 0; i < K2.num_keypts; ++i)
+            if ((rc = ovs::check_tri_keypt(K2, i, "neighbour", b)) != OVS_OK) return rc;
+        for (int k = 0; k < 9; ++k) OVS_REQUIRE(std::isfinite(E_12[9 * (size_t)b + k]), OVS_ERR_INVALID_ARG, "E_12 of neighbour %d is not finite", b);
+        for (int k = 0; k < 3; ++k)
+            OVS_REQUIRE(std::isfinite(epipole_in_2[3 * (size_t)b + k]), OVS_ERR_INVALID_ARG, "epipole of neighbour %d is not finite", b);
+    }
+    *num_out = 0;
+    std::vector<int> q1;
+    tri_order(n1, K1.has_landmark, K1.bow_node, q1);
+    const int Q = (int)q1.size();
+    std::vector<std::vector<int>> rank2((size_t)B);
+    std::vector<int> tbase((size_t)B + 1, 0);
+    for (int b = 0; b < B; ++b) {
+        tri_order(keyfrms_2[b].num_keypts, keyfrms_2[b].has_landmark, keyfrms_2[b].bow_node, rank2[b]);
+        tbase[b + 1] = tbase[b] + (int)rank2[b].size();
+    }
+    const int R = tbase[B];
+    // every (neighbour, query) has a list of kTriK slots, plus one re-query slot: the slot index of the kernels is an int
+    OVS_REQUIRE(((int64_t)B * Q + 1) * kTriK <= INT32_MAX, OVS_ERR_UNSUPPORTED,
+                "%d neighbours x %d queries: more candidate slots than one call holds (2^31 - 1)", B, Q);
+    if (Q == 0 || R == 0) return OVS_OK;
+    OVS_CUDA_CHECK(cudaSetDevice(m->device));
+    // queries of all neighbours, then one re-query slot; keypoint records: the Q queries of keyframe 1, then every candidate
+    const size_t sQ = (size_t)Q, sR = (size_t)R, NB = (size_t)B, NQ = NB * sQ, NS = (NQ + 1) * kTriK;
+    TriArgs A{};
+    ovs::TriLaunch L{};
+    uint8_t *hqd, *htd, *hq8, *ht8, *taken, *dtaken, *hvalid; double *hqb, *htb, *hE, *hep, *hrq, *drq, *hgpos, *dgpos; int2* hsg;
+    float* hqs; int *htb0, *hchosen, *dchosen; unsigned* hkeys; unsigned* dkeys; ovs::TriProblem* hprob; ovs::TriKeypt* hkp;
+    ovs::Staging S;
+    rc = ovs::stage(S, m->h_tri, m->h_tri_cap, m->d_tri, m->d_tri_cap, [&](ovs::Staging& S) {
+        A.qdesc = (const uint4*)S.in(hqd, 32 * sQ); A.tdesc = (const uint4*)S.in(htd, 32 * sR);
+        A.qbearing = S.in(hqb, 3 * sQ); A.tbearing = S.in(htb, 3 * sR); A.qseg = S.in(hsg, NQ); A.qscale = S.in(hqs, sQ);
+        A.qstereo = S.in(hq8, sQ); A.tstereo = S.in(ht8, sR);
+        A.prob_E = S.in(hE, 9 * NB); A.prob_epipole = S.in(hep, 3 * NB); A.prob_tbase = S.in(htb0, NB);
+        L.prob = S.in(hprob, NB); L.kp = S.in(hkp, sQ + sR); L.rank_base = A.prob_tbase;
+        dkeys = S.out(hkeys, NS); L.valid = S.out(hvalid, NS);
+        // host and device halves of the replay's own transfers, each copied explicitly when it is needed (the lists' download
+        // below stops before them): the taken flags (a node's slice per re-query), a re-query's point, the gather's slots and points
+        dtaken = S.out(taken, sR);
+        drq = S.out(hrq, 3);
+        dchosen = S.out(hchosen, (size_t)n1); dgpos = S.out(hgpos, 3 * (size_t)n1);
+        L.pos = S.dev<double>(3 * NS);
+    });
+    if (rc != OVS_OK) return rc;
     for (int k = 0; k < Q; ++k) {
-        const int i1 = q1[k];
-        const unsigned* keys = m->h_keys + (size_t)k * kTriK;
-        int pick = -1, seen = 0;
-        for (int j = 0; j < kTriK && keys[j] != 0xffffffffu; ++j) {
-            ++seen;
-            const int r = 0xffff - (int)(keys[j] & 0xffffu);
-            if (!taken[r]) { pick = r; break; }
+        const int i = q1[k];
+        memcpy(hqd + 32 * (size_t)k, K1.descriptors + 32 * (size_t)i, 32);
+        memcpy(hqb + 3 * (size_t)k, K1.bearings + 3 * (size_t)i, 24);
+        hqs[k] = K1.scale_factors[K1.undist_keypts[i].octave];
+        hq8[k] = K1.stereo_x_right && 0.0f <= K1.stereo_x_right[i];
+        hkp[k] = ovs::tri_keypt(K1, i);
+    }
+    for (int b = 0; b < B; ++b) {
+        const ovs_keyframe_view& K2 = keyfrms_2[b];
+        const std::vector<int>& rk = rank2[b];
+        for (size_t r = 0; r < rk.size(); ++r) {
+            const int i = rk[r];
+            const size_t g = (size_t)tbase[b] + r;
+            memcpy(htd + 32 * g, K2.descriptors + 32 * (size_t)i, 32);
+            memcpy(htb + 3 * g, K2.bearings + 3 * (size_t)i, 24);
+            ht8[g] = K2.stereo_x_right && 0.0f <= K2.stereo_x_right[i];
+            hkp[sQ + g] = ovs::tri_keypt(K2, i);
         }
-        if (pick < 0 && seen == kTriK) {
-            // all 8 listed candidates were taken and the list may be truncated: ask the GPU again for this keypoint alone,
-            // with the keyframe-2 keypoints of its node that are already claimed excluded (rare: needs 8 earlier keypoints
-            // of the same node to have claimed them).  The replay is sequential, so it waits for the answer.
-            ++m->num_requeries;
-            const size_t len = (size_t)(seg[k].y - seg[k].x);
-            OVS_CUDA_CHECK(cudaMemcpyAsync(dtaken + seg[k].x, taken + seg[k].x, len, cudaMemcpyHostToDevice, st));
-            TriArgs B = A;
-            B.q0 = k; B.nq = k + 1; B.out_shift = Q - k; B.taken = dtaken;
-            k_triangulation_topk<<<1, 128, 0, st>>>(B, m->d_keys);
+        tri_segments(q1, K1.bow_node, rk, K2.bow_node, hsg + sQ * b);
+        memcpy(hE + 9 * b, E_12 + 9 * (size_t)b, 72); memcpy(hep + 3 * b, epipole_in_2 + 3 * (size_t)b, 24);
+        htb0[b] = tbase[b];
+        hprob[b].c[0] = ovs::tri_cam(K1); hprob[b].c[1] = ovs::tri_cam(K2);
+        hprob[b].ratio_factor = 1.5f * K1.scale_factor;
+    }
+    A.nq = (int)NQ; A.queries_per_prob = Q;
+    L.n = (int)(NQ * kTriK); L.cos_thr = cos_thr; L.keys = dkeys; L.queries_per_prob = Q; L.fixed_prob = -1; L.rec_2_base = Q;
+    cudaStream_t st = m->stream;
+    OVS_CUDA_CHECK(S.upload(st));
+    OVS_CUDA_CHECK(cudaEventRecord(m->ev[0], st));
+    k_triangulation_topk<true><<<(A.nq + 3) / 4, 128, 0, st>>>(A, dkeys);
+    OVS_LAUNCH_CHECK();
+    if ((rc = ovs::launch_two_view_triangulate(L, st)) != OVS_OK) return rc;
+    OVS_CUDA_CHECK(cudaEventRecord(m->ev[1], st));
+    // the keys and the valid flags, carved one after the other: one copy
+    const size_t list_bytes = (size_t)((const uint8_t*)(hvalid + NS) - (const uint8_t*)hkeys);
+    OVS_CUDA_CHECK(cudaMemcpyAsync(hkeys, dkeys, list_bytes, cudaMemcpyDeviceToHost, st));
+    OVS_CUDA_CHECK(ovs::sync_stream(st));
+    float ms = 0; cudaEventElapsedTime(&ms, m->ev[0], m->ev[1]);
+    m->last_kernel_us = ms * 1000.f;
+
+    std::vector<uint8_t> got((size_t)n1, 0);           // keyframe-1 keypoints that got a landmark in this call
+    std::vector<int32_t> match((size_t)n1), slot((size_t)n1);
+    std::vector<float> angle_1((size_t)n1), angle_2;
+    for (int i = 0; i < n1; ++i) angle_1[i] = K1.undist_keypts[i].angle;
+    std::vector<int> list_rec;                           // records whose point comes from a list slot, in record order
+    int num = 0;
+    for (int b = 0; b < B; ++b) {
+        const ovs_keyframe_view& K2 = keyfrms_2[b];
+        const size_t qoff = sQ * b;
+        std::vector<double> rq_pos((size_t)3 * Q);       // a re-queried pair's point, by query
+        std::vector<uint8_t> rq_valid((size_t)Q, 0);
+        auto requery = [&](int k, int* pick) -> int {
+            const int2 sg = hsg[qoff + k];
+            OVS_CUDA_CHECK(cudaMemcpyAsync(dtaken + tbase[b] + sg.x, taken + tbase[b] + sg.x, (size_t)(sg.y - sg.x), cudaMemcpyHostToDevice, st));
+            TriArgs Aq = A;
+            Aq.q0 = (int)qoff + k; Aq.nq = Aq.q0 + 1; Aq.out_shift = (int)NQ - Aq.q0; Aq.taken = dtaken;
+            k_triangulation_topk<true><<<1, 128, 0, st>>>(Aq, dkeys);
             OVS_LAUNCH_CHECK();
-            OVS_CUDA_CHECK(cudaMemcpyAsync(m->h_keys + (size_t)Q * kTriK, m->d_keys + (size_t)Q * kTriK, kTriK * 4, cudaMemcpyDeviceToHost, st));
+            ovs::TriLaunch Lq = L;
+            Lq.n = 1; Lq.keys = dkeys + NQ * kTriK; Lq.fixed_prob = b; Lq.fixed_query = k; Lq.valid = L.valid + NQ * kTriK; Lq.pos = drq;
+            const int rc2 = ovs::launch_two_view_triangulate(Lq, st);
+            if (rc2 != OVS_OK) return rc2;
+            OVS_CUDA_CHECK(cudaMemcpyAsync(hkeys + NQ * kTriK, dkeys + NQ * kTriK, 4, cudaMemcpyDeviceToHost, st));
+            OVS_CUDA_CHECK(cudaMemcpyAsync(hvalid + NQ * kTriK, L.valid + NQ * kTriK, 1, cudaMemcpyDeviceToHost, st));
+            OVS_CUDA_CHECK(cudaMemcpyAsync(hrq, drq, 24, cudaMemcpyDeviceToHost, st));
             OVS_CUDA_CHECK(ovs::sync_stream(st));
-            const unsigned key = m->h_keys[(size_t)Q * kTriK];
-            if (key != 0xffffffffu) pick = 0xffff - (int)(key & 0xffffu);
+            const unsigned key = hkeys[NQ * kTriK];
+            *pick = key != 0xffffffffu ? 0xffff - (int)(key & 0xffffu) : -1;
+            rq_valid[k] = hvalid[NQ * kTriK];
+            for (int c = 0; c < 3; ++c) rq_pos[3 * (size_t)k + c] = hrq[c];
+            return OVS_OK;
+        };
+        angle_2.resize((size_t)K2.num_keypts);
+        for (int i = 0; i < K2.num_keypts; ++i) angle_2[i] = K2.undist_keypts[i].angle;
+        memset(taken + tbase[b], 0, rank2[b].size());
+        std::fill(match.begin(), match.end(), -1);
+        int nm = 0;
+        if ((rc = tri_replay(m, Q, q1.data(), rank2[b].data(), hkeys + qoff * kTriK, taken + tbase[b], got.data(), angle_1.data(),
+                             angle_2.data(), check_orientation, requery, match.data(), slot.data(), &nm)) != OVS_OK)
+            return rc;
+        // triangulate_with_two_keyframes: the pairs in idx_1 order
+        for (int i1 = 0; i1 < n1; ++i1) {
+            if (match[i1] < 0) continue;
+            const int sl = slot[i1];
+            if (!(sl >= 0 ? hvalid[qoff * kTriK + sl] : rq_valid[-1 - sl])) continue;
+            ovs_new_landmark& r = out[num];
+            r.neighbour = b; r.idx_1 = i1; r.idx_2 = match[i1]; r.reserved = 0;
+            if (sl >= 0) {
+                hchosen[list_rec.size()] = (int)(qoff * kTriK) + sl;
+                list_rec.push_back(num);
+            } else {
+                for (int c = 0; c < 3; ++c) r.pos_w[c] = rq_pos[3 * (size_t)(-1 - sl) + c];
+            }
+            got[i1] = 1;
+            ++num;
         }
-        if (pick < 0) continue;
-        taken[pick] = 1;
-        matched_idx_2_of_1[i1] = rank2[pick];
-        ++num;
-        if (check_orientation) { deltas.push_back(angle_1[i1] - angle_2[rank2[pick]]); delta_idx.push_back(i1); }
     }
-    if (check_orientation && !deltas.empty()) {
-        std::vector<uint8_t> invalid;
-        angle_checker_invalid(deltas, invalid);
-        for (size_t k = 0; k < deltas.size(); ++k) if (invalid[k]) { matched_idx_2_of_1[delta_idx[k]] = -1; --num; }
+    const int nc = (int)list_rec.size();
+    if (nc > 0) {
+        OVS_CUDA_CHECK(cudaMemcpyAsync(dchosen, hchosen, 4 * (size_t)nc, cudaMemcpyHostToDevice, st));
+        if ((rc = ovs::launch_gather_pos(nc, dchosen, L.pos, dgpos, st)) != OVS_OK) return rc;
+        OVS_CUDA_CHECK(cudaMemcpyAsync(hgpos, dgpos, 24 * (size_t)nc, cudaMemcpyDeviceToHost, st));
+        OVS_CUDA_CHECK(ovs::sync_stream(st));
+        for (int j = 0; j < nc; ++j)
+            for (int c = 0; c < 3; ++c) out[list_rec[j]].pos_w[c] = hgpos[3 * (size_t)j + c];
     }
-    *num_matches = num;
+    *num_out = num;
     return OVS_OK;
 }
 
