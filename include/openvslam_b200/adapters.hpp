@@ -20,6 +20,9 @@
 //     get_best_H_21() / get_best_F_21(), get_inlier_matches()                    (solve/{homography,fundamental}_solver.h)
 //   the compute step of mapping_module::create_new_landmarks over data::keyframe (module/mapping_module.cc): match_for_triangulation
 //     and two_view_triangulator::triangulate for every neighbour, as module::two_view_triangulator::create_new_landmarks
+//   initialize::perspective / initialize::bearing_vector(const data::frame&, unsigned, unsigned, float, float),
+//     initialize(const data::frame&, const std::vector<int>&), get_{rotation,translation}_ref_to_cur(),
+//     get_triangulated_{pts,flags}()                                                           (initialize/{perspective,bearing_vector}.h)
 //
 // Include it INSTEAD of openvslam_b200.hpp in a translation unit that can see the reference's headers (here: the stand-ins
 // under tests/cpp/standin, which declare the members used below with the names recalled in SURVEY.md section 2 / 8b;
@@ -600,6 +603,83 @@ inline std::vector<ovs_new_landmark> module::two_view_triangulator::create_new_l
         adapters::e12_and_epipole(k1.view.pose_cw, own.back().view.pose_cw, E[b], ep[b]);
     }
     return create_new_landmarks(k1.view, views, E, ep, check_orientation);
+}
+
+// ------------------------------------------------------------------------------------------- initialize::perspective / bearing_vector
+namespace adapters {
+
+//! camera_, undist_keypts_ (cv::KeyPoint is ovs_keypoint's layout) and bearings_ of a frame as an ovs_init_view; the bearings are
+//! copied into `bearings` (3 doubles per keypoint), which must outlive the view.
+template <class Frame>
+ovs_init_view init_view(const Frame& frm, std::vector<double>& bearings) {
+    bearings = flat_bearings(frm.bearings_);
+    ovs_init_view v{};
+    v.camera = to_camera(frm.camera_);
+    v.num_keypts = static_cast<std::int32_t>(frm.undist_keypts_.size());
+    v.undist_keypts = reinterpret_cast<const ovs_keypoint*>(frm.undist_keypts_.data());
+    v.bearings = bearings.data();
+    return v;
+}
+
+//! The sampler seed of an initialize() on the reference's frames: the hash of both views' keypoints and bearings and the matches.
+inline std::uint64_t init_seed(const ovs_init_view& ref, const ovs_init_view& cur, const std::vector<int>& ref_matches_with_cur) {
+    input_hash hash(static_cast<std::size_t>(ref.num_keypts) + static_cast<std::size_t>(cur.num_keypts));
+    for (const ovs_init_view* v : {&ref, &cur}) {
+        for (int i = 0; i < v->num_keypts; ++i) hash.add(&v->undist_keypts[i].x, 8);
+        hash.add(v->bearings, 24 * static_cast<std::size_t>(v->num_keypts));
+    }
+    hash.add(ref_matches_with_cur.data(), sizeof(int) * ref_matches_with_cur.size());
+    return hash.seed;
+}
+
+}  // namespace adapters
+
+template <class Frame>
+inline initialize::perspective::perspective(const Frame& ref_frm, const unsigned int num_ransac_iters, const unsigned int min_num_triangulated,
+                                            const float parallax_deg_thr, const float reproj_err_thr, const int device)
+    : base(true, nullptr, num_ransac_iters, min_num_triangulated, parallax_deg_thr, reproj_err_thr, device) {
+    own_ref_ = adapters::init_view(ref_frm, own_ref_bearings_);
+    ref_ = &own_ref_;
+}
+
+template <class Frame>
+inline initialize::bearing_vector::bearing_vector(const Frame& ref_frm, const unsigned int num_ransac_iters,
+                                                  const unsigned int min_num_triangulated, const float parallax_deg_thr,
+                                                  const float reproj_err_thr, const int device)
+    : base(false, nullptr, num_ransac_iters, min_num_triangulated, parallax_deg_thr, reproj_err_thr, device) {
+    own_ref_ = adapters::init_view(ref_frm, own_ref_bearings_);
+    ref_ = &own_ref_;
+}
+
+template <class Frame>
+inline bool initialize::base::initialize(const Frame& cur_frm, const std::vector<int>& ref_matches_with_cur) {
+    std::vector<double> bearings;
+    const ovs_init_view cur = adapters::init_view(cur_frm, bearings);
+    return initialize(cur, ref_matches_with_cur, adapters::init_seed(*ref_, cur, ref_matches_with_cur));
+}
+
+inline Mat33_t initialize::base::get_rotation_ref_to_cur() const {
+    Mat33_t R;
+    for (int r = 0; r < 3; ++r)
+        for (int c = 0; c < 3; ++c) R(r, c) = last_.record.rot_ref_to_cur[3 * r + c];
+    return R;
+}
+
+inline Vec3_t initialize::base::get_translation_ref_to_cur() const {
+    Vec3_t t;
+    for (int r = 0; r < 3; ++r) t(r) = last_.record.trans_ref_to_cur[r];
+    return t;
+}
+
+inline std::vector<Vec3_t> initialize::base::get_triangulated_pts() const {
+    std::vector<Vec3_t> out(last_.is_triangulated.size());
+    for (std::size_t i = 0; i < out.size(); ++i)
+        for (int r = 0; r < 3; ++r) out[i](r) = last_.triangulated_pts[3 * i + r];
+    return out;
+}
+
+inline std::vector<bool> initialize::base::get_triangulated_flags() const {
+    return std::vector<bool>(last_.is_triangulated.begin(), last_.is_triangulated.end());
 }
 
 }  // namespace openvslam

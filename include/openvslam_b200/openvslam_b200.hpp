@@ -1022,4 +1022,145 @@ private:
 };
 
 }  // namespace module
+
+namespace initialize {
+
+//! What initialize::perspective and initialize::bearing_vector share (initialize/base.h): the constructor's settings, a matcher
+//! handle (its CUDA stream and buffers) and the outcome of the last initialize().  On array views (ovs_init_view: a frame's
+//! camera, undist_keypts_.data() and its bearings as 3 doubles per keypoint; the views must outlive the call).
+class base {
+public:
+    //! One problem of the batched form: a reference view, a current view, ref_matches_with_cur (one entry per reference keypoint,
+    //! -1 = none) and the sampler seed.
+    struct problem {
+        const ovs_init_view* ref;
+        const ovs_init_view* cur;
+        std::vector<int> ref_matches_with_cur;
+        std::uint64_t seed;
+    };
+    //! One problem's outcome: the C ABI's record, and per reference keypoint the flag and the point (3 doubles).
+    struct result {
+        ovs_init_result record;
+        std::vector<std::uint8_t> is_triangulated;
+        std::vector<double> triangulated_pts;
+    };
+
+    base(const base&) = delete;
+    base& operator=(const base&) = delete;
+    virtual ~base() { ovs_matcher_destroy(h_); }
+    ovs_matcher* handle() const { return h_; }
+
+    //! initialize(cur_frm, ref_matches_with_cur) on the constructor's reference view with one sampler seed (used by every solver
+    //! of the call).  True when the map can be built from the getters below.
+    bool initialize(const ovs_init_view& cur, const std::vector<int>& ref_matches_with_cur, const std::uint64_t seed) {
+        if (!ref_) throw std::runtime_error("ovs_b200: initializer built without its reference view");
+        std::vector<result> r;
+        initialize(std::vector<problem>{problem{ref_, &cur, ref_matches_with_cur, seed}}, r);
+        last_ = std::move(r.front());
+        return last_.record.status == OVS_INIT_OK;
+    }
+    //! The same for B problems in one GPU call, with this object's settings; results[b] per problem.
+    void initialize(const std::vector<problem>& problems, std::vector<result>& results) const {
+        const std::size_t B = problems.size();
+        std::vector<ovs_init_view> refs(B), curs(B);
+        std::vector<std::int32_t> rm;
+        std::vector<std::uint64_t> seeds(B);
+        std::vector<std::size_t> off(B + 1, 0);
+        for (std::size_t b = 0; b < B; ++b) {
+            refs[b] = *problems[b].ref; curs[b] = *problems[b].cur; seeds[b] = problems[b].seed;
+            if (problems[b].ref_matches_with_cur.size() != static_cast<std::size_t>(refs[b].num_keypts))
+                throw std::runtime_error("ovs_b200: ref_matches_with_cur needs one entry per reference keypoint");
+            rm.insert(rm.end(), problems[b].ref_matches_with_cur.begin(), problems[b].ref_matches_with_cur.end());
+            off[b + 1] = rm.size();
+        }
+        const std::size_t K = rm.size();
+        std::vector<ovs_init_result> rec(std::max<std::size_t>(B, 1));
+        std::vector<std::uint8_t> flags(std::max<std::size_t>(K, 1));
+        std::vector<double> pts(3 * std::max<std::size_t>(K, 1));
+        detail::check((perspective_ ? ovs_initialize_perspective_host : ovs_initialize_bearing_vector_host)(
+            h_, static_cast<int>(B), refs.data(), curs.data(), rm.data(), static_cast<int>(num_ransac_iters_),
+            static_cast<int>(min_num_triangulated_), parallax_deg_thr_, reproj_err_thr_sq_, seeds.data(), rec.data(), flags.data(), pts.data()));
+        results.assign(B, result{});
+        for (std::size_t b = 0; b < B; ++b) {
+            results[b].record = rec[b];
+            results[b].is_triangulated.assign(flags.begin() + off[b], flags.begin() + off[b + 1]);
+            results[b].triangulated_pts.assign(pts.begin() + 3 * off[b], pts.begin() + 3 * off[b + 1]);
+        }
+    }
+
+    //! The last initialize()'s outcome on arrays: R row-major, t (unit norm), the flags and points per reference keypoint.
+    const ovs_init_result& last_result() const { return last_.record; }
+    std::array<double, 9> rotation_ref_to_cur() const {
+        std::array<double, 9> R;
+        std::copy(last_.record.rot_ref_to_cur, last_.record.rot_ref_to_cur + 9, R.begin());
+        return R;
+    }
+    std::array<double, 3> translation_ref_to_cur() const {
+        return {last_.record.trans_ref_to_cur[0], last_.record.trans_ref_to_cur[1], last_.record.trans_ref_to_cur[2]};
+    }
+    const std::vector<double>& triangulated_pts() const { return last_.triangulated_pts; }
+    const std::vector<std::uint8_t>& triangulated_flags() const { return last_.is_triangulated; }
+#ifdef OVS_B200_WITH_REFERENCE_TYPES
+    //! The reference's getters (bodies in adapters.hpp).
+    Mat33_t get_rotation_ref_to_cur() const;
+    Vec3_t get_translation_ref_to_cur() const;
+    std::vector<Vec3_t> get_triangulated_pts() const;
+    std::vector<bool> get_triangulated_flags() const;
+    //! initialize(cur_frm, ref_matches_with_cur) on the reference's frame (data::frame in the reference tree; body in adapters.hpp):
+    //! reads camera_, undist_keypts_ and bearings_; the sampler seed hashes both views and the matches.  A template deduced from its
+    //! argument, so it is compiled only where it is called.
+    template <class Frame>
+    bool initialize(const Frame& cur_frm, const std::vector<int>& ref_matches_with_cur);
+#endif
+
+protected:
+    //! The reference's constructor arguments (reproj_err_thr is compared with the squared pixel error, as check_pose does).
+    base(const bool perspective, const ovs_init_view* ref, const unsigned int num_ransac_iters, const unsigned int min_num_triangulated,
+         const float parallax_deg_thr, const float reproj_err_thr, const int device)
+        : perspective_(perspective), ref_(ref), num_ransac_iters_(num_ransac_iters), min_num_triangulated_(min_num_triangulated),
+          parallax_deg_thr_(parallax_deg_thr), reproj_err_thr_sq_(reproj_err_thr) {
+        detail::check(ovs_matcher_create(device, &h_));
+    }
+
+    const bool perspective_;
+    const ovs_init_view* ref_;
+    // the reference view's own arrays when the object was built from a frame (adapters.hpp)
+    ovs_init_view own_ref_{};
+    std::vector<double> own_ref_bearings_;
+    const unsigned int num_ransac_iters_, min_num_triangulated_;
+    const float parallax_deg_thr_, reproj_err_thr_sq_;
+    ovs_matcher* h_ = nullptr;
+    result last_{};
+};
+
+//! initialize::perspective (initialize/perspective.h): perspective cameras, and fisheye ones passed as perspective on their
+//! undistorted keypoints.  The homography and fundamental-matrix solvers, the model choice, the decomposition and check_pose.
+class perspective : public base {
+public:
+    perspective(const ovs_init_view& ref, const unsigned int num_ransac_iters = 100, const unsigned int min_num_triangulated = 50,
+                const float parallax_deg_thr = 1.0f, const float reproj_err_thr = 4.0f, const int device = 0)
+        : base(true, &ref, num_ransac_iters, min_num_triangulated, parallax_deg_thr, reproj_err_thr, device) {}
+#ifdef OVS_B200_WITH_REFERENCE_TYPES
+    //! The reference's constructor on its frame (body in adapters.hpp).
+    template <class Frame>
+    perspective(const Frame& ref_frm, const unsigned int num_ransac_iters, const unsigned int min_num_triangulated,
+                const float parallax_deg_thr, const float reproj_err_thr, const int device = 0);
+#endif
+};
+
+//! initialize::bearing_vector (initialize/bearing_vector.h): equirectangular cameras; the essential solver, 4 hypotheses, no depth
+//! test.
+class bearing_vector : public base {
+public:
+    bearing_vector(const ovs_init_view& ref, const unsigned int num_ransac_iters = 100, const unsigned int min_num_triangulated = 50,
+                   const float parallax_deg_thr = 1.0f, const float reproj_err_thr = 4.0f, const int device = 0)
+        : base(false, &ref, num_ransac_iters, min_num_triangulated, parallax_deg_thr, reproj_err_thr, device) {}
+#ifdef OVS_B200_WITH_REFERENCE_TYPES
+    template <class Frame>
+    bearing_vector(const Frame& ref_frm, const unsigned int num_ransac_iters, const unsigned int min_num_triangulated,
+                   const float parallax_deg_thr, const float reproj_err_thr, const int device = 0);
+#endif
+};
+
+}  // namespace initialize
 }  // namespace openvslam

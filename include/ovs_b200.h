@@ -418,6 +418,79 @@ int ovs_two_view_triangulate_host(ovs_matcher* h, int B, const ovs_keyframe_view
                                   const int32_t* pair_offsets, const int32_t* pairs, double rays_parallax_deg_thr, uint8_t* valid,
                                   double* pos_w);
 
+/* ---- monocular map initialisation: initialize::perspective and initialize::bearing_vector (initialize/perspective.cc, bearing_vector.cc) ---- */
+
+/* What an initialiser reads of one frame: camera_ (perspective -- fisheye passed as perspective on its undistorted keypoints --
+ * for ovs_initialize_perspective_host, equirectangular for ovs_initialize_bearing_vector_host; fx, fy, cx, cy or cols, rows are
+ * read), undist_keypts[num_keypts] = undist_keypts_.data() (pt is read), bearings[num_keypts*3] = bearings_ (unit). */
+typedef struct {
+    ovs_camera camera;
+    int32_t num_keypts;
+    const ovs_keypoint* undist_keypts;
+    const double* bearings;
+} ovs_init_view;
+
+#define OVS_INIT_OK 0                  /* initialize() returned true */
+#define OVS_INIT_NO_VALID_MODEL 1      /* no valid solution to decompose (e.g. fewer than 8 matches) */
+#define OVS_INIT_DECOMPOSITION_REFUSED 2  /* the homography's singular values are too close (d1/d2 or d2/d3 < 1.00001) */
+#define OVS_INIT_TOO_FEW 3             /* the best hypothesis has fewer than min_num_triangulated valid points */
+#define OVS_INIT_AMBIGUOUS 4           /* more than one hypothesis has more than 0.8 x the best count */
+#define OVS_INIT_SMALL_PARALLAX 5      /* the best hypothesis's parallax is below parallax_deg_thr */
+
+#define OVS_INIT_MODEL_NONE 0
+#define OVS_INIT_MODEL_H 1
+#define OVS_INIT_MODEL_F 2
+#define OVS_INIT_MODEL_E 3
+
+/* The outcome of one initialisation problem. */
+typedef struct {
+    int32_t status;                    /* OVS_INIT_* */
+    int32_t model;                     /* OVS_INIT_MODEL_*: the decomposed solution */
+    int32_t chosen;                    /* the hypothesis with the most valid points (first on ties), -1 with none */
+    int32_t num_hypotheses;            /* 8 (H), 4 (F, E), 0 */
+    int32_t num_valid[8];              /* per hypothesis: check_pose's count of valid points */
+    float cos_parallax[8];             /* per hypothesis: the min(50, n - 1)-th smallest cos_parallax of its n valid points (1: n = 0) */
+    double rot_ref_to_cur[9];          /* get_rotation_ref_to_cur(), row-major (p_cur = R p_ref + t), when status is OVS_INIT_OK */
+    double trans_ref_to_cur[3];        /* get_translation_ref_to_cur() (unit norm), when status is OVS_INIT_OK */
+    double solver_M[2][9];             /* perspective: H_21, F_21; bearing_vector: E_21, zero */
+    double solver_score[2];            /* the solvers' best scores, in the same order */
+    int32_t solver_num_inliers[2];
+    uint8_t solver_valid[2];
+    uint8_t reserved[6];
+} ovs_init_result;
+
+/* initialize::perspective(ref_frm, num_ransac_iters, min_num_triangulated, parallax_deg_thr, reproj_err_thr).initialize(cur_frm,
+ * ref_matches_with_cur) for B independent problems in one call.  Problem b has the reference view ref_views[b] and the current
+ * view cur_views[b]; its ref_matches_with_cur (one entry per reference keypoint: the matched current keypoint, or -1) and its
+ * outputs is_triangulated / triangulated_pts[*3] (get_triangulated_flags() / get_triangulated_pts(), in the reference camera's
+ * frame; zero where not triangulated and for a failed problem) are concatenated over the problems in order, ref_views[b].num_keypts
+ * entries each.  seeds[B]: one sampler seed per problem, used by both the homography and the fundamental-matrix solver (a
+ * problem gives the same result alone or inside a batch).  The steps (both solvers on the matches in reference-index order with
+ * sigma = 1 and recompute, the model choice S_H / (S_H + S_F) > 0.40, the decompositions into 8 or 4 hypotheses, check_pose with
+ * reproj_err_thr_sq (the reference passes 4.0) and depth_is_positive, find_most_plausible_pose) and their conventions are in
+ * DESIGN.md section 5; solver_M / solver_score / solver_num_inliers / solver_valid equal ovs_homography_solve_ransac_host and
+ * ovs_fundamental_solve_ransac_host on the same matches and seeds.
+ * Checked before any launch -- OVS_ERR_INVALID_ARG: B outside 0 .. 65535, a negative num_ransac_iters or min_num_triangulated,
+ * a parallax_deg_thr outside 0 .. 180, a reproj_err_thr_sq that is negative or not finite, a camera of another model or with
+ * fx, fy not positive and finite, a keypoint that is not finite, a bearing that is not a finite unit vector, an entry of
+ * ref_matches_with_cur outside -1 .. cur_views[b].num_keypts - 1, a missing array; OVS_ERR_UNSUPPORTED: 2^28 or more keypoints of
+ * one side or matches in all, or B x num_ransac_iters above 2^31 - 1.  B == 0 or no match at all returns without a launch.
+ * Otherwise the call is 13 launches (7 with num_ransac_iters == 0): the homography solve's 4, the fundamental solve's 4 and the 5
+ * initialiser kernels, one copy each way and one wait, whatever B and whichever model each problem takes.  The call has its own
+ * buffers on the handle: the matcher and solver entry points are unaffected by it. */
+int ovs_initialize_perspective_host(ovs_matcher* h, int B, const ovs_init_view* ref_views, const ovs_init_view* cur_views,
+                                    const int32_t* ref_matches_with_cur, int num_ransac_iters, int min_num_triangulated,
+                                    float parallax_deg_thr, float reproj_err_thr_sq, const uint64_t* seeds, ovs_init_result* results,
+                                    uint8_t* is_triangulated, double* triangulated_pts);
+/* initialize::bearing_vector(...).initialize(cur_frm, ref_matches_with_cur): the same for equirectangular cameras, with the
+ * essential solver on the matches' bearings (recompute on), 4 hypotheses and no depth test.  solver_M[0] / solver_score[0] /
+ * solver_num_inliers[0] / solver_valid[0] equal ovs_essential_solve_ransac_host on the gathered bearings and the same seeds.
+ * 8 launches (6 with num_ransac_iters == 0): the essential solve's 3 and the 5 initialiser kernels, one copy each way, one wait. */
+int ovs_initialize_bearing_vector_host(ovs_matcher* h, int B, const ovs_init_view* ref_views, const ovs_init_view* cur_views,
+                                       const int32_t* ref_matches_with_cur, int num_ransac_iters, int min_num_triangulated,
+                                       float parallax_deg_thr, float reproj_err_thr_sq, const uint64_t* seeds, ovs_init_result* results,
+                                       uint8_t* is_triangulated, double* triangulated_pts);
+
 /* A landmark create_new_landmarks makes: keyfrms_2[neighbour], keypoint idx_1 of keyframe 1, idx_2 of the neighbour, pos_w. */
 typedef struct {
     int32_t neighbour, idx_1, idx_2, reserved;

@@ -1,5 +1,5 @@
-// match_common.h -- the matcher handle shared by match_bruteforce.cu, match_window.cu, two_view_ransac.cu and
-// two_view_triangulate.cu.  Its arenas
+// match_common.h -- the matcher handle shared by match_bruteforce.cu, match_window.cu, two_view_ransac.cu,
+// two_view_triangulate.cu and initializer.cu.  Its arenas
 // grow and are carved through staging.h.
 #pragma once
 #include <algorithm>
@@ -32,6 +32,9 @@ struct ovs_matcher {
     // the two-view triangulator's and create_new_landmarks' own arenas (two_view_triangulate.cu, match_window.cu)
     uint8_t* d_tri = nullptr; size_t d_tri_cap = 0;
     uint8_t* h_tri = nullptr; size_t h_tri_cap = 0;     // pinned
+    // map initialisation's own arenas (initializer.cu): its solves and kernels leave the solver entry points' buffers untouched
+    uint8_t* d_init = nullptr; size_t d_init_cap = 0;
+    uint8_t* h_init = nullptr; size_t h_init_cap = 0;   // pinned
     cudaEvent_t ev[2]{};
     float last_kernel_us = 0.f;
     int num_requeries = 0;   // GPU re-queries issued by the greedy replays so far (diagnostic)

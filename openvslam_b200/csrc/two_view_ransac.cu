@@ -28,6 +28,7 @@
 #include "match_common.h"
 #include "ransac.cuh"
 #include "two_view_math.cuh"
+#include "two_view_ransac.h"
 
 namespace {
 
@@ -219,32 +220,32 @@ __global__ void __launch_bounds__(kRefineThreads) k_two_view_refine(Args<Model> 
     }
 }
 
-// The host copies of a solve's outputs.
-struct Results {
-    double* M; double* score; int* num; int* best; uint8_t* valid; uint8_t* flags;
-};
+// Point a solve's arguments at its carved outputs and scratch.
+template <class Model>
+void bind(Args<Model>& A, const ovs::SolveOut& o, const ovs::SolveScratch& s) {
+    A.M = o.M; A.score = o.score; A.num_inliers = o.num; A.best_iter = o.best; A.valid = o.valid; A.inlier = o.inlier;
+    A.hyp = s.hyp; A.hscore = s.hyp_score; A.hcount = s.hyp_count; A.cidx = s.cidx;
+    if constexpr (!std::is_same<Model, EssentialModel>::value) { A.model.np_1 = s.np_1; A.model.np_2 = s.np_2; A.model.norm = s.norm; }
+}
 
 // A solve's outputs and scratch, carved after its inputs.
 template <class Model>
-void carve_results(ovs::Staging& S, Args<Model>& A, Results& r, size_t N) {
-    const size_t NB = (size_t)A.B, H = (size_t)A.H;
-    A.M = S.out(r.M, 9 * NB); A.score = S.out(r.score, NB); A.num_inliers = S.out(r.num, NB); A.best_iter = S.out(r.best, NB);
-    A.valid = S.out(r.valid, NB); A.inlier = S.out(r.flags, N);
-    A.hyp = S.dev<double>(9 * NB * H); A.hscore = S.dev<double>(NB * H); A.hcount = S.dev<int>(NB * H); A.cidx = S.dev<int>(N);
+void carve_results(ovs::Staging& S, Args<Model>& A, ovs::SolveOut& o, size_t N, size_t K1, size_t K2) {
+    ovs::SolveScratch s;
+    ovs::carve_solve_out(S, o, (size_t)A.B, N);
+    ovs::carve_solve_scratch(S, s, (size_t)A.B, (size_t)A.H, N, K1, K2);
+    bind(A, o, s);
 }
 
-// The launches of a staged solve, the copy back and the host outputs (M_21 ... per problem, inlier_out per match).
+// The launches of a staged solve.
 template <class Model>
-int launch_and_fetch(cudaStream_t st, const ovs::Staging& S, const Args<Model>& A, const Results& r, size_t N, double* M_21,
-                     uint8_t* valid, int32_t* num_inliers, int32_t* best_iter, double* best_score, uint8_t* inlier_out) {
-    const size_t NB = (size_t)A.B;
-    OVS_CUDA_CHECK(S.upload(st));
+int enqueue(cudaStream_t st, const Args<Model>& A) {
     if (A.H > 0) {
         if constexpr (!std::is_same<Model, EssentialModel>::value) {
             k_two_view_normalize<<<(2 * A.B + kNormThreads - 1) / kNormThreads, kNormThreads, 0, st>>>(A.B, A.off, A.model);
             OVS_LAUNCH_CHECK();
         }
-        const size_t hyp_threads = NB * (size_t)A.H;
+        const size_t hyp_threads = (size_t)A.B * (size_t)A.H;
         k_two_view_hypotheses<Model><<<(unsigned)((hyp_threads + kHypThreads - 1) / kHypThreads), kHypThreads, 0, st>>>(A);
         OVS_LAUNCH_CHECK();
         k_two_view_score<Model><<<dim3((A.H + kScoreWarps - 1) / kScoreWarps, A.B), kScoreThreads, 0, st>>>(A);
@@ -252,11 +253,22 @@ int launch_and_fetch(cudaStream_t st, const ovs::Staging& S, const Args<Model>& 
     }
     k_two_view_refine<Model><<<A.B, kRefineThreads, 0, st>>>(A);
     OVS_LAUNCH_CHECK();
+    return OVS_OK;
+}
+
+// A staged solve: the upload, the launches, the copy back and the host outputs (M_21 ... per problem, inlier_out per match).
+template <class Model>
+int launch_and_fetch(cudaStream_t st, const ovs::Staging& S, const Args<Model>& A, const ovs::SolveOut& o, size_t N, double* M_21,
+                     uint8_t* valid, int32_t* num_inliers, int32_t* best_iter, double* best_score, uint8_t* inlier_out) {
+    const size_t NB = (size_t)A.B;
+    OVS_CUDA_CHECK(S.upload(st));
+    int rc = enqueue(st, A);
+    if (rc != OVS_OK) return rc;
     OVS_CUDA_CHECK(S.download(st));
     OVS_CUDA_CHECK(ovs::sync_stream(st));
-    memcpy(M_21, r.M, 9 * 8 * NB); memcpy(best_score, r.score, 8 * NB);
-    memcpy(num_inliers, r.num, 4 * NB); memcpy(best_iter, r.best, 4 * NB); memcpy(valid, r.valid, NB);
-    if (N) memcpy(inlier_out, r.flags, N);
+    memcpy(M_21, o.hM, 9 * 8 * NB); memcpy(best_score, o.hscore, 8 * NB);
+    memcpy(num_inliers, o.hnum, 4 * NB); memcpy(best_iter, o.hbest, 4 * NB); memcpy(valid, o.hvalid, NB);
+    if (N) memcpy(inlier_out, o.hinlier, N);
     return OVS_OK;
 }
 
@@ -277,7 +289,7 @@ int essential_run(ovs_matcher* h, int B, const int32_t* off, const int32_t* pair
     Args<EssentialModel> A{};
     A.B = B; A.H = max_num_iter; A.recompute = recompute ? 1 : 0;
     int* hoff; uint64_t* hseed; int* hpairs = nullptr; double* hb1 = nullptr; double* hb2 = nullptr;
-    Results r;
+    ovs::SolveOut r;
     ovs::Staging S;
     OVS_CUDA_CHECK(cudaSetDevice(h->device));
     int rc = ovs::stage(S, h->h_ess, h->h_ess_cap, h->d_ess, h->d_ess_cap, [&](ovs::Staging& S) {
@@ -285,7 +297,7 @@ int essential_run(ovs_matcher* h, int B, const int32_t* off, const int32_t* pair
         A.model.pairs = pairs ? S.in(hpairs, np) : nullptr;
         if (bear.on_device) { A.model.bear_1 = bear.b1; A.model.bear_2 = bear.b2; }
         else { A.model.bear_1 = S.in(hb1, 3 * bear.n1); A.model.bear_2 = S.in(hb2, 3 * bear.n2); }
-        carve_results(S, A, r, N);
+        carve_results(S, A, r, N, 0, 0);
     });
     if (rc != OVS_OK) return rc;
     memcpy(hoff, off, 4 * (NB + 1)); memcpy(hseed, seeds, 8 * NB);
@@ -309,7 +321,7 @@ int two_view_run(ovs_matcher* h, int B, const int32_t* koff_1, const ovs_keypoin
     A.B = B; A.H = max_num_iter; A.recompute = recompute ? 1 : 0;
     A.model.inv_sigma_sq = (double)ovs::two_view_inv_sigma_sq(sigma);
     int *hmoff, *hk1, *hk2, *hpairs; uint64_t* hseed; float *hkp1, *hkp2;
-    Results r;
+    ovs::SolveOut r;
     ovs::Staging S;
     OVS_CUDA_CHECK(cudaSetDevice(h->device));
     int rc = ovs::stage(S, h->h_tv, h->h_tv_cap, h->d_tv, h->d_tv_cap, [&](ovs::Staging& S) {
@@ -317,8 +329,7 @@ int two_view_run(ovs_matcher* h, int B, const int32_t* koff_1, const ovs_keypoin
         A.off = S.in(hmoff, NB + 1); m.koff_1 = S.in(hk1, NB + 1); m.koff_2 = S.in(hk2, NB + 1);
         A.seed = S.in(hseed, NB); m.pairs = S.in(hpairs, 2 * N);
         m.kp_1 = S.in(hkp1, 2 * K1); m.kp_2 = S.in(hkp2, 2 * K2);
-        carve_results(S, A, r, N);
-        m.np_1 = S.dev<float>(2 * K1); m.np_2 = S.dev<float>(2 * K2); m.norm = S.dev<ovs::TwoViewNorm>(2 * NB);
+        carve_results(S, A, r, N, K1, K2);
     });
     if (rc != OVS_OK) return rc;
     memcpy(hmoff, moff, 4 * (NB + 1)); memcpy(hk1, koff_1, 4 * (NB + 1)); memcpy(hk2, koff_2, 4 * (NB + 1));
@@ -334,16 +345,6 @@ void no_match_results(int B, double* M_21, uint8_t* valid, int32_t* num_inliers,
         for (int k = 0; k < 9; ++k) M_21[9 * (size_t)b + k] = 0.0;
         valid[b] = 0; num_inliers[b] = 0; best_iter[b] = -1; best_score[b] = 0.0;
     }
-}
-
-int check_bearings(const double* b, int n, const char* what) {
-    for (int i = 0; i < n; ++i) {
-        const double* v = b + 3 * (size_t)i;
-        OVS_REQUIRE(std::isfinite(v[0]) && std::isfinite(v[1]) && std::isfinite(v[2]) &&
-                    std::fabs(v[0] * v[0] + v[1] * v[1] + v[2] * v[2] - 1.0) <= 1e-6,
-                    OVS_ERR_INVALID_ARG, "%s %d is not a finite unit vector", what, i);
-    }
-    return OVS_OK;
 }
 
 // robust::match_frame_and_keyframe after its brute force: the solver on the pairs (find_via_ransac(max_num_iter, false)), then
@@ -408,6 +409,60 @@ int two_view_solve_host(ovs_matcher* h, int B, const int32_t* keypt_offsets_1, c
 
 }  // namespace
 
+namespace ovs {
+
+void carve_solve_out(Staging& S, SolveOut& o, size_t NB, size_t N) {
+    o.M = S.out(o.hM, 9 * NB); o.score = S.out(o.hscore, NB); o.num = S.out(o.hnum, NB); o.best = S.out(o.hbest, NB);
+    o.valid = S.out(o.hvalid, NB); o.inlier = S.out(o.hinlier, N);
+}
+
+void carve_solve_scratch(Staging& S, SolveScratch& s, size_t NB, size_t H, size_t N, size_t K1, size_t K2) {
+    s.hyp = S.dev<double>(9 * NB * H); s.hyp_score = S.dev<double>(NB * H); s.hyp_count = S.dev<int>(NB * H); s.cidx = S.dev<int>(N);
+    s.np_1 = s.np_2 = nullptr; s.norm = nullptr;
+    if (K1 + K2) { s.np_1 = S.dev<float>(2 * K1); s.np_2 = S.dev<float>(2 * K2); s.norm = S.dev<TwoViewNorm>(2 * NB); }
+}
+
+namespace {
+template <int Model>
+int enqueue_keypoint_solve(cudaStream_t st, const SolveInputs& in, const SolveOut& o, const SolveScratch& s, float sigma) {
+    Args<TwoViewModel<Model>> A{};
+    A.B = in.B; A.H = in.H; A.recompute = in.recompute; A.off = in.off; A.seed = in.seed;
+    TwoViewModel<Model>& m = A.model;
+    m.koff_1 = in.koff_1; m.koff_2 = in.koff_2; m.kp_1 = in.kp_1; m.kp_2 = in.kp_2; m.pairs = in.pairs;
+    m.inv_sigma_sq = (double)two_view_inv_sigma_sq(sigma);
+    bind(A, o, s);
+    return enqueue(st, A);
+}
+}  // namespace
+
+int enqueue_homography_solve(cudaStream_t st, const SolveInputs& in, const SolveOut& o, const SolveScratch& s, float sigma) {
+    return enqueue_keypoint_solve<kTwoViewH>(st, in, o, s, sigma);
+}
+
+int enqueue_fundamental_solve(cudaStream_t st, const SolveInputs& in, const SolveOut& o, const SolveScratch& s, float sigma) {
+    return enqueue_keypoint_solve<kTwoViewF>(st, in, o, s, sigma);
+}
+
+int enqueue_essential_solve(cudaStream_t st, const SolveInputs& in, const SolveOut& o, const SolveScratch& s) {
+    Args<EssentialModel> A{};
+    A.B = in.B; A.H = in.H; A.recompute = in.recompute; A.off = in.off; A.seed = in.seed;
+    A.model.bear_1 = in.bear_1; A.model.bear_2 = in.bear_2; A.model.pairs = nullptr;
+    bind(A, o, s);
+    return enqueue(st, A);
+}
+
+int check_bearings(const double* b, int n, const char* what) {
+    for (int i = 0; i < n; ++i) {
+        const double* v = b + 3 * (size_t)i;
+        OVS_REQUIRE(std::isfinite(v[0]) && std::isfinite(v[1]) && std::isfinite(v[2]) &&
+                    std::fabs(v[0] * v[0] + v[1] * v[1] + v[2] * v[2] - 1.0) <= 1e-6,
+                    OVS_ERR_INVALID_ARG, "%s %d is not a finite unit vector", what, i);
+    }
+    return OVS_OK;
+}
+
+}  // namespace ovs
+
 extern "C" int ovs_essential_solve_ransac_host(ovs_matcher* h, int B, const int32_t* match_offsets, const double* bearings_1,
                                                const double* bearings_2, int max_num_iter, int recompute, const uint64_t* seeds,
                                                double* E_21, uint8_t* valid, int32_t* num_inliers, int32_t* best_iter, double* best_score,
@@ -420,8 +475,8 @@ extern "C" int ovs_essential_solve_ransac_host(ovs_matcher* h, int B, const int3
     if ((rc = ovs::check_offsets(match_offsets, B, "match_offsets")) != OVS_OK) return rc;
     const int n_all = match_offsets[B];
     OVS_REQUIRE(n_all == 0 || (bearings_1 && bearings_2 && inlier_out), OVS_ERR_INVALID_ARG, "null argument");
-    if ((rc = check_bearings(bearings_1, n_all, "bearings_1 of match")) != OVS_OK) return rc;
-    if ((rc = check_bearings(bearings_2, n_all, "bearings_2 of match")) != OVS_OK) return rc;
+    if ((rc = ovs::check_bearings(bearings_1, n_all, "bearings_1 of match")) != OVS_OK) return rc;
+    if ((rc = ovs::check_bearings(bearings_2, n_all, "bearings_2 of match")) != OVS_OK) return rc;
     if (n_all == 0) {
         no_match_results(B, E_21, valid, num_inliers, best_iter, best_score);
         return OVS_OK;
@@ -443,8 +498,8 @@ extern "C" int ovs_robust_match_frame_and_keyframe_host(ovs_matcher* h, const ui
     if (n1 == 0 || n2 == 0) return OVS_OK;
     OVS_REQUIRE(bearings_frm && bearings_keyfrm, OVS_ERR_INVALID_ARG, "null argument");
     int rc;
-    if ((rc = check_bearings(bearings_frm, n1, "bearing of frame keypoint")) != OVS_OK) return rc;
-    if ((rc = check_bearings(bearings_keyfrm, n2, "bearing of keyframe keypoint")) != OVS_OK) return rc;
+    if ((rc = ovs::check_bearings(bearings_frm, n1, "bearing of frame keypoint")) != OVS_OK) return rc;
+    if ((rc = ovs::check_bearings(bearings_keyfrm, n2, "bearing of keyframe keypoint")) != OVS_OK) return rc;
     std::vector<int32_t> pairs(2 * (size_t)std::min(n1, n2));
     int np = 0;
     if ((rc = ovs_robust_brute_force_match_host(h, desc_frm, n1, desc_keyfrm, n2, lm_valid_2, lowe_ratio, pairs.data(),
