@@ -11,6 +11,9 @@ normal equations over poses and points -- no Schur complement, no Cholesky of ou
 residuals and Jacobians of `oracle.edge_eval` (pinned against finite differences) and the Huber weights rho'(chi2) at the
 linearisation point.  It shares no linear algebra with the oracle's Schur / Cholesky path or with the kernels.
 """
+import functools
+from types import SimpleNamespace
+
 import numpy as np
 import scipy.sparse as sp
 import scipy.sparse.linalg as spla
@@ -239,8 +242,10 @@ def _robust_chi2(g, poses, points, xr, active, delta):
     return float(np.where(c <= d2, c, 2 * np.sqrt(c) * delta - d2).sum())
 
 
-def _linearise(oracle, g, poses, points, xr, active, delta, with_points):
-    """H (full, sparse, poses then points) and b = -J^T W e at the current state"""
+def full_system(oracle, g, poses, points, xr, active, delta, with_points):
+    """The full normal equations at the current state, linearised edge by edge through `oracle.edge_eval`: H (sparse,
+    poses then points) and b = -J^T W e.  Returns the linear system as `reference_lm` takes it: diag (of H), b, free_idx and
+    solve(lam) = (H + lam I)^-1 b by scipy's sparse LU."""
     cam = oracle.camera(**g["cam"])
     free_idx = np.cumsum(g["fixed"] == 0) - 1
     free_idx[g["fixed"] != 0] = -1
@@ -270,13 +275,21 @@ def _linearise(oracle, g, poses, points, xr, active, delta, with_points):
                 rows.append(r.ravel()); cols.append(c.ravel()); vals.append(blk.ravel())
     H = sp.coo_matrix((np.concatenate(vals) if vals else np.zeros(0), (np.concatenate(rows) if rows else np.zeros(0, int),
                       np.concatenate(cols) if cols else np.zeros(0, int))), shape=(N, N)).tocsc()
-    return H, b, free_idx
+    return SimpleNamespace(diag=H.diagonal(), b=b, free_idx=free_idx,
+                           solve=lambda lam: spla.spsolve((H + lam * sp.identity(N, format="csc")).tocsc(), b))
 
 
-def reference_lm(oracle, g, iterations, use_huber=True, with_points=True, level=None, poses=None, points=None):
+def reference_lm(oracle, g, iterations, use_huber=True, with_points=True, level=None, poses=None, points=None, system=None, oplus=None):
     """g2o's OptimizationAlgorithmLevenberg on the full normal equations.  Returns (poses, points, dict(lambda_init,
     trials = trials per iteration, states = [(poses, points)] after each iteration)).  `level` marks excluded edges;
-    with_points=False keeps the points constant (motion-only problem)."""
+    with_points=False keeps the points constant (motion-only problem).  `system(g, poses, points, xr, active, delta,
+    with_points)` linearises (default: `full_system` through the oracle's edges) and `oplus(poses (k, 12), dx (k, 6))`
+    updates the free poses (default: `oracle.pose_oplus`): the driver is shared with the vectorised reference of
+    tests/ba_reference64.py."""
+    if system is None:
+        system = functools.partial(full_system, oracle)
+    if oplus is None:
+        oplus = lambda ps, us: np.array([oracle.pose_oplus(p, u) for p, u in zip(ps, us)]).reshape(-1, 12)
     poses = np.array(g["poses"] if poses is None else poses, np.float64).copy()
     points = np.array(g["points"] if points is None else points, np.float64).copy()
     xr = None if g["setup_is_mono"] else g["obs_xr"]
@@ -286,21 +299,20 @@ def reference_lm(oracle, g, iterations, use_huber=True, with_points=True, level=
     trials, states = [], []
     cur = _robust_chi2(g, poses, points, xr, active, delta)
     for it in range(iterations):
-        H, b, free_idx = _linearise(oracle, g, poses, points, xr, active, delta, with_points)
-        N = H.shape[0]
-        n = 6 * int((free_idx >= 0).sum())
+        lin = system(g, poses, points, xr, active, delta, with_points)
+        free = np.flatnonzero(lin.free_idx >= 0)
+        n = 6 * len(free)
         if it == 0:
-            lam = 1e-5 * float(np.abs(H.diagonal()).max())
+            lam = 1e-5 * float(np.abs(lin.diag).max())
             lam0, ni = lam, 2.0
         q = 0
         while True:
-            dx = spla.spsolve((H + lam * sp.identity(N, format="csc")).tocsc(), b)
+            dx = lin.solve(lam)
             cp = poses.copy()
-            for k in np.flatnonzero(free_idx >= 0):
-                cp[k] = oracle.pose_oplus(poses[k], dx[6 * free_idx[k]:6 * free_idx[k] + 6])
+            cp[free] = oplus(poses[free], dx[:n].reshape(-1, 6)[lin.free_idx[free]])
             cq = points + dx[n:].reshape(-1, 3) if with_points else points
             new = _robust_chi2(g, cp, cq, xr, active, delta)
-            rho = (cur - new) / (float(dx @ (lam * dx + b)) + 1e-3)
+            rho = (cur - new) / (float(dx @ (lam * dx + lin.b)) + 1e-3)
             q += 1
             if rho > 0 and np.isfinite(new):
                 lam *= max(1.0 / 3.0, min(1.0 - (2 * rho - 1) ** 3, 2.0 / 3.0))

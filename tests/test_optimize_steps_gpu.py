@@ -71,8 +71,12 @@ def _reference(name):
 
 def run_ba(oracle, name, kind, it):
     """one optimiser call of `it` iterations on the GPU and in the oracle -> results and step-error ratios"""
+    return run_ba_graph(oracle, _graph(name), _reference(name), kind, it)
+
+
+def run_ba_graph(oracle, g, ref, kind, it):
+    """run_ba on graph g, with the reference's Levenberg record `ref` (or None)"""
     from openvslam_b200 import optimize
-    g = _graph(name)
     mono = g["setup_is_mono"]
     if kind == "local":
         ba = optimize.local_bundle_adjuster(it, 0)
@@ -86,7 +90,6 @@ def run_ba(oracle, name, kind, it):
     ba.close()
     r = dict(g=g, st=st, ost=ost, outl=outl, ooutl=ooutl, poses=poses,
              pose_vs_oracle=bg.step_error(poses, oposes, g["poses"]), point_vs_oracle=bg.step_error(points, opoints, g["points"]))
-    ref = _reference(name)
     if ref is not None:
         rp, rq = ref["states"][it - 1]
         assert sum(ref["trials"][:it]) == ost["num_trials"]
@@ -125,16 +128,22 @@ def test_global_ba_steps(oracle, name, it):
 
 
 def run_pose(oracle, n, stereo, bad=0, num_trials=1):
+    return run_pose_graph(oracle, bg.pose_graph(n, stereo=stereo, bad=bad, seed=n), num_trials)
+
+
+def run_pose_graph(oracle, g, num_trials=1, ref=None):
+    """pose_optimizer(num_trials, 1) on the GPU and in the oracle on the motion-only graph g (edge i sees g["points"][i]), and
+    one reference iteration (`ref`: its Levenberg record, computed here when None)"""
     from openvslam_b200 import optimize
-    g = bg.pose_graph(n, stereo=stereo, bad=bad, seed=n)
     xr = None if g["setup_is_mono"] else g["obs_xr"]
     args = (g["setup_is_mono"], g["points"], g["obs_xy"], xr, g["inv_sigma_sq"], g["poses"][0])
     po = optimize.pose_optimizer(num_trials, 1)
     ninl, pose, flags, st = po.optimize(optimize.camera(**g["cam"]), *args)
     po.close()
     on, opose, oflags, ost = oracle.pose_optimize(oracle.camera(**g["cam"]), *args, num_trials=num_trials, num_each_iter=1)
-    rp, _, info = bg.reference_lm(oracle, g, 1, with_points=False)
-    return dict(ninl=ninl, on=on, flags=flags, oflags=oflags, st=st, ost=ost, ref_trials=info["trials"],
+    info = bg.reference_lm(oracle, g, 1, with_points=False)[2] if ref is None else ref
+    rp = info["states"][0][0]
+    return dict(ninl=ninl, on=on, flags=flags, oflags=oflags, st=st, ost=ost, ref_trials=info["trials"], ref_lambda_init=info["lambda_init"],
                 pose_vs_oracle=bg.step_error(pose, opose, g["poses"][0]), pose_vs_ref=bg.step_error(pose, rp[0], g["poses"][0]))
 
 
