@@ -23,6 +23,9 @@
 //   initialize::perspective / initialize::bearing_vector(const data::frame&, unsigned, unsigned, float, float),
 //     initialize(const data::frame&, const std::vector<int>&), get_{rotation,translation}_ref_to_cur(),
 //     get_triangulated_{pts,flags}()                                                           (initialize/{perspective,bearing_vector}.h)
+//   match::projection::match_current_and_last_frames(data::frame&, const data::frame&, float)                   (match/projection.h)
+//   the body of tracking_module::search_local_landmarks over data::frame and data::landmark, as adapters::search_local_landmarks
+//     (both templates deduced from their arguments; tests/cpp/test_tracking_search.cpp runs them on the GPU)
 //
 // Include it INSTEAD of openvslam_b200.hpp in a translation unit that can see the reference's headers (here: the stand-ins
 // under tests/cpp/standin, which declare the members used below with the names recalled in SURVEY.md section 2 / 8b;
@@ -208,6 +211,141 @@ inline unsigned int match::projection::match_frame_and_landmarks(data::frame& fr
     const unsigned int num = match_frame_and_landmarks(idx, frm.scale_factors_, static_cast<int>(L), usable.data(), reproj.data(), xr.data(), lvl.data(),
                                                        desc.data(), has.data(), matched, margin);
     for (unsigned int i = 0; i < n; ++i) if (matched[i] >= 0) frm.landmarks_.at(i) = local_landmarks[static_cast<std::size_t>(matched[i])];
+    return num;
+}
+
+namespace adapters {
+
+// The tracking adapters below are templates deduced from their arguments (data::frame / data::landmark in the reference tree), as
+// match::robust::match_frame_and_keyframe is: their bodies are compiled only where they are called, so a data model without the
+// members they read (here: the landmark's unscaled valid distances, INTEGRATION.md) can use the other adapters.
+
+//! What frame::can_observe and the motion model read of a frame: camera_ (fisheye and radial division reproject with the pinhole
+//! formula on undistorted keypoints), camera_->img_bounds_, cam_pose_cw_, get_cam_center(), num_scale_levels_, log_scale_factor_.
+template <class Frame>
+ovs_frame_geometry frame_geometry(const Frame& frm) {
+    ovs_frame_geometry g{};
+    g.camera = to_camera(frm.camera_);
+    const camera::image_bounds& b = frm.camera_->img_bounds_;
+    g.min_x = b.min_x_; g.max_x = b.max_x_; g.min_y = b.min_y_; g.max_y = b.max_y_;
+    double pose12[12];
+    to_Rt(frm.cam_pose_cw_, pose12);
+    for (int k = 0; k < 9; ++k) g.rot_cw[k] = pose12[k];
+    for (int k = 0; k < 3; ++k) g.trans_cw[k] = pose12[9 + k];
+    const Vec3_t c = frm.get_cam_center();
+    for (int k = 0; k < 3; ++k) g.cam_center[k] = c(k);
+    g.num_scale_levels = static_cast<std::int32_t>(frm.num_scale_levels_);
+    g.log_scale_factor = frm.log_scale_factor_;
+    return g;
+}
+
+//! kp_has_observed_lm of a frame: frm.landmarks_[i] present and has_observation()
+template <class Frame>
+std::vector<std::uint8_t> keypoints_with_observed_landmarks(const Frame& frm) {
+    const unsigned int n = frm.num_keypts_;
+    std::vector<std::uint8_t> has(std::max<unsigned int>(n, 1), 0);
+    for (unsigned int i = 0; i < n; ++i) has[i] = frm.landmarks_.at(i) && frm.landmarks_.at(i)->has_observation();
+    return has;
+}
+
+//! The body of tracking_module::search_local_landmarks (module/tracking_module.cc) with frame::can_observe on the device: the
+//! frame's own landmarks are marked (is_observable_in_tracking_ = false, identifier_in_local_lm_search_ = curr_frm.id_,
+//! increase_num_observable()); every other local landmark that is not will_be_erased() goes through can_observe(lm, 0.5) and,
+//! when observable, gets reproj_in_tracking_, x_right_in_tracking_, scale_level_in_tracking_, is_observable_in_tracking_ = true and
+//! increase_num_observable(), else is_observable_in_tracking_ = false; the observable ones are matched into curr_frm.landmarks_
+//! by the matcher's match_frame_and_landmarks(curr_frm, local_landmarks, margin).  Returns found_proj_candidate.  The caller picks
+//! the margin as the reference does (20 right after a relocalisation, 10 RGBD, 5 otherwise).
+template <class Frame, class Landmark>
+bool search_local_landmarks(const match::projection& matcher, Frame& curr_frm, const std::vector<Landmark*>& local_landmarks, const float margin) {
+    for (Landmark* lm : curr_frm.landmarks_) {
+        if (!lm || lm->will_be_erased()) continue;
+        lm->is_observable_in_tracking_ = false;
+        lm->identifier_in_local_lm_search_ = curr_frm.id_;
+        lm->increase_num_observable();
+    }
+    const std::size_t L = local_landmarks.size(), L1 = std::max<std::size_t>(L, 1);
+    std::vector<std::uint8_t> usable(L1, 0), desc(32 * L1), observable(L1, 0);
+    std::vector<double> pos(3 * L1, 0.0), nrm(3 * L1, 0.0);
+    std::vector<float> lo(L1, 0.0f), hi(L1, 0.0f), reproj(2 * L1), xr(L1);
+    std::vector<std::int32_t> lvl(L1);
+    for (std::size_t l = 0; l < L; ++l) {
+        const Landmark* lm = local_landmarks[l];
+        usable[l] = lm && lm->identifier_in_local_lm_search_ != curr_frm.id_ && !lm->will_be_erased();
+        if (!usable[l]) continue;
+        const Vec3_t p = lm->get_pos_in_world(), n = lm->get_obs_mean_normal();
+        for (int k = 0; k < 3; ++k) { pos[3 * l + k] = p(k); nrm[3 * l + k] = n(k); }
+        const std::pair<float, float> d = lm->get_unscaled_valid_distances();
+        lo[l] = d.first; hi[l] = d.second;
+        const cv::Mat dsc = lm->get_descriptor();
+        std::memcpy(&desc[32 * l], dsc.data, 32);
+    }
+    const frame_arrays arrays(curr_frm);
+    const match::frame_index idx(matcher, arrays.view);
+    const std::vector<std::uint8_t> has = keypoints_with_observed_landmarks(curr_frm);
+    std::vector<std::int32_t> matched;
+    matcher.search_local_landmarks(idx, frame_geometry(curr_frm), curr_frm.scale_factors_, static_cast<int>(L), usable.data(), pos.data(), nrm.data(),
+                                   lo.data(), hi.data(), desc.data(), has.data(), observable.data(), reproj.data(), xr.data(), lvl.data(), matched,
+                                   margin, 0.5f);
+    bool found_proj_candidate = false;
+    for (std::size_t l = 0; l < L; ++l) {
+        if (!usable[l]) continue;
+        Landmark* lm = local_landmarks[l];
+        lm->is_observable_in_tracking_ = observable[l] != 0;
+        if (!observable[l]) continue;
+        lm->reproj_in_tracking_(0) = reproj[2 * l]; lm->reproj_in_tracking_(1) = reproj[2 * l + 1];
+        lm->x_right_in_tracking_ = xr[l];
+        lm->scale_level_in_tracking_ = lvl[l];
+        lm->increase_num_observable();
+        found_proj_candidate = true;
+    }
+    for (unsigned int i = 0; i < curr_frm.num_keypts_; ++i)
+        if (matched[i] >= 0) curr_frm.landmarks_.at(i) = local_landmarks[static_cast<std::size_t>(matched[i])];
+    return found_proj_candidate;
+}
+
+//! The same with the reference's own matcher, match::projection projection_matcher(0.8), made for the call.
+template <class Frame, class Landmark>
+bool search_local_landmarks(Frame& curr_frm, const std::vector<Landmark*>& local_landmarks, const float margin) {
+    const match::projection projection_matcher(0.8);
+    return search_local_landmarks(projection_matcher, curr_frm, local_landmarks, margin);
+}
+
+}  // namespace adapters
+
+// match_current_and_last_frames: every keypoint of last_frm with a landmark that is not an outlier is reprojected into curr_frm with
+// its pose on the device; the direction comes from the two poses and curr_frm.camera_: setup_type_, and true_baseline =
+// focal_x_baseline_ / fx_, the value the reference's perspective-family camera constructors store (as create_new_landmarks reads it).
+template <class Frame>
+inline unsigned int match::projection::match_current_and_last_frames(Frame& curr_frm, const Frame& last_frm, const float margin) const {
+    const unsigned int n_last = last_frm.num_keypts_, N1 = std::max<unsigned int>(n_last, 1);
+    std::vector<std::uint8_t> usable(N1, 0), desc(32 * static_cast<std::size_t>(N1));
+    std::vector<double> pos(3 * static_cast<std::size_t>(N1), 0.0);
+    std::vector<std::int32_t> octave(N1, 0);
+    std::vector<float> angle(N1, 0.0f);
+    for (unsigned int i = 0; i < n_last; ++i) {
+        const auto* lm = last_frm.landmarks_.at(i);
+        usable[i] = lm && !last_frm.outlier_flags_.at(i);
+        octave[i] = last_frm.undist_keypts_.at(i).octave;
+        angle[i] = last_frm.undist_keypts_.at(i).angle;
+        if (!usable[i]) continue;
+        const Vec3_t p = lm->get_pos_in_world();
+        for (int k = 0; k < 3; ++k) pos[3 * i + k] = p(k);
+        const cv::Mat d = lm->get_descriptor();
+        std::memcpy(&desc[32 * static_cast<std::size_t>(i)], d.data, 32);
+    }
+    const adapters::frame_arrays arrays(curr_frm);
+    const frame_index idx(*this, arrays.view);
+    const std::vector<std::uint8_t> has = adapters::keypoints_with_observed_landmarks(curr_frm);
+    double last_pose[12];
+    adapters::to_Rt(last_frm.cam_pose_cw_, last_pose);
+    const ovs_frame_geometry geometry = adapters::frame_geometry(curr_frm);
+    const double true_baseline = geometry.camera.fx != 0.0 ? geometry.camera.focal_x_baseline / geometry.camera.fx : 0.0;
+    std::vector<std::int32_t> matched;
+    const unsigned int num = match_current_and_last_frames_reproject(
+        idx, geometry, curr_frm.camera_->setup_type_ == camera::setup_type_t::Monocular, true_baseline, last_pose, curr_frm.scale_factors_,
+        static_cast<int>(n_last), usable.data(), pos.data(), octave.data(), angle.data(), desc.data(), has.data(), matched, margin);
+    for (unsigned int i = 0; i < curr_frm.num_keypts_; ++i)
+        if (matched[i] >= 0) curr_frm.landmarks_.at(i) = last_frm.landmarks_.at(static_cast<std::size_t>(matched[i]));
     return num;
 }
 

@@ -331,6 +331,65 @@ public:
         matched_last_of_kp.resize(curr.num_keypts());
         return static_cast<unsigned int>(n);
     }
+#ifdef OVS_B200_WITH_REFERENCE_TYPES
+    //! The reference's signature (match/projection.h); body in adapters.hpp.  The last frame's landmarks are reprojected on the device.
+    //! A template deduced from the arguments (data::frame in the reference tree), compiled only where it is called.
+    template <class Frame>
+    unsigned int match_current_and_last_frames(Frame& curr_frm, const Frame& last_frm, const float margin) const;
+#endif
+    //! frame::can_observe(lm, ray_cos_thr, reproj, x_right, pred_scale_level) for num_landmarks landmarks in one launch
+    //! (ovs_frame_can_observe_host): usable = the tracker's skip rule (nullptr: all), pos_w / mean_normal 3 doubles per landmark,
+    //! the raw min_valid_dist_ / max_valid_dist_; outputs one entry per landmark (reproj: 2 floats).  Returns how many are observable.
+    unsigned int can_observe(const ovs_frame_geometry& geometry, const int num_landmarks, const std::uint8_t* usable, const double* pos_w,
+                             const double* mean_normal, const float* min_valid_dist, const float* max_valid_dist, const float ray_cos_thr,
+                             std::uint8_t* observable, float* reproj, float* x_right, std::int32_t* pred_scale_level) const {
+        detail::check(ovs_frame_can_observe_host(h_, &geometry, num_landmarks, usable, pos_w, mean_normal, min_valid_dist, max_valid_dist,
+                                                 ray_cos_thr, observable, reproj, x_right, pred_scale_level));
+        unsigned int num = 0;
+        for (int l = 0; l < num_landmarks; ++l) num += observable[l] ? 1u : 0u;
+        return num;
+    }
+    //! The compute of tracking_module::search_local_landmarks (ovs_projection_search_local_landmarks_host): can_observe on the device,
+    //! then match_frame_and_landmarks on its outputs.  The matcher is frm's (built on this or another projection handle).
+    unsigned int search_local_landmarks(const frame_index& frm, const ovs_frame_geometry& geometry, const std::vector<float>& scale_factors,
+                                        const int num_landmarks, const std::uint8_t* usable, const double* pos_w, const double* mean_normal,
+                                        const float* min_valid_dist, const float* max_valid_dist, const std::uint8_t* lm_descriptors,
+                                        const std::uint8_t* kp_has_observed_lm, std::uint8_t* observable, float* reproj, float* x_right,
+                                        std::int32_t* pred_scale_level, std::vector<std::int32_t>& matched_lm_of_kp, const float margin = 5.0,
+                                        const float ray_cos_thr = 0.5) const {
+        if (static_cast<int>(scale_factors.size()) != geometry.num_scale_levels)
+            throw std::invalid_argument("search_local_landmarks: one scale factor per level of the frame geometry");
+        matched_lm_of_kp.assign(std::max(1, frm.num_keypts()), -1);
+        int n = 0;
+        detail::check(ovs_projection_search_local_landmarks_host(frm.handle(), &geometry, scale_factors.data(), num_landmarks, usable, pos_w,
+                                                                 mean_normal, min_valid_dist, max_valid_dist, lm_descriptors, kp_has_observed_lm,
+                                                                 ray_cos_thr, margin, lowe_ratio_, observable, reproj, x_right, pred_scale_level,
+                                                                 matched_lm_of_kp.data(), &n));
+        matched_lm_of_kp.resize(frm.num_keypts());
+        return static_cast<unsigned int>(n);
+    }
+    //! match_current_and_last_frames(curr_frm, last_frm, margin) with the reprojections made on the device
+    //! (ovs_projection_match_current_and_last_reproject_host): last_pose_cw = last_frm.cam_pose_cw_ as {R row-major, t}; per last
+    //! keypoint: usable (landmark present, not an outlier; nullptr: all), pos_w (3 doubles), octave, angle, descriptor.
+    //! in_image / reproj (optional, together): the device's reprojection of each last keypoint's landmark.
+    unsigned int match_current_and_last_frames_reproject(const frame_index& curr, const ovs_frame_geometry& geometry, const bool is_monocular,
+                                                         const double true_baseline, const double* last_pose_cw,
+                                                         const std::vector<float>& scale_factors, const int num_last_keypts,
+                                                         const std::uint8_t* last_usable, const double* pos_w, const std::int32_t* last_octave,
+                                                         const float* last_angle, const std::uint8_t* lm_descriptors,
+                                                         const std::uint8_t* kp_has_observed_lm, std::vector<std::int32_t>& matched_last_of_kp,
+                                                         const float margin, std::uint8_t* in_image = nullptr, float* reproj = nullptr) const {
+        if (static_cast<int>(scale_factors.size()) != geometry.num_scale_levels)
+            throw std::invalid_argument("match_current_and_last_frames_reproject: one scale factor per level of the frame geometry");
+        matched_last_of_kp.assign(std::max(1, curr.num_keypts()), -1);
+        int n = 0;
+        detail::check(ovs_projection_match_current_and_last_reproject_host(curr.handle(), &geometry, is_monocular, true_baseline, last_pose_cw,
+                                                                           scale_factors.data(), num_last_keypts, last_usable, pos_w, last_octave,
+                                                                           last_angle, lm_descriptors, kp_has_observed_lm, margin, check_orientation_,
+                                                                           matched_last_of_kp.data(), &n, in_image, reproj));
+        matched_last_of_kp.resize(curr.num_keypts());
+        return static_cast<unsigned int>(n);
+    }
     //! match_frame_and_keyframe(curr_frm, keyfrm, already_matched_lms, margin, hamm_dist_thr): the keyframe's landmarks
     //! reprojected into curr_frm by the caller (reproj, pred_scale_level, usable); window levels [pred - 1, pred + 1]
     unsigned int match_frame_and_keyframe(const frame_index& curr, const std::vector<float>& scale_factors, const int num_landmarks,

@@ -371,6 +371,67 @@ typedef struct {
     double cols, rows;
 } ovs_camera;
 
+/* ---- tracking: frame::can_observe and the reprojections of the two projection searches (data/frame.cc, data/landmark.cc,
+ * camera/perspective.cc, camera/equirectangular.cc,
+ * module/tracking_module.cc search_local_landmarks, module/frame_tracker.cc motion_based_track) ---- */
+
+/* What the tracker's geometry reads of the current frame: camera_ (OVS_CAMERA_PERSPECTIVE, FISHEYE and RADIAL_DIVISION all
+ * reproject with the pinhole formula on undistorted keypoints; EQUIRECTANGULAR), camera_->img_bounds_ (min/max x/y; not read
+ * for equirectangular), rot_cw_ / trans_cw_ (row-major), cam_center_ (as the frame holds it: the library does not derive it),
+ * num_scale_levels_ (1 .. 16) and log_scale_factor_. */
+typedef struct {
+    ovs_camera camera;
+    float min_x, max_x, min_y, max_y;
+    double rot_cw[9], trans_cw[3], cam_center[3];
+    int32_t num_scale_levels;
+    float log_scale_factor;
+} ovs_frame_geometry;
+
+/* frame::can_observe(lm, ray_cos_thr, reproj, x_right, pred_scale_level) for nlm landmarks in one launch (one copy each way, one
+ * wait).  usable[l] (NULL: all) = the tracker's skip rule: the landmark is present, not will_be_erased() and not already
+ * observed in the frame.  pos_w[nlm*3] = get_pos_in_world(); mean_normal[nlm*3] = get_obs_mean_normal(); min_valid_dist /
+ * max_valid_dist = the landmark's raw min_valid_dist_ / max_valid_dist_ (the 0.7 / 1.3 factors are applied inside).  Outputs:
+ * observable[l]; where observable, reproj_xy[l*2] (the double reprojection rounded to float), x_right[l] (-1 equirectangular)
+ * and pred_scale_level[l] (landmark::predict_scale_level); elsewhere 0, 0, 0 and 0.  The conventions (summation orders, the
+ * float scale range, the double ray test, the level's log) are in DESIGN.md section 5.
+ * OVS_ERR_INVALID_ARG before any launch: nlm < 0, a null array with nlm > 0, an unknown camera model, num_scale_levels outside
+ * 1 .. 16, a log_scale_factor <= 0 or not finite, a non-finite pose or camera centre.  nlm == 0 returns without a launch. */
+int ovs_frame_can_observe_host(ovs_matcher* m, const ovs_frame_geometry* geometry, int nlm, const uint8_t* usable, const double* pos_w,
+                               const double* mean_normal, const float* min_valid_dist, const float* max_valid_dist, float ray_cos_thr,
+                               uint8_t* observable, float* reproj_xy, float* x_right, int32_t* pred_scale_level);
+
+/* The compute of tracking_module::search_local_landmarks: ovs_frame_can_observe_host on the matcher of f, then
+ * ovs_projection_match_frame_and_landmarks_host(f, scale_factors, num_scale_levels, nlm, observable, reproj_xy, x_right,
+ * pred_scale_level, lm_desc, kp_has_observed_lm, margin, lowe_ratio, ...) on those outputs: the same matcher and first-taker
+ * replay, so one launch more than that call.  scale_factors[num_scale_levels] = scale_factors_; lm_desc[nlm*32] =
+ * get_descriptor().  The per-landmark outputs are returned so that the caller can set reproj_in_tracking_,
+ * x_right_in_tracking_, scale_level_in_tracking_ and is_observable_in_tracking_ and call increase_num_observable().  Checks of
+ * ovs_frame_can_observe_host plus a null scale table, descriptor or output array. */
+int ovs_projection_search_local_landmarks_host(ovs_frame_index* f, const ovs_frame_geometry* geometry, const float* scale_factors, int nlm,
+                                               const uint8_t* usable, const double* pos_w, const double* mean_normal,
+                                               const float* min_valid_dist, const float* max_valid_dist, const uint8_t* lm_desc,
+                                               const uint8_t* kp_has_observed_lm, float ray_cos_thr, float margin, float lowe_ratio,
+                                               uint8_t* observable, float* reproj_xy, float* x_right, int32_t* pred_scale_level,
+                                               int32_t* matched_lm_of_kp, int* num_matches);
+
+/* match::projection::match_current_and_last_frames(curr_frm, last_frm, margin) with the reprojections made on the device: every
+ * landmark of the last frame is reprojected into the current frame (camera->reproject_to_image with the current pose, one
+ * launch), the direction comes from the two poses (trans_lc = R_lw (-R_cw^T t_cw) + t_lw against +-true_baseline, neither for
+ * is_monocular), and ovs_projection_match_current_and_last_host runs on the in-image ones: one launch more than that call.
+ * last_usable[i] (NULL: all) = last_frm.landmarks_[i] present and not an outlier; pos_w[n_last*3] = its position;
+ * last_pose_cw[12] = last_frm's cam_pose_cw_ {R row-major, t}; last_octave / last_angle = last_frm.undist_keypts_[i].octave /
+ * .angle; lm_desc[n_last*32] = landmark descriptors.  in_image_out[n_last] / reproj_xy_out[n_last*2] (both NULL or both given):
+ * the in-image flag and the reprojection (0, 0 where not in the image).  Checks of ovs_frame_can_observe_host plus a non-finite
+ * last pose or true_baseline, a null scale table, descriptor or octave array, an octave of a usable keypoint outside the scale
+ * table. */
+int ovs_projection_match_current_and_last_reproject_host(ovs_frame_index* curr, const ovs_frame_geometry* geometry, int is_monocular,
+                                                         double true_baseline, const double* last_pose_cw, const float* scale_factors,
+                                                         int n_last, const uint8_t* last_usable, const double* pos_w,
+                                                         const int32_t* last_octave, const float* last_angle, const uint8_t* lm_desc,
+                                                         const uint8_t* kp_has_observed_lm, float margin, int check_orientation,
+                                                         int32_t* matched_last_of_kp, int* num_matches, uint8_t* in_image_out,
+                                                         float* reproj_xy_out);
+
 /* ---- local mapping: module::two_view_triangulator (module/two_view_triangulator.cc) and the compute step of
  * mapping_module::create_new_landmarks (module/mapping_module.cc) ---- */
 

@@ -1,5 +1,5 @@
 // match_common.h -- the matcher handle shared by match_bruteforce.cu, match_window.cu, two_view_ransac.cu,
-// two_view_triangulate.cu and initializer.cu.  Its arenas
+// two_view_triangulate.cu, initializer.cu and tracking_search.cu.  Its arenas
 // grow and are carved through staging.h.
 #pragma once
 #include <algorithm>
@@ -35,8 +35,16 @@ struct ovs_matcher {
     // map initialisation's own arenas (initializer.cu): its solves and kernels leave the solver entry points' buffers untouched
     uint8_t* d_init = nullptr; size_t d_init_cap = 0;
     uint8_t* h_init = nullptr; size_t h_init_cap = 0;   // pinned
+    // the tracker's per-landmark geometry (tracking_search.cu): its kernel leaves the matchers' buffers untouched
+    uint8_t* d_trk = nullptr; size_t d_trk_cap = 0;
+    uint8_t* h_trk = nullptr; size_t h_trk_cap = 0;     // pinned
     cudaEvent_t ev[2]{};
     float last_kernel_us = 0.f;
     int num_requeries = 0;   // GPU re-queries issued by the greedy replays so far (diagnostic)
     std::vector<ovs_index_buf> index_pool;
 };
+
+namespace ovs {
+// the matcher a frame index was built on (match_window.cu): the composed tracking calls (tracking_search.cu) run on its stream
+ovs_matcher* frame_index_matcher(const ovs_frame_index* f);
+}  // namespace ovs

@@ -42,6 +42,8 @@ struct ovs_frame_index {
     bool has_xr = false;
 };
 
+ovs_matcher* ovs::frame_index_matcher(const ovs_frame_index* f) { return f->m; }
+
 namespace {
 
 constexpr int kTopK = 4;

@@ -4,6 +4,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
+from .optimize import Camera
 
 HAMMING_DIST_THR_LOW = 50
 HAMMING_DIST_THR_HIGH = 100
@@ -151,6 +152,40 @@ def camera_grid(min_x, max_x, min_y, max_y, num_grid_cols=64, num_grid_rows=48):
                 num_grid_cols, num_grid_rows)
 
 
+class FrameGeometry(C.Structure):
+    """ovs_frame_geometry: what frame::can_observe and the motion model's reprojection read of the current frame."""
+    _fields_ = [("camera", Camera), ("min_x", C.c_float), ("max_x", C.c_float), ("min_y", C.c_float), ("max_y", C.c_float),
+                ("rot_cw", C.c_double * 9), ("trans_cw", C.c_double * 3), ("cam_center", C.c_double * 3),
+                ("num_scale_levels", C.c_int32), ("log_scale_factor", C.c_float)]
+
+
+def _pose12(pose_cw):
+    """12 values (R row-major, t) from a 12-vector or a 3x4 / 4x4 cam_pose_cw_"""
+    P = np.asarray(pose_cw, np.float64)
+    if P.ndim == 2:
+        return np.concatenate([P[:3, :3].reshape(9), P[:3, 3]])
+    return P.reshape(12)
+
+
+def frame_geometry(camera, img_bounds, pose_cw, num_scale_levels, log_scale_factor, cam_center=None):
+    """camera: optimize.camera(...) (perspective, fisheye and radial_division reproject with the pinhole formula on undistorted
+    keypoints); img_bounds = (min_x, max_x, min_y, max_y) (camera_->img_bounds_); pose_cw: 12 values (R row-major, t) or a 3x4 / 4x4
+    matrix; cam_center: the frame's cam_center_ (default -R^T t); log_scale_factor: frame::log_scale_factor_ (float)."""
+    P = _pose12(pose_cw)
+    R, t = P[:9].reshape(3, 3), P[9:]
+    if cam_center is None:
+        cam_center = -(R.T @ t)
+    g = FrameGeometry()
+    g.camera = camera
+    g.min_x, g.max_x, g.min_y, g.max_y = (float(np.float32(v)) for v in img_bounds)
+    g.rot_cw[:] = [float(v) for v in R.reshape(9)]
+    g.trans_cw[:] = [float(v) for v in t]
+    g.cam_center[:] = [float(v) for v in np.reshape(cam_center, 3)]
+    g.num_scale_levels = int(num_scale_levels)
+    g.log_scale_factor = float(np.float32(log_scale_factor))
+    return g
+
+
 def _f32(a):
     a = np.ascontiguousarray(a, np.float32)
     return a, a.ctypes.data_as(C.c_void_p)
@@ -230,6 +265,27 @@ class frame_index:
         return idx, dist
 
 
+def _landmark_arrays(pos_w, mean_normal, min_valid_dist, max_valid_dist):
+    pos, pp = _f64(np.reshape(pos_w, (-1, 3))); nrm, pn = _f64(np.reshape(mean_normal, (-1, 3)))
+    lo, plo = _f32(min_valid_dist); hi, phi = _f32(max_valid_dist)
+    n = len(pos)
+    if len(nrm) != n or len(lo) != n or len(hi) != n:
+        raise ValueError("one position, mean normal and pair of valid distances per landmark")
+    return pos, pp, nrm, pn, lo, plo, hi, phi, n
+
+
+def _u8n(a, n, what):
+    """_u8p of an optional per-item flag array that must have n entries"""
+    if a is not None and np.size(a) != n:
+        raise ValueError("%s: %d entries, expected %d" % (what, np.size(a), n))
+    return _u8p(a)
+
+
+def _can_observe_outputs(n):
+    return (np.zeros(max(n, 1), np.uint8), np.zeros((max(n, 1), 2), np.float32), np.zeros(max(n, 1), np.float32),
+            np.zeros(max(n, 1), np.int32))
+
+
 class projection(_matcher_handle):
     """openvslam::match::projection (lowe_ratio_, check_orientation_)."""
 
@@ -264,6 +320,56 @@ class projection(_matcher_handle):
                                                                          int(self.check_orientation_), out.ctypes.data_as(C.c_void_p), C.byref(n)))
         return n.value, out[:curr.n]
 
+
+    def can_observe(self, geometry, pos_w, mean_normal, min_valid_dist, max_valid_dist, ray_cos_thr=0.5, usable=None):
+        """frame::can_observe(lm, ray_cos_thr, ...) for every landmark in one launch.  pos_w / mean_normal: (n, 3); min_valid_dist /
+        max_valid_dist: the landmarks' raw min_valid_dist_ / max_valid_dist_; usable: the tracker's skip rule (None: all)
+        -> observable (n,) bool, reproj_xy (n, 2) f32, x_right (n,) f32, pred_scale_level (n,) i32 (zeros where not observable)."""
+        pos, pp, nrm, pn, lo, plo, hi, phi, n = _landmark_arrays(pos_w, mean_normal, min_valid_dist, max_valid_dist)
+        _keep, pu = _u8n(usable, n, "usable")
+        ok, uv, xr, lv = _can_observe_outputs(n)
+        _lib.check(_lib.lib().ovs_frame_can_observe_host(self._h, C.byref(geometry), n, pu, pp, pn, plo, phi, C.c_float(ray_cos_thr),
+                                                         *(a.ctypes.data_as(C.c_void_p) for a in (ok, uv, xr, lv))))
+        return ok[:n].astype(bool), uv[:n], xr[:n], lv[:n]
+
+    def search_local_landmarks(self, frm, geometry, scale_factors, pos_w, mean_normal, min_valid_dist, max_valid_dist, lm_desc, usable=None,
+                               kp_has_observed_lm=None, margin=5.0, ray_cos_thr=0.5):
+        """The compute of tracking_module::search_local_landmarks: can_observe on the device, then match_frame_and_landmarks on its
+        outputs -> (num_matches, matched_lm_of_kp (frm.n,), observable, reproj_xy, x_right, pred_scale_level)."""
+        pos, pp, nrm, pn, lo, plo, hi, phi, n = _landmark_arrays(pos_w, mean_normal, min_valid_dist, max_valid_dist)
+        sf, psf = _f32(scale_factors); d, pd = _desc(lm_desc)
+        if len(sf) != geometry.num_scale_levels:
+            raise ValueError("search_local_landmarks: one scale factor per level")
+        if len(d) != n:
+            raise ValueError("search_local_landmarks: one descriptor per landmark")
+        _keep, pu = _u8n(usable, n, "usable"); _keep2, pk = _u8n(kp_has_observed_lm, frm.n, "kp_has_observed_lm")
+        ok, uv, xr, lv = _can_observe_outputs(n)
+        out = np.full(max(frm.n, 1), -1, np.int32); nm = C.c_int(0)
+        _lib.check(_lib.lib().ovs_projection_search_local_landmarks_host(
+            frm._h, C.byref(geometry), psf, n, pu, pp, pn, plo, phi, pd, pk, C.c_float(ray_cos_thr), C.c_float(margin), C.c_float(self.lowe_ratio_),
+            *(a.ctypes.data_as(C.c_void_p) for a in (ok, uv, xr, lv, out)), C.byref(nm)))
+        return nm.value, out[:frm.n], ok[:n].astype(bool), uv[:n], xr[:n], lv[:n]
+
+    def match_current_and_last_frames_reproject(self, curr, geometry, last_pose_cw, scale_factors, pos_w, last_octave, last_angle, lm_desc,
+                                                last_usable=None, kp_has_observed_lm=None, margin=20.0, is_monocular=True, true_baseline=0.0):
+        """match_current_and_last_frames(curr_frm, last_frm, margin) with the last frame's landmarks reprojected on the device and the
+        direction taken from the two poses -> (num_matches, matched_last_of_kp (curr.n,), in_image (n,) bool, reproj_xy (n, 2))."""
+        pos, pp = _f64(np.reshape(pos_w, (-1, 3)))
+        n = len(pos)
+        sf, psf = _f32(scale_factors); lv, plv = _i32(last_octave); la, pla = _f32(last_angle); d, pd = _desc(lm_desc)
+        if len(sf) != geometry.num_scale_levels:
+            raise ValueError("match_current_and_last_frames_reproject: one scale factor per level")
+        if len(lv) != n or len(la) != n or len(d) != n:
+            raise ValueError("match_current_and_last_frames_reproject: one octave, angle and descriptor per last-frame keypoint")
+        lp, plp = _f64(_pose12(last_pose_cw))
+        _keep, pu = _u8n(last_usable, n, "last_usable"); _keep2, pk = _u8n(kp_has_observed_lm, curr.n, "kp_has_observed_lm")
+        ok = np.zeros(max(n, 1), np.uint8); uv = np.zeros((max(n, 1), 2), np.float32)
+        out = np.full(max(curr.n, 1), -1, np.int32); nm = C.c_int(0)
+        _lib.check(_lib.lib().ovs_projection_match_current_and_last_reproject_host(
+            curr._h, C.byref(geometry), int(bool(is_monocular)), C.c_double(true_baseline), plp, psf, n, pu, pp, plv, pla, pd, pk,
+            C.c_float(margin), int(self.check_orientation_), out.ctypes.data_as(C.c_void_p), C.byref(nm), ok.ctypes.data_as(C.c_void_p),
+            uv.ctypes.data_as(C.c_void_p)))
+        return nm.value, out[:curr.n], ok[:n].astype(bool), uv[:n]
 
     def match_best(self, frm, ref_xy, ref_x_right, margin, min_level, max_level, q_angle, q_desc, usable=None, kp_unavailable=None,
                    hamm_dist_thr=HAMMING_DIST_THR_HIGH):
