@@ -143,9 +143,38 @@ OVS_BA_HD bool inv3_sym(const double* D, double* Di) {
     return true;
 }
 
-// Index of element (i, j) of a packed symmetric 3x3 / 6x6 (upper triangle, row-major).
-OVS_BA_HD int sym3(int i, int j) { return i <= j ? (i * 3 - i * (i - 1) / 2 + (j - i)) : (j * 3 - j * (j - 1) / 2 + (i - j)); }
-OVS_BA_HD int sym6(int i, int j) { return i <= j ? (i * 6 - i * (i - 1) / 2 + (j - i)) : (j * 6 - j * (j - 1) / 2 + (i - j)); }
+// Index of element (i, j) of a packed symmetric N x N (upper triangle, row-major).
+template <int N>
+OVS_BA_HD int sym(int i, int j) { return i <= j ? (i * N - i * (i - 1) / 2 + (j - i)) : (j * N - j * (j - 1) / 2 + (i - j)); }
+OVS_BA_HD int sym3(int i, int j) { return sym<3>(i, j); }
+OVS_BA_HD int sym6(int i, int j) { return sym<6>(i, j); }
+
+// (H + lambda I) x = b for a packed symmetric N x N H by Cholesky (thread-local).  Returns false if not positive definite.
+template <int N>
+OVS_BA_HD bool solve_spd(const double* Hs, double lambda, const double* b, double* x) {
+    double Lm[N][N];
+    for (int i = 0; i < N; ++i)
+        for (int j = 0; j <= i; ++j) {
+            double s = Hs[sym<N>(j, i)] + (i == j ? lambda : 0.0);
+            for (int k = 0; k < j; ++k) s -= Lm[i][k] * Lm[j][k];
+            if (i == j) {
+                if (!(s > 0.0) || !isfinite(s)) return false;
+                Lm[i][i] = sqrt(s);
+            } else Lm[i][j] = s / Lm[j][j];
+        }
+    double y[N];
+    for (int i = 0; i < N; ++i) {
+        double s = b[i];
+        for (int k = 0; k < i; ++k) s -= Lm[i][k] * y[k];
+        y[i] = s / Lm[i][i];
+    }
+    for (int i = N - 1; i >= 0; --i) {
+        double s = y[i];
+        for (int k = i + 1; k < N; ++k) s -= Lm[k][i] * x[k];
+        x[i] = s / Lm[i][i];
+    }
+    return true;
+}
 
 // ---- per-edge blocks of the normal equations from the edge's Jacobians, residual and robust weight ww (= rho'(chi2) * info)
 // The bundle adjusters store only {Jp, Jl, ww, e} per edge and form these blocks where they are read, in several kernels; the

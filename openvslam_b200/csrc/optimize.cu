@@ -27,6 +27,8 @@
 //
 // Transform optimiser (loop closure, optimize::transform_optimizer): the same shape with one Sim3 vertex and a 7x7
 // system -- both rounds, the outlier cut, the early exit and the write-back are ONE kernel, k_sim3_optimize.
+// The two kernels share the cluster reduction (ClusterSum), the Levenberg round (cluster_lm_round) and the packed SPD
+// solve (ovs::solve_spd, ba_math.cuh); each keeps its own edge pass, update and round structure.
 //
 // Pose graph (loop closure, optimize::graph_optimizer): one Sim3 vertex per keyframe, a dense 7 n_free system assembled per trial
 // batch (k_pg_*) and factorised by the local BA's solver, under the same device-side Levenberg controller (LmCtl, k_ba_reduce,
@@ -116,6 +118,49 @@ __device__ __forceinline__ void cluster_sync_mem() {
     asm volatile("barrier.cluster.arrive.release.aligned;\n" ::: "memory");
     asm volatile("barrier.cluster.wait.acquire.aligned;\n" ::: "memory");
 }
+
+// Sum of up to NS per-thread values over a cluster of CLUSTER CTAs of THREADS threads each, the same bits in every CTA: each
+// value is summed over the warp, then over the warps in index order, then over the ranks in rank order.  Every CTA pushes its
+// block sums into slot [its rank] of EVERY CTA's shared memory (st.shared::cluster), one cluster barrier (release / acquire)
+// makes them visible, every CTA adds the slots in rank order.  The slots are double-buffered by the parity of the reduction,
+// so one barrier per reduction is enough: a CTA that is already pushing reduction q + 1 writes the other buffer, and it can
+// only push reduction q + 2 after every CTA has arrived at barrier q + 1, i.e. has finished reading buffer q.
+// Every thread of the cluster calls it; the result stays valid until the next call.
+template <int NS, int CLUSTER, int THREADS>
+struct ClusterSum {
+    int parity = 0;
+    __device__ __forceinline__ const double* operator()(const double* acc, int count) {
+        constexpr int NW = THREADS / 32;
+        __shared__ double sm_red[NS][NW];
+        __shared__ double s_slots[2][CLUSTER][NS];
+        __shared__ double s_sys[NS];
+        const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+        const unsigned rank = cluster_rank();
+        __syncthreads();
+        for (int k = 0; k < count; ++k) {
+            const double v = warp_sum(acc[k]);
+            if (lane == 0) sm_red[k][wid] = v;
+        }
+        __syncthreads();
+        if (tid < count) {
+            double t = 0;
+#pragma unroll
+            for (int k = 0; k < NW; ++k) t += sm_red[tid][k];
+#pragma unroll
+            for (unsigned r = 0; r < (unsigned)CLUSTER; ++r) st_dsmem(&s_slots[parity][rank][tid], r, t);
+        }
+        cluster_sync_mem();
+        if (tid < count) {
+            double v = 0;
+#pragma unroll
+            for (int r = 0; r < CLUSTER; ++r) v += s_slots[parity][r][tid];
+            s_sys[tid] = v;
+        }
+        parity ^= 1;
+        __syncthreads();
+        return s_sys;
+    }
+};
 
 // Speculative Levenberg trials: g2o rejects a step by multiplying lambda by ni (2, 4, 8, ...), so the
 // damping values of the next trials are known in advance.  kSpec of them are evaluated in one batch
@@ -1988,52 +2033,119 @@ struct PoseOptArgs {
     double* stats;             // [0] iterations [1] trials(solves) [2] rounds [3] final chi2 [4] inliers [5..] lambda_init per round
 };
 
-// 6x6 SPD solve by Cholesky (thread-local).  Returns false if not positive definite.
-__device__ bool solve6(const double* Hs /* packed 21 */, double lambda, const double* b, double* x) {
-    double Lm[6][6];
-    for (int i = 0; i < 6; ++i)
-        for (int j = 0; j <= i; ++j) {
-            double s = Hs[ovs::sym6(j, i)] + (i == j ? lambda : 0.0);
-            for (int k = 0; k < j; ++k) s -= Lm[i][k] * Lm[j][k];
-            if (i == j) {
-                if (!(s > 0.0) || !isfinite(s)) return false;
-                Lm[i][i] = sqrt(s);
-            } else Lm[i][j] = s / Lm[j][j];
+struct LmRoundStats {
+    int iterations, trials;      // iterations run, trials (solves) over them
+    double lambda_init;          // set when iterations > 0
+    double lambda, chi2;         // after the last iteration; set when iterations > 0
+};
+
+// SparseOptimizer::optimize(iterations) of g2o's OptimizationAlgorithmLevenberg with a fresh initializeOptimization (lambda_init
+// again) for one vertex of D parameters (an estimate of P doubles in shared memory, est), run redundantly by every CTA of the
+// cluster on the sums `reduce` leaves in every CTA.  build(est, acc) is the kernel's edge pass at an estimate: the edge errors
+// it stores and this thread's share of {H (packed D x D), b (D), robust chi2} in acc; oplus(est, x, out) applies an update.
+// g2o evaluates the errors at the candidate of a trial and, once the trial is accepted, evaluates them again at the same
+// estimate at the top of the next iteration, where it also linearises.  Here the trial's pass over the edges already forms H
+// and b at the candidate (same code, same summation order as the pass at the top of an iteration), so an accepted trial hands
+// the next iteration its system: one pass over the edges and one cluster reduction per iteration instead of two.  A round
+// starts with a fresh pass.
+template <int D, int P, class Reduce, class Build, class Oplus>
+__device__ __forceinline__ LmRoundStats cluster_lm_round(int iterations, double* est, Reduce& reduce, Build&& build, Oplus&& oplus) {
+    constexpr int NH = D * (D + 1) / 2, NS = NH + D + 1;
+    __shared__ double s_cand[P], s_x[D];
+    __shared__ int s_flag;
+    const int tid = threadIdx.x;
+    LmRoundStats st{0, 0, 0.0, 0.0, 0.0};
+    double lambda = 0, ni = 2;
+    bool ok = true, have_sys = false;
+    int it = 0;
+    double Hs[NH], bs[D], currentChi = 0;
+    for (; it < iterations && ok; ++it) {
+        if (!have_sys) {
+            double acc[NS];
+            build(est, acc);
+            const double* sys = reduce(acc, NS);
+#pragma unroll
+            for (int k = 0; k < NH; ++k) Hs[k] = sys[k];
+#pragma unroll
+            for (int k = 0; k < D; ++k) bs[k] = sys[NH + k];
+            currentChi = sys[NH + D];
+            have_sys = true;
         }
-    double y[6];
-    for (int i = 0; i < 6; ++i) {
-        double s = b[i];
-        for (int k = 0; k < i; ++k) s -= Lm[i][k] * y[k];
-        y[i] = s / Lm[i][i];
+        if (it == 0) {
+            double md = 0;
+#pragma unroll
+            for (int k = 0; k < D; ++k) md = fmax(md, fabs(Hs[ovs::sym<D>(k, k)]));
+            lambda = 1e-5 * md;
+            ni = 2;
+            st.lambda_init = lambda;
+        }
+        double rho = 0;
+        int qmax = 0;
+        do {
+            if (tid == 0) {
+                double xs[D];
+                const bool ok2 = ovs::solve_spd<D>(Hs, lambda, bs, xs);
+                s_flag = ok2 ? 1 : 0;
+                if (ok2) {
+                    for (int k = 0; k < D; ++k) s_x[k] = xs[k];
+                    double out[P];
+                    oplus(est, xs, out);
+                    for (int k = 0; k < P; ++k) s_cand[k] = out[k];
+                } else {
+                    for (int k = 0; k < P; ++k) s_cand[k] = est[k];
+                }
+            }
+            __syncthreads();
+            const bool ok2 = s_flag != 0;
+            const double* sys;
+            {
+                double acc[NS];
+                build(s_cand, acc);
+                sys = reduce(acc, NS);
+            }
+            double tempChi = sys[NH + D];
+            if (!ok2) tempChi = DBL_MAX;
+            rho = currentChi - tempChi;
+            double scale = 0;
+            if (ok2) for (int k = 0; k < D; ++k) scale += s_x[k] * (lambda * s_x[k] + bs[k]);
+            scale += 1e-3;
+            rho /= scale;
+            const bool accept = rho > 0 && isfinite(tempChi);
+            if (accept) {
+                double alpha = 1. - pow((2 * rho - 1), 3);
+                alpha = fmin(alpha, 2. / 3.);
+                lambda *= fmax(1. / 3., alpha);
+                ni = 2;
+                currentChi = tempChi;
+#pragma unroll
+                for (int k = 0; k < NH; ++k) Hs[k] = sys[k];      // the system at the accepted estimate
+#pragma unroll
+                for (int k = 0; k < D; ++k) bs[k] = sys[NH + k];
+            } else {
+                lambda *= ni;
+                ni *= 2;
+            }
+            __syncthreads();                    // the sums, s_x, est and s_cand have been read by every thread
+            if (accept && tid < P) est[tid] = s_cand[tid];
+            __syncthreads();
+            ++qmax; ++st.trials;
+        } while (rho < 0 && qmax < kMaxTrials);
+        if (qmax == kMaxTrials || rho == 0) ok = false;
     }
-    for (int i = 5; i >= 0; --i) {
-        double s = y[i];
-        for (int k = i + 1; k < 6; ++k) s -= Lm[k][i] * x[k];
-        x[i] = s / Lm[i][i];
-    }
-    return true;
+    st.iterations = it;
+    st.lambda = lambda; st.chi2 = currentChi;
+    return st;
 }
 
 // pose_optimizer::optimize: the whole call is ONE kernel on a thread-block cluster of kPoseCluster
 // CTAs (the edge linearisation is FP64-throughput bound on one SM).  Every CTA owns a slice of the
-// edges; the 6x6 normal equations and the chi2 sums are reduced across the cluster through
-// distributed shared memory in a fixed order, so every CTA then takes the same Levenberg decision
-// redundantly (no broadcast needed).  Edge state lives in global scratch (err: n x 3 doubles,
-// level: n bytes).
-// Reduction across the cluster: every CTA pushes its block sums into slot [its rank] of EVERY CTA's shared memory
-// (st.shared::cluster), one cluster barrier (release / acquire) makes them visible, every CTA adds the slots in rank order.
-// The slots are double-buffered by the parity of the reduction, so one barrier per reduction is enough: a CTA that is
-// already pushing reduction q + 1 writes the other buffer, and it can only push reduction q + 2 after every CTA has arrived
-// at barrier q + 1, i.e. has finished reading buffer q.
-
+// edges; the 6x6 normal equations and the chi2 sums are reduced across the cluster (ClusterSum),
+// so every CTA then takes the same Levenberg decision redundantly (no broadcast needed).  Edge state
+// lives in global scratch (err: n x 3 doubles, level: n bytes).
 __global__ void __cluster_dims__(kPoseCluster, 1, 1) __launch_bounds__(kPoseThreads, 1)
 k_pose_optimize(PoseOptArgs A, double* __restrict__ err, unsigned char* __restrict__ level) {
-    constexpr int NW = kPoseThreads / 32;
-    __shared__ double sm_red[28][NW];
-    __shared__ double s_slots[2][kPoseCluster][28];
-    __shared__ double s_sys[28], s_pose[12], s_cand[12], s_x[6];
-    __shared__ int s_flag;
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    __shared__ double s_pose[12];
+    const int tid = threadIdx.x;
     const unsigned my_rank = cluster_rank();
     const int gtid = (int)my_rank * kPoseThreads + tid;
     constexpr int GS = kPoseCluster * kPoseThreads;
@@ -2041,37 +2153,12 @@ k_pose_optimize(PoseOptArgs A, double* __restrict__ err, unsigned char* __restri
     if (tid < 12) s_pose[tid] = A.pose[tid];
     for (int i = gtid; i < n; i += GS) { level[i] = 0; A.outlier[i] = 0; }
     cluster_sync_mem();     // every CTA of the cluster is running before anyone writes into its shared memory
-
-    // block-reduces `count` per-thread values (acc), then sums over the cluster into s_sys (the same bits in every CTA)
-    int parity = 0;
-    auto reduce_all = [&](const double* acc, int count) {
-        __syncthreads();
-        for (int k = 0; k < count; ++k) {
-            const double v = warp_sum(acc[k]);
-            if (lane == 0) sm_red[k][wid] = v;
-        }
-        __syncthreads();
-        if (tid < count) {
-            double t = 0;
-#pragma unroll
-            for (int k = 0; k < NW; ++k) t += sm_red[tid][k];
-#pragma unroll
-            for (unsigned r = 0; r < (unsigned)kPoseCluster; ++r) st_dsmem(&s_slots[parity][my_rank][tid], r, t);
-        }
-        cluster_sync_mem();
-        if (tid < count) {
-            double v = 0;
-#pragma unroll
-            for (int r = 0; r < kPoseCluster; ++r) v += s_slots[parity][r][tid];
-            s_sys[tid] = v;
-        }
-        parity ^= 1;
-        __syncthreads();
-    };
+    ClusterSum<28, kPoseCluster, kPoseThreads> reduce_all;
+    bool use_huber = true;
 
     // computeActiveErrors + buildSystem in one pass at pose `ps`: edge errors to err[], this thread's share of
     // {H (21), b (6), robust chi2} over its active edges into acc
-    auto build_local = [&](const double* ps, bool use_huber, double* acc) {
+    auto build_local = [&](const double* ps, double* acc) {
 #pragma unroll
         for (int k = 0; k < 28; ++k) acc[k] = 0;
         double pose[12];
@@ -2107,93 +2194,14 @@ k_pose_optimize(PoseOptArgs A, double* __restrict__ err, unsigned char* __restri
         }
     };
 
-    bool use_huber = true;
     int total_iters = 0, total_trials = 0, rounds = 0, num_bad = 0;
     for (int trial = 0; trial < A.num_trials; ++trial) {
-        // ---- optimizer.optimize(num_each_iter).  g2o evaluates the errors at the candidate of a trial and, once the trial
-        // is accepted, evaluates them again at the same pose at the top of the next iteration, where it also linearises.
-        // Here the trial's pass over the edges already forms H and b at the candidate (same code, same summation order as
-        // the pass at the top of an iteration), so an accepted trial hands the next iteration its system: one pass over the
-        // edges and one cluster reduction per iteration instead of two.  A round starts with a fresh pass (the outlier levels
-        // and the robust kernel change between rounds).
-        double lambda = 0, ni = 2;
-        bool ok = true;
-        int it = 0;
-        bool have_sys = false;
-        double Hs[21], bs[6], currentChi = 0;
-        for (; it < A.num_each_iter && ok; ++it) {
-            if (!have_sys) {
-                double acc[28];
-                build_local(s_pose, use_huber, acc);
-                reduce_all(acc, 28);
-#pragma unroll
-                for (int k = 0; k < 21; ++k) Hs[k] = s_sys[k];
-#pragma unroll
-                for (int k = 0; k < 6; ++k) bs[k] = s_sys[21 + k];
-                currentChi = s_sys[27];
-                have_sys = true;
-            }
-            if (it == 0) {
-                double md = 0;
-                const int dg[6] = {0, 6, 11, 15, 18, 20};
-                for (int k = 0; k < 6; ++k) md = fmax(md, fabs(Hs[dg[k]]));
-                lambda = 1e-5 * md;
-                ni = 2;
-                if (gtid == 0 && rounds < 8) A.stats[5 + rounds] = lambda;
-            }
-            double rho = 0;
-            int qmax = 0;
-            do {
-                if (tid == 0) {
-                    double xs[6];
-                    const bool ok2 = solve6(Hs, lambda, bs, xs);
-                    s_flag = ok2 ? 1 : 0;
-                    if (ok2) {
-                        for (int k = 0; k < 6; ++k) s_x[k] = xs[k];
-                        double out[12];
-                        ovs::pose_oplus(s_pose, xs, out);
-                        for (int k = 0; k < 12; ++k) s_cand[k] = out[k];
-                    } else {
-                        for (int k = 0; k < 12; ++k) s_cand[k] = s_pose[k];
-                    }
-                }
-                __syncthreads();
-                const bool ok2 = s_flag != 0;
-                {
-                    double acc[28];
-                    build_local(s_cand, use_huber, acc);
-                    reduce_all(acc, 28);
-                }
-                double tempChi = s_sys[27];
-                if (!ok2) tempChi = DBL_MAX;
-                rho = currentChi - tempChi;
-                double scale = 0;
-                if (ok2) for (int k = 0; k < 6; ++k) scale += s_x[k] * (lambda * s_x[k] + bs[k]);
-                scale += 1e-3;
-                rho /= scale;
-                const bool accept = rho > 0 && isfinite(tempChi);
-                if (accept) {
-                    double alpha = 1. - pow((2 * rho - 1), 3);
-                    alpha = fmin(alpha, 2. / 3.);
-                    lambda *= fmax(1. / 3., alpha);
-                    ni = 2;
-                    currentChi = tempChi;
-#pragma unroll
-                    for (int k = 0; k < 21; ++k) Hs[k] = s_sys[k];      // the system at the accepted pose
-#pragma unroll
-                    for (int k = 0; k < 6; ++k) bs[k] = s_sys[21 + k];
-                } else {
-                    lambda *= ni;
-                    ni *= 2;
-                }
-                __syncthreads();                    // s_sys, s_x, s_pose, s_cand have been read by every thread
-                if (accept && tid < 12) s_pose[tid] = s_cand[tid];
-                __syncthreads();
-                ++qmax; ++total_trials;
-            } while (rho < 0 && qmax < 10);
-            if (qmax == 10 || rho == 0) ok = false;
-        }
-        total_iters += it; ++rounds;
+        // ---- optimizer.optimize(num_each_iter); a round starts with a fresh pass (the outlier levels and the robust kernel
+        // change between rounds)
+        const LmRoundStats r = cluster_lm_round<6, 12>(A.num_each_iter, s_pose, reduce_all, build_local,
+                                                       [](const double* ps, const double* x, double* out) { ovs::pose_oplus(ps, x, out); });
+        if (r.iterations > 0 && gtid == 0 && rounds < 8) A.stats[5 + rounds] = r.lambda_init;
+        total_iters += r.iterations; total_trials += r.trials; ++rounds;
         // ---- outlier re-classification
         {
             double pose[12];
@@ -2220,8 +2228,7 @@ k_pose_optimize(PoseOptArgs A, double* __restrict__ err, unsigned char* __restri
                 A.outlier[i] = outl ? 1 : 0;
                 bad[0] += outl ? 1.0 : 0.0;
             }
-            reduce_all(bad, 1);
-            num_bad = (int)(s_sys[0] + 0.5);
+            num_bad = (int)(reduce_all(bad, 1)[0] + 0.5);
             __syncthreads();
         }
         if (trial == A.num_trials - 2) use_huber = false;
@@ -2236,9 +2243,9 @@ k_pose_optimize(PoseOptArgs A, double* __restrict__ err, unsigned char* __restri
         const double e0 = err[3 * (size_t)i], e1 = err[3 * (size_t)i + 1], e2 = err[3 * (size_t)i + 2];
         fc[0] += w * (e0 * e0 + e1 * e1) + (stereo ? w * e2 * e2 : 0.0);
     }
-    reduce_all(fc, 1);
+    const double final_chi2 = reduce_all(fc, 1)[0];
     if (gtid == 0) {
-        A.stats[0] = total_iters; A.stats[1] = total_trials; A.stats[2] = rounds; A.stats[3] = s_sys[0]; A.stats[4] = n - num_bad;
+        A.stats[0] = total_iters; A.stats[1] = total_trials; A.stats[2] = rounds; A.stats[3] = final_chi2; A.stats[4] = n - num_bad;
     }
     if (gtid < 12) A.pose[gtid] = s_pose[gtid];
 }
@@ -2367,50 +2374,21 @@ struct Sim3OptArgs {
 
 // transform_optimizer::optimize: the whole call is ONE kernel on a cluster of kSim3Cluster CTAs, organised as
 // k_pose_optimize: every CTA owns a grid-stride slice of the pairs (both edges of a pair in one thread), the 7x7 system and the
-// chi2 are reduced across the cluster through distributed shared memory in a fixed order (warp, then warps, then ranks), so
-// every CTA holds the same bits and takes the same Levenberg decision.  err (n x 4: e12, e21) keeps the errors of the last
-// evaluated trial, which the outlier tests read as g2o's chi2() does; level (n) is 1 for the pairs cut so far.
+// chi2 are reduced across the cluster (ClusterSum), so every CTA holds the same bits and takes the same Levenberg decision.
+// err (n x 4: e12, e21) keeps the errors of the last evaluated trial, which the outlier tests read as g2o's chi2() does;
+// level (n) is 1 for the pairs cut so far.
 __global__ void __cluster_dims__(kSim3Cluster, 1, 1) __launch_bounds__(kSim3Threads, 1)
 k_sim3_optimize(Sim3OptArgs A, double* __restrict__ err, unsigned char* __restrict__ level) {
-    constexpr int NW = kSim3Threads / 32;
     constexpr int NS = kSim3Sums;
-    __shared__ double sm_red[NS][NW];
-    __shared__ double s_slots[2][kSim3Cluster][NS];
-    __shared__ double s_sys[NS], s_S[13], s_cand[13], s_x[7];
-    __shared__ int s_flag;
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    __shared__ double s_S[13];
+    const int tid = threadIdx.x;
     const unsigned my_rank = cluster_rank();
     const int gtid = (int)my_rank * kSim3Threads + tid;
     const int n = A.n;
     if (tid < 13) s_S[tid] = A.sim3[tid];
     for (int i = gtid; i < n; i += kSim3Stride) { level[i] = 0; A.inlier[i] = 0; }
     cluster_sync_mem();     // every CTA of the cluster is running before anyone writes into its shared memory
-
-    int parity = 0;
-    auto reduce_all = [&](const double* acc, int count) {
-        __syncthreads();
-        for (int k = 0; k < count; ++k) {
-            const double v = warp_sum(acc[k]);
-            if (lane == 0) sm_red[k][wid] = v;
-        }
-        __syncthreads();
-        if (tid < count) {
-            double t = 0;
-#pragma unroll
-            for (int k = 0; k < NW; ++k) t += sm_red[tid][k];
-#pragma unroll
-            for (unsigned r = 0; r < (unsigned)kSim3Cluster; ++r) st_dsmem(&s_slots[parity][my_rank][tid], r, t);
-        }
-        cluster_sync_mem();
-        if (tid < count) {
-            double v = 0;
-#pragma unroll
-            for (int r = 0; r < kSim3Cluster; ++r) v += s_slots[parity][r][tid];
-            s_sys[tid] = v;
-        }
-        parity ^= 1;
-        __syncthreads();
-    };
+    ClusterSum<NS, kSim3Cluster, kSim3Threads> reduce_all;
 
     // computeActiveErrors + buildSystem at S in one pass: errors to err[], this thread's share of {H, b, robust chi2}
     auto build_local = [&](const double* Sp, double* acc) {
@@ -2443,7 +2421,7 @@ k_sim3_optimize(Sim3OptArgs A, double* __restrict__ err, unsigned char* __restri
                 const double ww = r1 * w;
                 for (int a = 0; a < 7; ++a) {
                     acc[28 + a] -= J[a] * ww * e[0] + J[7 + a] * ww * e[1];
-                    for (int c = a; c < 7; ++c) acc[ovs::sym7(a, c)] += J[a] * ww * J[c] + J[7 + a] * ww * J[7 + c];
+                    for (int c = a; c < 7; ++c) acc[ovs::sym<7>(a, c)] += J[a] * ww * J[c] + J[7 + a] * ww * J[7 + c];
                 }
             }
         }
@@ -2462,103 +2440,27 @@ k_sim3_optimize(Sim3OptArgs A, double* __restrict__ err, unsigned char* __restri
         return bad;
     };
 
-    int total_iters = 0, total_trials = 0, rounds = 0;
+    // round 0: num_first_iter iterations and the outlier cut; fewer than 10 pairs left: return 0, g2o_Sim3_12 untouched.
+    // round 1: num_iter iterations and the outlier cut.
+    int total_iters = 0, total_trials = 0, rounds = 0, num_outliers = 0;
     double last_lambda = 0, last_chi = 0;
-    // SparseOptimizer::optimize(iterations) with a fresh initializeOptimization (lambda_init again).  As in k_pose_optimize
-    // the pass that evaluates a trial also forms H and b at the candidate, which an accepted trial hands to the next iteration.
-    auto lm_round = [&](int iterations) {
-        double lambda = 0, ni = 2;
-        bool ok = true, have_sys = false;
-        int it = 0;
-        double Hs[28], bs[7], currentChi = 0;
-        for (; it < iterations && ok; ++it) {
-            if (!have_sys) {
-                double acc[NS];
-                build_local(s_S, acc);
-                reduce_all(acc, NS);
-#pragma unroll
-                for (int k = 0; k < 28; ++k) Hs[k] = s_sys[k];
-#pragma unroll
-                for (int k = 0; k < 7; ++k) bs[k] = s_sys[28 + k];
-                currentChi = s_sys[35];
-                have_sys = true;
-            }
-            if (it == 0) {
-                double md = 0;
-                for (int k = 0; k < 7; ++k) md = fmax(md, fabs(Hs[ovs::sym7(k, k)]));
-                lambda = 1e-5 * md;
-                ni = 2;
-                if (gtid == 0) A.stats[5 + rounds] = lambda;
-            }
-            double rho = 0;
-            int qmax = 0;
-            do {
-                if (tid == 0) {
-                    double xs[7];
-                    const bool ok2 = ovs::solve7(Hs, lambda, bs, xs);
-                    s_flag = ok2 ? 1 : 0;
-                    if (ok2) {
-                        for (int k = 0; k < 7; ++k) s_x[k] = xs[k];
-                        double out[13];
-                        ovs::sim3_oplus(s_S, xs, A.fix_scale != 0, out);
-                        for (int k = 0; k < 13; ++k) s_cand[k] = out[k];
-                    } else {
-                        for (int k = 0; k < 13; ++k) s_cand[k] = s_S[k];
-                    }
-                }
-                __syncthreads();
-                const bool ok2 = s_flag != 0;
-                {
-                    double acc[NS];
-                    build_local(s_cand, acc);
-                    reduce_all(acc, NS);
-                }
-                double tempChi = s_sys[35];
-                if (!ok2) tempChi = DBL_MAX;
-                rho = currentChi - tempChi;
-                double scale = 0;
-                if (ok2) for (int k = 0; k < 7; ++k) scale += s_x[k] * (lambda * s_x[k] + bs[k]);   // all seven components
-                scale += 1e-3;
-                rho /= scale;
-                const bool accept = rho > 0 && isfinite(tempChi);
-                if (accept) {
-                    double alpha = 1. - pow((2 * rho - 1), 3);
-                    alpha = fmin(alpha, 2. / 3.);
-                    lambda *= fmax(1. / 3., alpha);
-                    ni = 2;
-                    currentChi = tempChi;
-#pragma unroll
-                    for (int k = 0; k < 28; ++k) Hs[k] = s_sys[k];
-#pragma unroll
-                    for (int k = 0; k < 7; ++k) bs[k] = s_sys[28 + k];
-                } else {
-                    lambda *= ni;
-                    ni *= 2;
-                }
-                __syncthreads();                    // s_sys, s_x, s_S, s_cand have been read by every thread
-                if (accept && tid < 13) s_S[tid] = s_cand[tid];
-                __syncthreads();
-                ++qmax; ++total_trials;
-            } while (rho < 0 && qmax < 10);
-            last_lambda = lambda; last_chi = currentChi;
-            if (qmax == 10 || rho == 0) ok = false;
+    bool success = true;
+    for (; rounds < 2 && success; ++rounds) {
+        const LmRoundStats r = cluster_lm_round<7, 13>(rounds == 0 ? A.num_first_iter : A.num_iter, s_S, reduce_all, build_local,
+                                                       [&](const double* S, const double* x, double* out) {
+                                                           ovs::sim3_oplus(S, x, A.fix_scale != 0, out);
+                                                       });
+        if (r.iterations > 0) {
+            if (gtid == 0) A.stats[5 + rounds] = r.lambda_init;
+            last_lambda = r.lambda; last_chi = r.chi2;
         }
-        if (gtid == 0) A.stats[7 + rounds] = it;
-        total_iters += it; ++rounds;
-    };
-
-    lm_round(A.num_first_iter);
-    double cnt[1] = {cut_outliers()};
-    reduce_all(cnt, 1);
-    const int num_outliers = (int)(s_sys[0] + 0.5);
-    const bool success = n - num_outliers >= 10;     // otherwise: return 0, g2o_Sim3_12 untouched
-    int num_inliers = 0;
-    if (success) {
-        lm_round(A.num_iter);
-        cnt[0] = cut_outliers();
-        reduce_all(cnt, 1);
-        num_inliers = n - num_outliers - (int)(s_sys[0] + 0.5);
+        if (gtid == 0) A.stats[7 + rounds] = r.iterations;
+        total_iters += r.iterations; total_trials += r.trials;
+        const double cnt[1] = {cut_outliers()};
+        num_outliers += (int)(reduce_all(cnt, 1)[0] + 0.5);
+        if (rounds == 0) success = n - num_outliers >= 10;
     }
+    const int num_inliers = success ? n - num_outliers : 0;
     double fc[1] = {0};
     for (int i = gtid; i < n; i += kSim3Stride) {
         A.inlier[i] = level[i] ? 0 : 1;
@@ -2566,9 +2468,9 @@ k_sim3_optimize(Sim3OptArgs A, double* __restrict__ err, unsigned char* __restri
         const double* e = err + 4 * (size_t)i;
         fc[0] += (double)A.w1[i] * (e[0] * e[0] + e[1] * e[1]) + (double)A.w2[i] * (e[2] * e[2] + e[3] * e[3]);
     }
-    reduce_all(fc, 1);
+    const double final_chi2 = reduce_all(fc, 1)[0];
     if (gtid == 0) {
-        A.stats[0] = total_iters; A.stats[1] = total_trials; A.stats[2] = rounds; A.stats[3] = s_sys[0]; A.stats[4] = num_inliers;
+        A.stats[0] = total_iters; A.stats[1] = total_trials; A.stats[2] = rounds; A.stats[3] = final_chi2; A.stats[4] = num_inliers;
         A.stats[9] = last_lambda; A.stats[10] = last_chi;
     }
     if (success && gtid < 13) A.sim3[gtid] = s_S[gtid];

@@ -139,34 +139,8 @@ OVS_BA_HD void sim3_edge_backward(const CameraD& cam2, const double* S, const do
     }
 }
 
-// Packed upper-triangle index of element (i, j) of a symmetric 7 x 7.
-OVS_BA_HD int sym7(int i, int j) { return i <= j ? (i * 7 - i * (i - 1) / 2 + (j - i)) : (j * 7 - j * (j - 1) / 2 + (i - j)); }
-
-// (H + lambda I) x = b for a packed symmetric 7 x 7 H by Cholesky.  Returns false if not positive definite.
-OVS_BA_HD bool solve7(const double* Hs, double lambda, const double* b, double* x) {
-    double Lm[7][7];
-    for (int i = 0; i < 7; ++i)
-        for (int j = 0; j <= i; ++j) {
-            double s = Hs[sym7(j, i)] + (i == j ? lambda : 0.0);
-            for (int k = 0; k < j; ++k) s -= Lm[i][k] * Lm[j][k];
-            if (i == j) {
-                if (!(s > 0.0) || !isfinite(s)) return false;
-                Lm[i][i] = sqrt(s);
-            } else Lm[i][j] = s / Lm[j][j];
-        }
-    double y[7];
-    for (int i = 0; i < 7; ++i) {
-        double s = b[i];
-        for (int k = 0; k < i; ++k) s -= Lm[i][k] * y[k];
-        y[i] = s / Lm[i][i];
-    }
-    for (int i = 6; i >= 0; --i) {
-        double s = y[i];
-        for (int k = i + 1; k < 7; ++k) s -= Lm[k][i] * x[k];
-        x[i] = s / Lm[i][i];
-    }
-    return true;
-}
+// (H + lambda I) x = b for the packed symmetric 7 x 7 H of the transform optimiser (ba_math.cuh's solve_spd).
+OVS_BA_HD bool solve7(const double* Hs, double lambda, const double* b, double* x) { return solve_spd<7>(Hs, lambda, b, x); }
 
 // ------------------------------------------------------------------ pose graph (optimize::graph_optimizer, loop closure)
 // One Sim3 vertex per keyframe (S_iw, camera from world), one relative edge per keyframe pair with the measurement S_ji:

@@ -165,19 +165,21 @@ def test_math_header_equals_oracle(s3, shim, model):
 
 
 def test_math_header_solve7(shim):
+    """the packed SPD solve of both cluster optimisers: N = 7 (Sim3) and N = 6 (pose)"""
     rng = np.random.default_rng(14)
-    for _ in range(50):
-        A = rng.normal(size=(12, 7))
-        H = A.T @ A
-        b = rng.normal(size=7)
-        lam = 10.0 ** rng.uniform(-6, 1)
-        packed = np.array([H[i, j] for i in range(7) for j in range(i, 7)])
-        x = np.zeros(7)
-        assert shim.sc_solve7(_ptr(packed), C.c_double(lam), _ptr(b), _ptr(x)) == 1
-        ref = np.linalg.solve(H + lam * np.eye(7), b)
-        assert np.abs(x - ref).max() <= 1e-9 * max(1.0, np.abs(ref).max())
-    neg = np.zeros(28); neg[0] = -1.0
-    assert shim.sc_solve7(_ptr(neg), C.c_double(0.0), _ptr(np.zeros(7)), _ptr(np.zeros(7))) == 0
+    for N, solve in ((7, shim.sc_solve7), (6, shim.sc_solve6)):
+        for _ in range(50):
+            A = rng.normal(size=(12, N))
+            H = A.T @ A
+            b = rng.normal(size=N)
+            lam = 10.0 ** rng.uniform(-6, 1)
+            packed = np.array([H[i, j] for i in range(N) for j in range(i, N)])
+            x = np.zeros(N)
+            assert solve(_ptr(packed), C.c_double(lam), _ptr(b), _ptr(x)) == 1
+            ref = np.linalg.solve(H + lam * np.eye(N), b)
+            assert np.abs(x - ref).max() <= 1e-9 * max(1.0, np.abs(ref).max())
+        neg = np.zeros(N * (N + 1) // 2); neg[0] = -1.0
+        assert solve(_ptr(neg), C.c_double(0.0), _ptr(np.zeros(N)), _ptr(np.zeros(N))) == 0
 
 
 def test_class_layer_program_compiles_and_fails_loudly_without_gpu(tmp_path):
