@@ -11,13 +11,14 @@
 // A sorted (distance, index) top-4 is what the reference's sequential `<` scan needs: best =
 // lowest index among the minimum distances, second best = next key.  robust::brute_force_match
 // also removes already-matched frame keypoints from later scans (a sequential dependency); the
-// host replays that greedy rule on the top-4 lists and re-queries the GPU (with an exclusion
-// bitmask) only when a list is exhausted -- see ovs_robust_brute_force_match_host.
+// host replays that greedy rule on the top-8 lists (greedy_replay.h) and re-queries the GPU (with an
+// exclusion bitmask) only when a list cannot decide -- see ovs_robust_brute_force_match_host.
 #include <algorithm>
 #include <cstring>
 #include <new>
 #include <vector>
 
+#include "greedy_replay.h"
 #include "match_common.h"
 
 namespace {
@@ -176,7 +177,7 @@ int launch_topk(ovs_matcher* h, const uint8_t* d_q, int nq, const uint8_t* d_t, 
     return OVS_OK;
 }
 
-inline int key_dist(unsigned key) { return key == 0xffffffffu ? OVS_MAX_HAMMING_DIST : (int)(key >> 16); }
+using ovs::key_dist;
 inline int key_idx(unsigned key) { return key == 0xffffffffu ? -1 : (int)(key & 0xffffu); }
 
 }  // namespace
@@ -300,63 +301,36 @@ int robust_replay(ovs_matcher* h, const uint8_t* d_query, const uint8_t* d_train
                   int32_t* pairs_out, int capacity, int* num_matches) {
     int rc;
     std::vector<unsigned> claimed((size_t)(n1 + 31) / 32, 0u);
-    auto is_claimed = [&](int i) { return (claimed[i >> 5] >> (i & 31)) & 1u; };
-    // A frame keypoint farther than d_star can neither be an acceptable best (> HAMMING_DIST_THR_LOW) nor
-    // make the ratio test fail (lowe_ratio * d_star >= THR_LOW >= best): a list that reaches d_star is
-    // complete for every decision the reference takes.
-    int d_star = OVS_HAMMING_DIST_THR_LOW + 1;
-    while (d_star < OVS_MAX_HAMMING_DIST && lowe_ratio * (float)(unsigned)d_star < (float)OVS_HAMMING_DIST_THR_LOW) ++d_star;
-    ++d_star;
+    const auto unclaimed = [&](int i, int) { return !((claimed[i >> 5] >> (i & 31)) & 1u); };
+    const auto ratio = [&](const ovs::ReplayList<kTopK>& L, int second, ovs::Second) { return !(lowe_ratio * (float)(unsigned)second < (float)L.dist[0]); };
+    const int complete_at = ovs::d_star(lowe_ratio);
     int nm = 0;
     for (int q = 0; q < n2; ++q) {
         if (lm_valid_2 && !lm_valid_2[q]) continue;
-        unsigned keys[kTopK];
-        memcpy(keys, h->h_keys + (size_t)q * kTopK, sizeof(keys));
-        for (int attempt = 0; attempt < 2; ++attempt) {
-            // remaining (unclaimed) entries of the list, in (distance, index) order
-            int rem[kTopK], r = 0;
-            bool exhausted = false;  // list ends with sentinels: nothing exists beyond it
-            for (int k = 0; k < kTopK; ++k) {
-                if (keys[k] == 0xffffffffu) { exhausted = true; break; }
-                if (!is_claimed(key_idx(keys[k]))) rem[r++] = k;
-            }
-            const int lb = exhausted ? OVS_MAX_HAMMING_DIST : key_dist(keys[kTopK - 1]);  // unlisted entries are >= this
-            const bool complete = exhausted || lb >= d_star || attempt == 1;
-            int best = OVS_MAX_HAMMING_DIST, best_i = -1, second = OVS_MAX_HAMMING_DIST;
-            bool decided = true;
-            if (r >= 2 || complete) {
-                if (r >= 1) { best = key_dist(keys[rem[0]]); best_i = key_idx(keys[rem[0]]); }
-                if (r >= 2) second = key_dist(keys[rem[1]]);
-            } else if (r == 1) {
-                best = key_dist(keys[rem[0]]); best_i = key_idx(keys[rem[0]]);
-                if (best <= OVS_HAMMING_DIST_THR_LOW && lowe_ratio * (float)(unsigned)lb < (float)best) decided = false;  // needs the true second best
-                second = lb;  // only used when the ratio test passes already with the lower bound
-            } else {  // r == 0
-                if (lb <= OVS_HAMMING_DIST_THR_LOW) decided = false;
-            }
-            if (!decided) {
-                // re-query this keyframe descriptor on the GPU against the unclaimed frame descriptors
-                if ((rc = grow_dev(&h->d_mask, &h->d_mask_cap, claimed.size())) != OVS_OK) return rc;
-                OVS_CUDA_CHECK(cudaMemcpyAsync(h->d_mask, claimed.data(), claimed.size() * sizeof(unsigned), cudaMemcpyHostToDevice, h->stream));
-                unsigned* d_slot = h->d_keys + (size_t)n2 * kTopK;
-                unsigned* h_slot = h->h_keys + (size_t)n2 * kTopK;
-                k_hamming_one<<<1, 256, 0, h->stream>>>(reinterpret_cast<const uint4*>(d_query + (size_t)q * 32), reinterpret_cast<const uint4*>(d_train), n1,
-                                                        h->d_mask, d_slot);
-                OVS_LAUNCH_CHECK();
-                OVS_CUDA_CHECK(cudaMemcpyAsync(h_slot, d_slot, kTopK * sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
-                OVS_CUDA_CHECK(ovs::sync_stream(h->stream));
-                memcpy(keys, h_slot, sizeof(keys));
-                ++h->num_requeries;
-                continue;
-            }
-            if (OVS_HAMMING_DIST_THR_LOW < best) break;
-            if (lowe_ratio * (float)(unsigned)second < (float)best) break;
-            OVS_REQUIRE(nm < capacity, OVS_ERR_CAPACITY, "pairs_out capacity %d too small", capacity);
-            pairs_out[2 * nm] = best_i; pairs_out[2 * nm + 1] = q;
-            claimed[best_i >> 5] |= 1u << (best_i & 31);
-            ++nm;
-            break;
-        }
+        // re-query this keyframe descriptor on the GPU against the unclaimed frame descriptors, into the spare row n2
+        const auto requery = [&](unsigned* fresh) -> int {
+            const int rc2 = grow_dev(&h->d_mask, &h->d_mask_cap, claimed.size());
+            if (rc2 != OVS_OK) return rc2;
+            OVS_CUDA_CHECK(cudaMemcpyAsync(h->d_mask, claimed.data(), claimed.size() * sizeof(unsigned), cudaMemcpyHostToDevice, h->stream));
+            unsigned* d_slot = h->d_keys + (size_t)n2 * kTopK;
+            unsigned* h_slot = h->h_keys + (size_t)n2 * kTopK;
+            k_hamming_one<<<1, 256, 0, h->stream>>>(reinterpret_cast<const uint4*>(d_query + (size_t)q * 32), reinterpret_cast<const uint4*>(d_train), n1,
+                                                    h->d_mask, d_slot);
+            OVS_LAUNCH_CHECK();
+            OVS_CUDA_CHECK(cudaMemcpyAsync(h_slot, d_slot, kTopK * sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
+            OVS_CUDA_CHECK(ovs::sync_stream(h->stream));
+            memcpy(fresh, h_slot, kTopK * sizeof(unsigned));
+            ++h->num_requeries;
+            return OVS_OK;
+        };
+        ovs::ReplayPick p;
+        rc = ovs::replay_query<kTopK>(h->h_keys + (size_t)q * kTopK, OVS_HAMMING_DIST_THR_LOW, complete_at, key_idx, unclaimed, ratio, requery, &p);
+        if (rc != OVS_OK) return rc;
+        if (p.id < 0) continue;
+        OVS_REQUIRE(nm < capacity, OVS_ERR_CAPACITY, "pairs_out capacity %d too small", capacity);
+        pairs_out[2 * nm] = p.id; pairs_out[2 * nm + 1] = q;
+        claimed[p.id >> 5] |= 1u << (p.id & 31);
+        ++nm;
     }
     *num_matches = nm;
     return OVS_OK;

@@ -16,8 +16,8 @@
 // k_stereo_subpixel one warp per left keypoint: 11 SAD windows (11 x 11, centre-normalised) on the
 //                   extractor's device pyramids, warp-reduced with __reduce_add_sync, parabola fit.
 //
-// The sequential parts of the reference (greedy "a keypoint is matched once" bookkeeping, the angle
-// histogram, the median test of stereo) run on the host over these results.
+// The sequential parts of the reference (greedy "a keypoint is matched once" bookkeeping and the angle histogram,
+// greedy_replay.h; the median test of stereo) run on the host over these results.
 #include <algorithm>
 #include <cmath>
 #include <cstdint>
@@ -25,6 +25,7 @@
 #include <new>
 #include <vector>
 
+#include "greedy_replay.h"
 #include "match_common.h"
 #include "two_view_triangulate.h"
 
@@ -59,6 +60,34 @@ __device__ __forceinline__ void topk_insert(unsigned (&k)[kTopK], unsigned key) 
 
 __device__ __forceinline__ int cv_floor_f(float v) { return __float2int_rd(v); }
 __device__ __forceinline__ int cv_ceil_f(float v) { return __float2int_ru(v); }
+
+// match::compute_descriptor_distance_32 by eight population counts
+__device__ __forceinline__ int hamming256(const uint4& qa, const uint4& qb, const uint4& ta, const uint4& tb) {
+    return __popc(qa.x ^ ta.x) + __popc(qa.y ^ ta.y) + __popc(qa.z ^ ta.z) + __popc(qa.w ^ ta.w)
+           + __popc(qb.x ^ tb.x) + __popc(qb.y ^ tb.y) + __popc(qb.z ^ tb.z) + __popc(qb.w ^ tb.w);
+}
+
+// One chunk of a warp's running top-K (k_triangulation_topk, k_node_topk): lane r < K carries entry r in `extra`, every lane
+// holds up to K keys of the chunk in mine[]; returns lane r's entry r of the K smallest keys of both.  Keys are unique (they
+// carry the candidate's rank).
+template <int K>
+__device__ __forceinline__ unsigned warp_merge_topk(unsigned extra, unsigned (&mine)[K], int lane) {
+    unsigned next_extra = 0xffffffffu;
+#pragma unroll
+    for (int r = 0; r < K; ++r) {
+        unsigned lmin = extra;
+#pragma unroll
+        for (int k = 0; k < K; ++k) lmin = min(lmin, mine[k]);
+        const unsigned wmin = __reduce_min_sync(0xffffffffu, lmin);
+        if (wmin != 0xffffffffu) {
+            if (extra == wmin) extra = 0xffffffffu;
+#pragma unroll
+            for (int k = 0; k < K; ++k) if (mine[k] == wmin) mine[k] = 0xffffffffu;
+        }
+        if (lane == r) next_extra = wmin;
+    }
+    return next_extra;
+}
 
 struct WindowFrame {
     float min_x, min_y, inv_w, inv_h;
@@ -122,8 +151,7 @@ __global__ void __launch_bounds__(128) k_window_topk(WindowFrame F, WindowQuerie
                     }
                 }
                 const uint4 ta = __ldg(F.desc + 2 * (size_t)r), tb = __ldg(F.desc + 2 * (size_t)r + 1);
-                const int d = __popc(qa.x ^ ta.x) + __popc(qa.y ^ ta.y) + __popc(qa.z ^ ta.z) + __popc(qa.w ^ ta.w)
-                              + __popc(qb.x ^ tb.x) + __popc(qb.y ^ tb.y) + __popc(qb.z ^ tb.z) + __popc(qb.w ^ tb.w);
+                const int d = hamming256(qa, qb, ta, tb);
                 if (F.cap && !(d < (int)F.cap[r])) continue;
                 topk_insert(best, ((unsigned)d << 16) | (unsigned)r);
             }
@@ -183,8 +211,7 @@ __global__ void __launch_bounds__(128) k_stereo_match(StereoArgs A, unsigned* __
             const float xr = s_rx[j];
             if (xr < min_x_right || max_x_right < xr) continue;
             const uint4 ta = s_desc[2 * j], tb = s_desc[2 * j + 1];
-            const int d = __popc(qa.x ^ ta.x) + __popc(qa.y ^ ta.y) + __popc(qa.z ^ ta.z) + __popc(qa.w ^ ta.w)
-                          + __popc(qb.x ^ tb.x) + __popc(qb.y ^ tb.y) + __popc(qb.z ^ tb.z) + __popc(qb.w ^ tb.w);
+            const int d = hamming256(qa, qb, ta, tb);
             const unsigned key = ((unsigned)d << 16) | (unsigned)(t0 + j);
             if ((key >> 16) < (best >> 16)) best = key;   // strict '<' on the distance: first (lowest index) wins ties
         }
@@ -263,7 +290,7 @@ __global__ void __launch_bounds__(128) k_stereo_subpixel(StereoArgs A, const uns
     if (lane == 0) { x_right_out[il] = xr_res; depth_out[il] = depth_res; corr_out[il] = corr_res; }
 }
 
-inline int key_dist(unsigned key) { return key == 0xffffffffu ? OVS_MAX_HAMMING_DIST : (int)(key >> 16); }
+using ovs::key_dist;
 inline int key_rank(unsigned key) { return key == 0xffffffffu ? -1 : (int)(key & 0xffffu); }
 
 // data::get_cell_indices
@@ -274,10 +301,10 @@ inline bool cell_of(const ovs_grid& g, float x, float y, int* cx, int* cy) {
 }
 
 // Runs k_window_topk for nq host queries; keys land in m->h_keys[0 .. nq*4).  `cap` (rank order, n
-// entries) or nullptr.
-int window_topk(ovs_frame_index* f, int nq, const float* ref_xy, const float* margin, const int* min_level, const int* max_level,
-                const float* xr_q, const uint8_t* qdesc, const unsigned short* cap_rank_order, const float* fuse_inv_sigma_sq = nullptr,
-                int fuse_levels = 0) {
+// entries) or nullptr.  use_xr: the keypoints' x_right take part (the x_right test, or the fuse gate's x_right term).
+int window_topk(const ovs_frame_index* f, bool use_xr, int nq, const float* ref_xy, const float* margin, const int* min_level,
+                const int* max_level, const float* xr_q, const uint8_t* qdesc, const unsigned short* cap_rank_order,
+                const float* fuse_inv_sigma_sq = nullptr, int fuse_levels = 0) {
     ovs_matcher* m = f->m;
     cudaStream_t st = m->stream;
     const size_t N = (size_t)nq;
@@ -299,7 +326,7 @@ int window_topk(ovs_frame_index* f, int nq, const float* ref_xy, const float* ma
     WindowFrame F;
     F.min_x = f->grid.min_x; F.min_y = f->grid.min_y; F.inv_w = f->grid.inv_cell_width; F.inv_h = f->grid.inv_cell_height;
     F.cols = f->grid.num_grid_cols; F.rows = f->grid.num_grid_rows;
-    F.x = f->d_x; F.y = f->d_y; F.xr = f->has_xr ? f->d_xr : nullptr; F.oct = f->d_oct; F.desc = f->d_desc;
+    F.x = f->d_x; F.y = f->d_y; F.xr = use_xr ? f->d_xr : nullptr; F.oct = f->d_oct; F.desc = f->d_desc;
     F.cell_start = f->d_cell_start; F.cap = cap_rank_order ? f->d_cap : nullptr;
     Q.nq = nq; Q.xr = xr_q ? dxr : nullptr;
     Q.fuse_gate = fuse_inv_sigma_sq ? 1 : 0;
@@ -315,33 +342,13 @@ int window_topk(ovs_frame_index* f, int nq, const float* ref_xy, const float* ma
     return OVS_OK;
 }
 
-// Greedy replay helper: the unclaimed/valid entries of a query's sorted key list.
-struct Resolved {
-    int r = 0;               // valid entries found in the list
-    int dist[kTopK], idx[kTopK];
-    bool exhausted = false;  // the list ended before 4 entries: nothing exists beyond it
-    int lower_bound = OVS_MAX_HAMMING_DIST;  // every unlisted candidate has distance >= this
-};
-
-template <typename Valid>
-Resolved resolve(const ovs_frame_index* f, const unsigned* keys, Valid valid) {
-    Resolved R;
-    for (int k = 0; k < kTopK; ++k) {
-        if (keys[k] == 0xffffffffu) { R.exhausted = true; break; }
-        const int idx = f->rank_to_idx[key_rank(keys[k])], d = key_dist(keys[k]);
-        if (valid(idx, d)) { R.dist[R.r] = d; R.idx[R.r] = idx; ++R.r; }
-    }
-    R.lower_bound = R.exhausted ? OVS_MAX_HAMMING_DIST : key_dist(keys[kTopK - 1]);
-    return R;
-}
-
 // Re-runs one query with a distance cap per keypoint (cap[idx]: candidate valid iff d < cap[idx]).
-int requery(ovs_frame_index* f, const float* ref_xy, float margin, int min_level, int max_level, const float* xr_q,
+int requery(const ovs_frame_index* f, bool use_xr, const float* ref_xy, float margin, int min_level, int max_level, const float* xr_q,
             const uint8_t* qdesc, const std::vector<unsigned short>& cap_by_idx, unsigned* keys_out) {
     ++f->m->num_requeries;
     std::vector<unsigned short> cap((size_t)std::max(f->nranked, 1));
     for (int r = 0; r < f->nranked; ++r) cap[r] = cap_by_idx[f->rank_to_idx[r]];
-    int rc = window_topk(f, 1, ref_xy, &margin, &min_level, &max_level, xr_q, qdesc, cap.data());
+    int rc = window_topk(f, use_xr, 1, ref_xy, &margin, &min_level, &max_level, xr_q, qdesc, cap.data());
     if (rc != OVS_OK) return rc;
     memcpy(keys_out, f->m->h_keys, kTopK * sizeof(unsigned));
     return OVS_OK;
@@ -530,7 +537,7 @@ extern "C" int ovs_match_window_topk_host(ovs_frame_index* f, int nq, const floa
     OVS_REQUIRE(f && nq >= 0 && (nq == 0 || (ref_xy && margin && min_level && max_level && qdesc && idx_out && dist_out)), OVS_ERR_INVALID_ARG, "bad argument");
     if (nq == 0) return OVS_OK;
     OVS_CUDA_CHECK(cudaSetDevice(f->m->device));
-    int rc = window_topk(f, nq, ref_xy, margin, min_level, max_level, x_right_q, qdesc, nullptr);
+    int rc = window_topk(f, f->has_xr, nq, ref_xy, margin, min_level, max_level, x_right_q, qdesc, nullptr);
     if (rc != OVS_OK) return rc;
     for (size_t i = 0; i < (size_t)nq * kTopK; ++i) {
         const unsigned k = f->m->h_keys[i];
@@ -567,7 +574,7 @@ extern "C" int ovs_projection_match_keyframes_mutually_host(ovs_frame_index* f1,
             lo[q] = l - 1; hi[q] = l;
             if (usable && !usable[q]) { lo[q] = 1; hi[q] = 0; }   // empty level range: no candidates
         }
-        const int rc = window_topk(dst, nq, reproj, mg.data(), lo.data(), hi.data(), nullptr, desc, nullptr);
+        const int rc = window_topk(dst, dst->has_xr, nq, reproj, mg.data(), lo.data(), hi.data(), nullptr, desc, nullptr);
         if (rc != OVS_OK) return rc;
         best.assign(nq, -1);
         for (int q = 0; q < nq; ++q) {
@@ -628,40 +635,29 @@ extern "C" int ovs_projection_match_frame_and_landmarks_host(ovs_frame_index* f,
     {
         std::vector<unsigned short> cap_rank((size_t)std::max(f->nranked, 1));
         for (int r = 0; r < f->nranked; ++r) cap_rank[r] = cap[f->rank_to_idx[r]];
-        rc = window_topk(f, nq, ref.data(), mg.data(), lo.data(), hi.data(), f->has_xr ? xr.data() : nullptr, qd.data(), cap_rank.data());
+        rc = window_topk(f, f->has_xr, nq, ref.data(), mg.data(), lo.data(), hi.data(), f->has_xr ? xr.data() : nullptr, qd.data(), cap_rank.data());
         if (rc != OVS_OK) return rc;
     }
-    std::vector<unsigned> keys(f->m->h_keys, f->m->h_keys + (size_t)nq * kTopK);
+    std::vector<unsigned> keys(f->m->h_keys, f->m->h_keys + (size_t)nq * kTopK);   // a re-query overwrites h_keys
+    const auto decode = [&](unsigned key) { return f->rank_to_idx[key_rank(key)]; };
+    const auto available = [&](int idx, int) { return cap[idx] != 0; };
+    // the reference's ratio test applies only when the best and the second best share a level; against a lower bound it
+    // always applies (only the true second could pass it)
+    const auto ratio = [&](const ovs::ReplayList<kTopK>& L, int second, ovs::Second kind) {
+        if (kind == ovs::Second::bound) return !((float)L.dist[0] > lowe_ratio * (float)second);
+        const int second_level = kind == ovs::Second::listed ? f->hoct[L.id[1]] : -1;
+        return !(f->hoct[L.id[0]] == second_level && (float)L.dist[0] > lowe_ratio * (float)second);
+    };
     int nm = 0;
     for (int q = 0; q < nq; ++q) {
-        unsigned kq[kTopK];
-        memcpy(kq, &keys[(size_t)q * kTopK], sizeof(kq));
-        for (int attempt = 0; attempt < 2; ++attempt) {
-            const Resolved R = resolve(f, kq, [&](int idx, int) { return cap[idx] != 0; });
-            bool decided = true, accept = false;
-            int best_idx = -1;
-            if (R.r >= 2 || R.exhausted || attempt == 1) {
-                if (R.r >= 1 && R.dist[0] <= OVS_HAMMING_DIST_THR_HIGH) {
-                    best_idx = R.idx[0];
-                    const int second = R.r >= 2 ? R.dist[1] : OVS_MAX_HAMMING_DIST;
-                    const int best_level = f->hoct[R.idx[0]], second_level = R.r >= 2 ? f->hoct[R.idx[1]] : -1;
-                    accept = !(best_level == second_level && (float)R.dist[0] > lowe_ratio * (float)second);
-                }
-            } else if (R.r == 1) {
-                if (R.dist[0] <= OVS_HAMMING_DIST_THR_HIGH) {
-                    best_idx = R.idx[0];
-                    if ((float)R.dist[0] > lowe_ratio * (float)R.lower_bound) decided = false;   // the ratio test needs the true second best
-                    else accept = true;
-                }
-            } else if (R.lower_bound <= OVS_HAMMING_DIST_THR_HIGH) decided = false;
-            if (!decided) {
-                rc = requery(f, &ref[2 * q], mg[q], lo[q], hi[q], f->has_xr ? &xr[q] : nullptr, &qd[32 * (size_t)q], cap, kq);
-                if (rc != OVS_OK) return rc;
-                continue;
-            }
-            if (accept) { matched_lm_of_kp[best_idx] = qlm[q]; cap[best_idx] = 0; ++nm; }
-            break;
-        }
+        const auto requery_q = [&](unsigned* fresh) {
+            return requery(f, f->has_xr, &ref[2 * q], mg[q], lo[q], hi[q], f->has_xr ? &xr[q] : nullptr, &qd[32 * (size_t)q], cap, fresh);
+        };
+        ovs::ReplayPick p;
+        rc = ovs::replay_query<kTopK>(&keys[(size_t)q * kTopK], OVS_HAMMING_DIST_THR_HIGH, ovs::kNeverComplete, decode, available, ratio,
+                                      requery_q, &p);
+        if (rc != OVS_OK) return rc;
+        if (p.id >= 0) { matched_lm_of_kp[p.id] = qlm[q]; cap[p.id] = 0; ++nm; }
     }
     *num_matches = nm;
     return OVS_OK;
@@ -701,7 +697,7 @@ extern "C" int ovs_fuse_best_keypoints_host(ovs_frame_index* f, int nq, const ui
         xr[k] = reproj_x_right ? reproj_x_right[q] : -1.0f;
         memcpy(&qd[32 * (size_t)k], lm_desc + 32 * (size_t)q, 32);
     }
-    const int rc = window_topk(f, nu, ref.data(), mg.data(), lo.data(), hi.data(), reproj_x_right ? xr.data() : nullptr, qd.data(), nullptr,
+    const int rc = window_topk(f, f->has_xr, nu, ref.data(), mg.data(), lo.data(), hi.data(), reproj_x_right ? xr.data() : nullptr, qd.data(), nullptr,
                                inv_level_sigma_sq, num_scale_levels);
     if (rc != OVS_OK) return rc;
     int num = 0;
@@ -712,32 +708,6 @@ extern "C" int ovs_fuse_best_keypoints_host(ovs_frame_index* f, int nq, const ui
     *num_matches = num;
     return OVS_OK;
 }
-
-namespace {
-// match::angle_checker<int>(30, 3)::get_invalid_matches over (delta_angle, tag) pairs
-void angle_checker_invalid(const std::vector<float>& deltas, std::vector<uint8_t>& invalid) {
-    const int H = 30, keepn = 3;
-    const float inv_len = 1.0f / H;
-    std::vector<int> bin(deltas.size()), count(H, 0), order(H);
-    for (size_t i = 0; i < deltas.size(); ++i) {
-        float d = deltas[i];
-        if (d < 0.0) d += 360.0;
-        if (360.0 <= d) d -= 360.0;
-        bin[i] = (int)((unsigned)lrintf(d * inv_len) % (unsigned)H);
-        count[bin[i]]++;
-    }
-    for (int b = 0; b < H; ++b) order[b] = b;
-    std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return count[a] > count[b]; });
-    std::vector<uint8_t> keep(H, 0);
-    const int top = count[order[0]];
-    for (int r = 0; r < keepn; ++r) {
-        if (r > 0 && (float)count[order[r]] < 0.1f * (float)top) break;
-        keep[order[r]] = 1;
-    }
-    invalid.resize(deltas.size());
-    for (size_t i = 0; i < deltas.size(); ++i) invalid[i] = !keep[bin[i]];
-}
-}  // namespace
 
 // The loop shared by projection::match_current_and_last_frames, match_frame_and_keyframe,
 // match_by_Sim3_transform and each direction of match_keyframes_mutually (match/projection.cc): for
@@ -776,41 +746,27 @@ extern "C" int ovs_projection_match_best_host(ovs_frame_index* f, int nq, const 
         std::vector<unsigned short> cap_rank((size_t)std::max(f->nranked, 1));
         for (int r = 0; r < f->nranked; ++r) cap_rank[r] = cap[f->rank_to_idx[r]];
         // without reprojected x_right the x_right test of the reference is not part of this matcher
-        const bool saved = f->has_xr;
-        f->has_xr = use_xr;
-        rc = window_topk(f, nu, ref.data(), mg.data(), lo.data(), hi.data(), use_xr ? xr.data() : nullptr, qd.data(), cap_rank.data());
-        f->has_xr = saved;
+        rc = window_topk(f, use_xr, nu, ref.data(), mg.data(), lo.data(), hi.data(), use_xr ? xr.data() : nullptr, qd.data(), cap_rank.data());
         if (rc != OVS_OK) return rc;
     }
-    std::vector<unsigned> keys(f->m->h_keys, f->m->h_keys + (size_t)nu * kTopK);
+    std::vector<unsigned> keys(f->m->h_keys, f->m->h_keys + (size_t)nu * kTopK);   // a re-query overwrites h_keys
+    const auto decode = [&](unsigned key) { return f->rank_to_idx[key_rank(key)]; };
+    const auto available = [&](int idx, int) { return cap[idx] != 0; };
     int nm = 0;
-    std::vector<float> deltas; std::vector<int> delta_kp;
+    ovs::OrientationCheck orientation;
     for (int q = 0; q < nu; ++q) {
-        unsigned kq[kTopK];
-        memcpy(kq, &keys[(size_t)q * kTopK], sizeof(kq));
-        for (int attempt = 0; attempt < 2; ++attempt) {
-            const Resolved R = resolve(f, kq, [&](int idx, int) { return cap[idx] != 0; });
-            if (R.r == 0 && !R.exhausted && attempt == 0 && R.lower_bound <= (int)hamm_dist_thr) {
-                const bool saved = f->has_xr;
-                f->has_xr = use_xr;
-                rc = requery(f, &ref[2 * q], mg[q], lo[q], hi[q], use_xr ? &xr[q] : nullptr, &qd[32 * (size_t)q], cap, kq);
-                f->has_xr = saved;
-                if (rc != OVS_OK) return rc;
-                continue;
-            }
-            if (R.r >= 1 && !((int)hamm_dist_thr < R.dist[0])) {
-                const int best_idx = R.idx[0];
-                matched_query_of_kp[best_idx] = ql[q]; cap[best_idx] = 0; ++nm;
-                if (check_orientation) { deltas.push_back(q_angle[ql[q]] - f->hangle[best_idx]); delta_kp.push_back(best_idx); }
-            }
-            break;
-        }
+        const auto requery_q = [&](unsigned* fresh) {
+            return requery(f, use_xr, &ref[2 * q], mg[q], lo[q], hi[q], use_xr ? &xr[q] : nullptr, &qd[32 * (size_t)q], cap, fresh);
+        };
+        ovs::ReplayPick p;
+        rc = ovs::replay_query<kTopK>(&keys[(size_t)q * kTopK], (int)hamm_dist_thr, ovs::kNeverComplete, decode, available, ovs::no_ratio_test,
+                                      requery_q, &p);
+        if (rc != OVS_OK) return rc;
+        if (p.id < 0) continue;
+        matched_query_of_kp[p.id] = ql[q]; cap[p.id] = 0; ++nm;
+        if (check_orientation) orientation.add(q_angle[ql[q]] - f->hangle[p.id], p.id);
     }
-    if (check_orientation && !deltas.empty()) {
-        std::vector<uint8_t> invalid;
-        angle_checker_invalid(deltas, invalid);
-        for (size_t k = 0; k < deltas.size(); ++k) if (invalid[k]) { matched_query_of_kp[delta_kp[k]] = -1; --nm; }
-    }
+    orientation.unset_invalid([&](int kp) { matched_query_of_kp[kp] = -1; --nm; });
     *num_matches = nm;
     return OVS_OK;
 }
@@ -847,7 +803,7 @@ extern "C" int ovs_area_match_in_consistent_area_host(ovs_frame_index* f2, int n
     OVS_REQUIRE(f2 && num_matches && n1 >= 0 && (n1 == 0 || (octave_1 && desc_1 && prev_matched_xy && matched_idx_2_in_1)), OVS_ERR_INVALID_ARG, "bad argument");
     OVS_REQUIRE(!check_orientation || angle_1 || n1 == 0, OVS_ERR_INVALID_ARG, "angles required for the orientation check");
     OVS_CUDA_CHECK(cudaSetDevice(f2->m->device));
-    ovs_frame_index* f = f2;
+    const ovs_frame_index* f = f2;
     const int n2 = f->n;
     for (int i = 0; i < n1; ++i) matched_idx_2_in_1[i] = -1;
     *num_matches = 0;
@@ -862,62 +818,38 @@ extern "C" int ovs_area_match_in_consistent_area_host(ovs_frame_index* f2, int n
         lo[q] = octave_1[i]; hi[q] = octave_1[i];
         memcpy(&qd[32 * (size_t)q], desc_1 + 32 * (size_t)i, 32);
     }
-    // the area matcher has no x_right test: a stereo frame's index searches here as a monocular one (restored on return)
-    struct NoXr {
-        ovs_frame_index* f; bool saved;
-        ~NoXr() { f->has_xr = saved; }
-    } no_xr{f, f->has_xr};
-    f->has_xr = false;
-    int rc = window_topk(f, nq, ref.data(), mg.data(), lo.data(), hi.data(), nullptr, qd.data(), nullptr);
+    // the area matcher has no x_right test: a stereo frame's index searches here as a monocular one
+    int rc = window_topk(f, false, nq, ref.data(), mg.data(), lo.data(), hi.data(), nullptr, qd.data(), nullptr);
     if (rc != OVS_OK) return rc;
-    std::vector<unsigned> keys(f->m->h_keys, f->m->h_keys + (size_t)nq * kTopK);
+    std::vector<unsigned> keys(f->m->h_keys, f->m->h_keys + (size_t)nq * kTopK);   // a re-query overwrites h_keys
     // matched_dists_in_frm_2 doubles as the per-keypoint distance cap (candidate valid iff d < cap)
     std::vector<unsigned short> cap(std::max(n2, 1), (unsigned short)OVS_MAX_HAMMING_DIST);
     std::vector<int> matched_idx_1_in_2(std::max(n2, 1), -1);
-    std::vector<float> deltas; std::vector<int> delta_idx;
+    const auto decode = [&](unsigned key) { return f->rank_to_idx[key_rank(key)]; };
+    const auto closer = [&](int idx, int d) { return d < (int)cap[idx]; };
+    const auto ratio = [&](const ovs::ReplayList<kTopK>& L, int second, ovs::Second) { return !((float)second * lowe_ratio < (float)L.dist[0]); };
+    ovs::OrientationCheck orientation;
     int nm = 0;
     for (int q = 0; q < nq; ++q) {
         const int idx_1 = q1[q];
-        unsigned kq[kTopK];
-        memcpy(kq, &keys[(size_t)q * kTopK], sizeof(kq));
-        for (int attempt = 0; attempt < 2; ++attempt) {
-            const Resolved R = resolve(f, kq, [&](int idx, int d) { return d < (int)cap[idx]; });
-            bool decided = true, accept = false;
-            if (R.r >= 2 || R.exhausted || attempt == 1) {
-                if (R.r >= 1 && !(OVS_HAMMING_DIST_THR_LOW < R.dist[0])) {
-                    const int second = R.r >= 2 ? R.dist[1] : OVS_MAX_HAMMING_DIST;
-                    accept = !((float)second * lowe_ratio < (float)R.dist[0]);
-                }
-            } else if (R.r == 1) {
-                if (!(OVS_HAMMING_DIST_THR_LOW < R.dist[0])) {
-                    if ((float)R.lower_bound * lowe_ratio < (float)R.dist[0]) decided = false;
-                    else accept = true;
-                }
-            } else if (R.lower_bound <= OVS_HAMMING_DIST_THR_LOW) decided = false;
-            if (!decided) {
-                rc = requery(f, &ref[2 * q], mg[q], lo[q], hi[q], nullptr, &qd[32 * (size_t)q], cap, kq);
-                if (rc != OVS_OK) return rc;
-                continue;
-            }
-            if (accept) {
-                const int best_idx_2 = R.idx[0];
-                const int prev_idx_1 = matched_idx_1_in_2[best_idx_2];
-                if (0 <= prev_idx_1) { matched_idx_2_in_1[prev_idx_1] = -1; --nm; }
-                matched_idx_2_in_1[idx_1] = best_idx_2;
-                matched_idx_1_in_2[best_idx_2] = idx_1;
-                cap[best_idx_2] = (unsigned short)R.dist[0];
-                ++nm;
-                if (check_orientation) { deltas.push_back(angle_1[idx_1] - f->hangle[best_idx_2]); delta_idx.push_back(idx_1); }
-            }
-            break;
-        }
+        const auto requery_q = [&](unsigned* fresh) {
+            return requery(f, false, &ref[2 * q], mg[q], lo[q], hi[q], nullptr, &qd[32 * (size_t)q], cap, fresh);
+        };
+        ovs::ReplayPick p;
+        rc = ovs::replay_query<kTopK>(&keys[(size_t)q * kTopK], OVS_HAMMING_DIST_THR_LOW, ovs::kNeverComplete, decode, closer, ratio, requery_q, &p);
+        if (rc != OVS_OK) return rc;
+        if (p.id < 0) continue;
+        const int prev_idx_1 = matched_idx_1_in_2[p.id];
+        if (0 <= prev_idx_1) { matched_idx_2_in_1[prev_idx_1] = -1; --nm; }
+        matched_idx_2_in_1[idx_1] = p.id;
+        matched_idx_1_in_2[p.id] = idx_1;
+        cap[p.id] = (unsigned short)p.dist;
+        ++nm;
+        if (check_orientation) orientation.add(angle_1[idx_1] - f->hangle[p.id], idx_1);
     }
-    if (check_orientation && !deltas.empty()) {
-        std::vector<uint8_t> invalid;
-        angle_checker_invalid(deltas, invalid);
-        for (size_t k = 0; k < deltas.size(); ++k)
-            if (invalid[k] && 0 <= matched_idx_2_in_1[delta_idx[k]]) { matched_idx_2_in_1[delta_idx[k]] = -1; --nm; }
-    }
+    orientation.unset_invalid([&](int i1) {
+        if (0 <= matched_idx_2_in_1[i1]) { matched_idx_2_in_1[i1] = -1; --nm; }
+    });
     for (int i = 0; i < n1; ++i)
         if (0 <= matched_idx_2_in_1[i]) { prev_matched_xy[2 * i] = f->hx[matched_idx_2_in_1[i]]; prev_matched_xy[2 * i + 1] = f->hy[matched_idx_2_in_1[i]]; }
     *num_matches = nm;
@@ -1087,8 +1019,7 @@ __global__ void __launch_bounds__(128) k_triangulation_topk(TriArgs A, unsigned*
             const int c = c0 + k * 32 + lane;
             if (c < seg.y && !(taken && taken[c])) {
                 const uint4 ta = tdesc[2 * (size_t)c], tb = tdesc[2 * (size_t)c + 1];
-                const int d = __popc(qa.x ^ ta.x) + __popc(qa.y ^ ta.y) + __popc(qa.z ^ ta.z) + __popc(qa.w ^ ta.w)
-                              + __popc(qb.x ^ tb.x) + __popc(qb.y ^ tb.y) + __popc(qb.z ^ tb.z) + __popc(qb.w ^ tb.w);
+                const int d = hamming256(qa, qb, ta, tb);
                 if (d <= OVS_HAMMING_DIST_THR_LOW) {
                     const double b2x = tbearing[3 * (size_t)c], b2y = tbearing[3 * (size_t)c + 1], b2z = tbearing[3 * (size_t)c + 2];
                     bool ok = true;
@@ -1100,36 +1031,22 @@ __global__ void __launch_bounds__(128) k_triangulation_topk(TriArgs A, unsigned*
                 }
             }
         }
-        // the 8 smallest keys of {this chunk} U {running top-8}; keys are unique (they carry the rank)
-        unsigned next_extra = 0xffffffffu;
-#pragma unroll
-        for (int r = 0; r < kTriK; ++r) {
-            unsigned lmin = extra;
-#pragma unroll
-            for (int k = 0; k < kTriK; ++k) lmin = min(lmin, mine[k]);
-            const unsigned wmin = __reduce_min_sync(0xffffffffu, lmin);
-            if (wmin != 0xffffffffu) {
-                if (extra == wmin) extra = 0xffffffffu;
-#pragma unroll
-                for (int k = 0; k < kTriK; ++k) if (mine[k] == wmin) mine[k] = 0xffffffffu;
-            }
-            if (lane == r) next_extra = wmin;
-        }
-        extra = next_extra;
+        extra = warp_merge_topk(extra, mine, lane);
     }
     if (lane < kTriK) keys_out[(size_t)(q + A.out_shift) * kTriK + lane] = extra;
 }
 
-// The keypoints of a keyframe that take part (no landmark, a vocabulary node), node by node and in index order inside a node:
+// The keypoints of a keyframe that take part (keep(i), a vocabulary node), node by node and in index order inside a node:
 // the reference's walk over the BoW feature vector.
-void tri_order(int n, const uint8_t* has_lm, const int32_t* bow_node, std::vector<int>& out) {
+template <class Keep>
+void node_order(int n, const int32_t* bow_node, Keep&& keep, std::vector<int>& out) {
     out.clear();
-    for (int i = 0; i < n; ++i) if (!has_lm[i] && bow_node[i] >= 0) out.push_back(i);
+    for (int i = 0; i < n; ++i) if (keep(i) && bow_node[i] >= 0) out.push_back(i);
     std::stable_sort(out.begin(), out.end(), [&](int a, int b) { return bow_node[a] < bow_node[b]; });
 }
 
 // seg[k] = the range of rank2 in the node of query q1[k]
-void tri_segments(const std::vector<int>& q1, const int32_t* bow_node_1, const std::vector<int>& rank2, const int32_t* bow_node_2, int2* seg) {
+void node_segments(const std::vector<int>& q1, const int32_t* bow_node_1, const std::vector<int>& rank2, const int32_t* bow_node_2, int2* seg) {
     size_t lo = 0;
     for (size_t k = 0; k < q1.size(); ++k) {
         const int node = bow_node_1[q1[k]];
@@ -1143,45 +1060,34 @@ void tri_segments(const std::vector<int>& q1, const int32_t* bow_node_1, const s
 // The sequential part of match_for_triangulation on one keyframe pair, given each query's candidate list (keys[kTriK k]): the
 // queries k = 0 .. Q - 1 (keyframe-1 keypoint q1[k], in the reference's visiting order; skipped where skip_1[q1[k]] is set, as
 // a keypoint that holds a landmark is no query) each take the first listed candidate not taken yet (taken[rank], all zero on
-// entry); a list of kTriK entries that are all taken may be truncated, so requery(k, &rank) asks the device again with the
-// taken candidates excluded.  Then the orientation histogram, if requested.  matched_idx_2_of_1[n1] (all -1 on entry) gets
-// rank2[rank] of each match; slot_of_1 (may be null) the list entry kTriK k + j it came from, or -1 - k for a re-query.
+// entry).  The device already applied the distance and epipolar tests, so there is no threshold and no ratio test: only a
+// list of kTriK entries that are all taken may be truncated, and then requery(k, keys) asks the device again with the taken
+// candidates excluded (rare: needs 8 earlier keypoints of the same node to have claimed them).  Then the orientation
+// histogram, if requested.  matched_idx_2_of_1[n1] (all -1 on entry) gets rank2[rank] of each match; slot_of_1 (may be null)
+// the list entry kTriK k + j it came from, or -1 - k for a re-query.
 template <class Requery>
-int tri_replay(ovs_matcher* m, int Q, const int* q1, const int* rank2, const unsigned* keys, unsigned char* taken, const uint8_t* skip_1,
+int tri_replay(int Q, const int* q1, const int* rank2, const unsigned* keys, unsigned char* taken, const uint8_t* skip_1,
                const float* angle_1, const float* angle_2, int check_orientation, Requery&& requery, int32_t* matched_idx_2_of_1,
                int32_t* slot_of_1, int* num_matches) {
-    std::vector<float> deltas; std::vector<int> delta_idx;
+    const auto decode = [](unsigned key) { return 0xffff - (int)(key & 0xffffu); };
+    const auto not_taken = [&](int r, int) { return !taken[r]; };
+    ovs::OrientationCheck orientation;
     int num = 0;
     for (int k = 0; k < Q; ++k) {
         const int i1 = q1[k];
         if (skip_1 && skip_1[i1]) continue;
-        const unsigned* lk = keys + (size_t)k * kTriK;
-        int pick = -1, seen = 0, slot = -1;
-        for (int j = 0; j < kTriK && lk[j] != 0xffffffffu; ++j) {
-            ++seen;
-            const int r = 0xffff - (int)(lk[j] & 0xffffu);
-            if (!taken[r]) { pick = r; slot = kTriK * k + j; break; }
-        }
-        if (pick < 0 && seen == kTriK) {
-            // all 8 listed candidates were taken and the list may be truncated (rare: needs 8 earlier keypoints of the same
-            // node to have claimed them).  The replay is sequential, so it waits for the answer.
-            ++m->num_requeries;
-            const int rc = requery(k, &pick);
-            if (rc != OVS_OK) return rc;
-            slot = -1 - k;
-        }
-        if (pick < 0) continue;
-        taken[pick] = 1;
-        matched_idx_2_of_1[i1] = rank2[pick];
-        if (slot_of_1) slot_of_1[i1] = slot;
+        ovs::ReplayPick p;
+        const int rc = ovs::replay_query<kTriK>(keys + (size_t)k * kTriK, OVS_MAX_HAMMING_DIST, ovs::kNeverComplete, decode, not_taken,
+                                                ovs::no_ratio_test, [&](unsigned* fresh) { return requery(k, fresh); }, &p);
+        if (rc != OVS_OK) return rc;
+        if (p.id < 0) continue;
+        taken[p.id] = 1;
+        matched_idx_2_of_1[i1] = rank2[p.id];
+        if (slot_of_1) slot_of_1[i1] = p.requeried ? -1 - k : kTriK * k + p.pos;
         ++num;
-        if (check_orientation) { deltas.push_back(angle_1[i1] - angle_2[rank2[pick]]); delta_idx.push_back(i1); }
+        if (check_orientation) orientation.add(angle_1[i1] - angle_2[rank2[p.id]], i1);
     }
-    if (check_orientation && !deltas.empty()) {
-        std::vector<uint8_t> invalid;
-        angle_checker_invalid(deltas, invalid);
-        for (size_t k = 0; k < deltas.size(); ++k) if (invalid[k]) { matched_idx_2_of_1[delta_idx[k]] = -1; --num; }
-    }
+    orientation.unset_invalid([&](int i1) { matched_idx_2_of_1[i1] = -1; --num; });
     *num_matches = num;
     return OVS_OK;
 }
@@ -1207,12 +1113,12 @@ extern "C" int ovs_robust_match_for_triangulation_host(ovs_matcher* m, int n1, c
     OVS_CUDA_CHECK(cudaSetDevice(m->device));
     // keyframe 2: candidates; keyframe 1: queries in the order the reference visits them
     std::vector<int> rank2, q1;
-    tri_order(n2, has_lm_2, bow_node_2, rank2);
-    tri_order(n1, has_lm_1, bow_node_1, q1);
+    node_order(n2, bow_node_2, [&](int i) { return !has_lm_2[i]; }, rank2);
+    node_order(n1, bow_node_1, [&](int i) { return !has_lm_1[i]; }, q1);
     const int R = (int)rank2.size(), Q = (int)q1.size();
     if (R == 0 || Q == 0) return OVS_OK;
     std::vector<int2> seg(Q);
-    tri_segments(q1, bow_node_1, rank2, bow_node_2, seg.data());
+    node_segments(q1, bow_node_1, rank2, bow_node_2, seg.data());
     const size_t sQ = (size_t)Q, sR = (size_t)R;
     TriArgs A{};
     uint8_t *hqd, *htd, *hq8, *ht8, *taken, *dtaken; double *hqb, *htb; int2* hsg; float* hqs;
@@ -1255,7 +1161,8 @@ extern "C" int ovs_robust_match_for_triangulation_host(ovs_matcher* m, int n1, c
     m->last_kernel_us = ms * 1000.f;
     // the flags live in the pinned staging area so that a re-query can upload the slice of a node
     memset(taken, 0, (size_t)R);
-    auto requery = [&](int k, int* pick) -> int {
+    auto requery = [&](int k, unsigned* fresh) -> int {
+        ++m->num_requeries;
         const size_t len = (size_t)(seg[k].y - seg[k].x);
         OVS_CUDA_CHECK(cudaMemcpyAsync(dtaken + seg[k].x, taken + seg[k].x, len, cudaMemcpyHostToDevice, st));
         TriArgs B = A;
@@ -1264,11 +1171,10 @@ extern "C" int ovs_robust_match_for_triangulation_host(ovs_matcher* m, int n1, c
         OVS_LAUNCH_CHECK();
         OVS_CUDA_CHECK(cudaMemcpyAsync(m->h_keys + (size_t)Q * kTriK, m->d_keys + (size_t)Q * kTriK, kTriK * 4, cudaMemcpyDeviceToHost, st));
         OVS_CUDA_CHECK(ovs::sync_stream(st));
-        const unsigned key = m->h_keys[(size_t)Q * kTriK];
-        *pick = key != 0xffffffffu ? 0xffff - (int)(key & 0xffffu) : -1;
+        memcpy(fresh, m->h_keys + (size_t)Q * kTriK, kTriK * 4);
         return OVS_OK;
     };
-    return tri_replay(m, Q, q1.data(), rank2.data(), m->h_keys, taken, nullptr, angle_1, angle_2, check_orientation, requery,
+    return tri_replay(Q, q1.data(), rank2.data(), m->h_keys, taken, nullptr, angle_1, angle_2, check_orientation, requery,
                       matched_idx_2_of_1, nullptr, num_matches);
 }
 
@@ -1302,12 +1208,12 @@ extern "C" int ovs_create_new_landmarks_host(ovs_matcher* m, const ovs_keyframe_
     }
     *num_out = 0;
     std::vector<int> q1;
-    tri_order(n1, K1.has_landmark, K1.bow_node, q1);
+    node_order(n1, K1.bow_node, [&](int i) { return !K1.has_landmark[i]; }, q1);
     const int Q = (int)q1.size();
     std::vector<std::vector<int>> rank2((size_t)B);
     std::vector<int> tbase((size_t)B + 1, 0);
     for (int b = 0; b < B; ++b) {
-        tri_order(keyfrms_2[b].num_keypts, keyfrms_2[b].has_landmark, keyfrms_2[b].bow_node, rank2[b]);
+        node_order(keyfrms_2[b].num_keypts, keyfrms_2[b].bow_node, [&](int i) { return !keyfrms_2[b].has_landmark[i]; }, rank2[b]);
         tbase[b + 1] = tbase[b] + (int)rank2[b].size();
     }
     const int R = tbase[B];
@@ -1357,7 +1263,7 @@ extern "C" int ovs_create_new_landmarks_host(ovs_matcher* m, const ovs_keyframe_
             ht8[g] = K2.stereo_x_right && 0.0f <= K2.stereo_x_right[i];
             hkp[sQ + g] = ovs::tri_keypt(K2, i);
         }
-        tri_segments(q1, K1.bow_node, rk, K2.bow_node, hsg + sQ * b);
+        node_segments(q1, K1.bow_node, rk, K2.bow_node, hsg + sQ * b);
         memcpy(hE + 9 * b, E_12 + 9 * (size_t)b, 72); memcpy(hep + 3 * b, epipole_in_2 + 3 * (size_t)b, 24);
         htb0[b] = tbase[b];
         hprob[b].c[0] = ovs::tri_cam(K1); hprob[b].c[1] = ovs::tri_cam(K2);
@@ -1390,7 +1296,8 @@ extern "C" int ovs_create_new_landmarks_host(ovs_matcher* m, const ovs_keyframe_
         const size_t qoff = sQ * b;
         std::vector<double> rq_pos((size_t)3 * Q);       // a re-queried pair's point, by query
         std::vector<uint8_t> rq_valid((size_t)Q, 0);
-        auto requery = [&](int k, int* pick) -> int {
+        auto requery = [&](int k, unsigned* fresh) -> int {
+            ++m->num_requeries;
             const int2 sg = hsg[qoff + k];
             OVS_CUDA_CHECK(cudaMemcpyAsync(dtaken + tbase[b] + sg.x, taken + tbase[b] + sg.x, (size_t)(sg.y - sg.x), cudaMemcpyHostToDevice, st));
             TriArgs Aq = A;
@@ -1401,12 +1308,11 @@ extern "C" int ovs_create_new_landmarks_host(ovs_matcher* m, const ovs_keyframe_
             Lq.n = 1; Lq.keys = dkeys + NQ * kTriK; Lq.fixed_prob = b; Lq.fixed_query = k; Lq.valid = L.valid + NQ * kTriK; Lq.pos = drq;
             const int rc2 = ovs::launch_two_view_triangulate(Lq, st);
             if (rc2 != OVS_OK) return rc2;
-            OVS_CUDA_CHECK(cudaMemcpyAsync(hkeys + NQ * kTriK, dkeys + NQ * kTriK, 4, cudaMemcpyDeviceToHost, st));
+            OVS_CUDA_CHECK(cudaMemcpyAsync(hkeys + NQ * kTriK, dkeys + NQ * kTriK, kTriK * 4, cudaMemcpyDeviceToHost, st));
             OVS_CUDA_CHECK(cudaMemcpyAsync(hvalid + NQ * kTriK, L.valid + NQ * kTriK, 1, cudaMemcpyDeviceToHost, st));
             OVS_CUDA_CHECK(cudaMemcpyAsync(hrq, drq, 24, cudaMemcpyDeviceToHost, st));
             OVS_CUDA_CHECK(ovs::sync_stream(st));
-            const unsigned key = hkeys[NQ * kTriK];
-            *pick = key != 0xffffffffu ? 0xffff - (int)(key & 0xffffu) : -1;
+            memcpy(fresh, hkeys + NQ * kTriK, kTriK * 4);
             rq_valid[k] = hvalid[NQ * kTriK];
             for (int c = 0; c < 3; ++c) rq_pos[3 * (size_t)k + c] = hrq[c];
             return OVS_OK;
@@ -1416,7 +1322,7 @@ extern "C" int ovs_create_new_landmarks_host(ovs_matcher* m, const ovs_keyframe_
         memset(taken + tbase[b], 0, rank2[b].size());
         std::fill(match.begin(), match.end(), -1);
         int nm = 0;
-        if ((rc = tri_replay(m, Q, q1.data(), rank2[b].data(), hkeys + qoff * kTriK, taken + tbase[b], got.data(), angle_1.data(),
+        if ((rc = tri_replay(Q, q1.data(), rank2[b].data(), hkeys + qoff * kTriK, taken + tbase[b], got.data(), angle_1.data(),
                              angle_2.data(), check_orientation, requery, match.data(), slot.data(), &nm)) != OVS_OK)
             return rc;
         // triangulate_with_two_keyframes: the pairs in idx_1 order
@@ -1485,26 +1391,10 @@ __global__ void __launch_bounds__(128) k_node_topk(NodeArgs A, unsigned* __restr
             const int c = c0 + k * 32 + lane;
             if (c < seg.y && !(A.taken && A.taken[c])) {
                 const uint4 ta = A.tdesc[2 * (size_t)c], tb = A.tdesc[2 * (size_t)c + 1];
-                const int d = __popc(qa.x ^ ta.x) + __popc(qa.y ^ ta.y) + __popc(qa.z ^ ta.z) + __popc(qa.w ^ ta.w)
-                              + __popc(qb.x ^ tb.x) + __popc(qb.y ^ tb.y) + __popc(qb.z ^ tb.z) + __popc(qb.w ^ tb.w);
-                mine[k] = ((unsigned)d << 16) | (unsigned)c;
+                mine[k] = ((unsigned)hamming256(qa, qb, ta, tb) << 16) | (unsigned)c;
             }
         }
-        unsigned next_extra = 0xffffffffu;
-#pragma unroll
-        for (int r = 0; r < kNodeK; ++r) {
-            unsigned lmin = extra;
-#pragma unroll
-            for (int k = 0; k < kNodeK; ++k) lmin = min(lmin, mine[k]);
-            const unsigned wmin = __reduce_min_sync(0xffffffffu, lmin);
-            if (wmin != 0xffffffffu) {
-                if (extra == wmin) extra = 0xffffffffu;
-#pragma unroll
-                for (int k = 0; k < kNodeK; ++k) if (mine[k] == wmin) mine[k] = 0xffffffffu;
-            }
-            if (lane == r) next_extra = wmin;
-        }
-        extra = next_extra;
+        extra = warp_merge_topk(extra, mine, lane);
     }
     if (lane < kNodeK) keys_out[(size_t)(q + A.out_shift) * kNodeK + lane] = extra;
 }
@@ -1518,24 +1408,13 @@ int bow_core(ovs_matcher* m, int na, const uint8_t* desc_a, const uint8_t* valid
     if (na == 0 || nb == 0) return OVS_OK;
     OVS_CUDA_CHECK(cudaSetDevice(m->device));
     std::vector<int> rankb, qa;
-    for (int i = 0; i < nb; ++i) if ((!valid_b || valid_b[i]) && node_b[i] >= 0) rankb.push_back(i);
-    std::stable_sort(rankb.begin(), rankb.end(), [&](int x, int y) { return node_b[x] < node_b[y]; });
-    for (int i = 0; i < na; ++i) if ((!valid_a || valid_a[i]) && node_a[i] >= 0) qa.push_back(i);
-    std::stable_sort(qa.begin(), qa.end(), [&](int x, int y) { return node_a[x] < node_a[y]; });
+    node_order(nb, node_b, [&](int i) { return !valid_b || valid_b[i]; }, rankb);
+    node_order(na, node_a, [&](int i) { return !valid_a || valid_a[i]; }, qa);
     const int R = (int)rankb.size(), Q = (int)qa.size();
     if (R == 0 || Q == 0) return OVS_OK;
     OVS_REQUIRE(R < 65536, OVS_ERR_UNSUPPORTED, "more than 65535 candidate keypoints");
     std::vector<int2> seg(Q);
-    {
-        size_t lo = 0;
-        for (int k = 0; k < Q; ++k) {
-            const int node = node_a[qa[k]];
-            while (lo < rankb.size() && node_b[rankb[lo]] < node) ++lo;
-            size_t hi = lo;
-            while (hi < rankb.size() && node_b[rankb[hi]] == node) ++hi;
-            seg[k] = make_int2((int)lo, (int)hi);
-        }
-    }
+    node_segments(qa, node_a, rankb, node_b, seg.data());
     NodeArgs A{};
     uint8_t *hqd, *htd, *taken, *dtaken; int2* hsg;
     ovs::Staging S;
@@ -1562,55 +1441,33 @@ int bow_core(ovs_matcher* m, int na, const uint8_t* desc_a, const uint8_t* valid
     OVS_CUDA_CHECK(ovs::sync_stream(st));
     float ms = 0; cudaEventElapsedTime(&ms, m->ev[0], m->ev[1]);
     m->last_kernel_us = ms * 1000.f;
-    // a candidate farther than d_star can neither be an acceptable best nor make the ratio test fail (see brute_force_match)
-    int d_star = OVS_HAMMING_DIST_THR_LOW + 1;
-    while (d_star < OVS_MAX_HAMMING_DIST && lowe_ratio * (float)(unsigned)d_star < (float)OVS_HAMMING_DIST_THR_LOW) ++d_star;
-    ++d_star;
     memset(taken, 0, (size_t)R);
+    const auto decode = [](unsigned key) { return (int)(key & 0xffffu); };
+    const auto not_taken = [&](int r, int) { return !taken[r]; };
+    const auto ratio = [&](const ovs::ReplayList<kNodeK>& L, int second, ovs::Second) { return !(lowe_ratio * (float)(unsigned)second < (float)L.dist[0]); };
+    const int complete_at = ovs::d_star(lowe_ratio);
     for (int k = 0; k < Q; ++k) {
-        unsigned keys[kNodeK];
-        memcpy(keys, m->h_keys + (size_t)k * kNodeK, sizeof(keys));
-        for (int attempt = 0; attempt < 2; ++attempt) {
-            int rem[kNodeK], r = 0;
-            bool exhausted = false;
-            for (int j = 0; j < kNodeK; ++j) {
-                if (keys[j] == 0xffffffffu) { exhausted = true; break; }
-                if (!taken[keys[j] & 0xffffu]) rem[r++] = j;
-            }
-            const int lb = exhausted ? OVS_MAX_HAMMING_DIST : (int)(keys[kNodeK - 1] >> 16);   // unlisted candidates are >= this
-            const bool complete = exhausted || lb >= d_star || attempt == 1;
-            int best = OVS_MAX_HAMMING_DIST, best_r = -1, second = OVS_MAX_HAMMING_DIST;
-            bool decided = true;
-            if (r >= 2 || complete) {
-                if (r >= 1) { best = (int)(keys[rem[0]] >> 16); best_r = (int)(keys[rem[0]] & 0xffffu); }
-                if (r >= 2) second = (int)(keys[rem[1]] >> 16);
-            } else if (r == 1) {
-                best = (int)(keys[rem[0]] >> 16); best_r = (int)(keys[rem[0]] & 0xffffu);
-                if (best <= OVS_HAMMING_DIST_THR_LOW && lowe_ratio * (float)(unsigned)lb < (float)best) decided = false;   // needs the true second best
-                second = lb;
-            } else if (lb <= OVS_HAMMING_DIST_THR_LOW) {
-                decided = false;
-            }
-            if (!decided) {
-                ++m->num_requeries;
-                const size_t len = (size_t)(seg[k].y - seg[k].x);
-                OVS_CUDA_CHECK(cudaMemcpyAsync(dtaken + seg[k].x, taken + seg[k].x, len, cudaMemcpyHostToDevice, st));
-                NodeArgs B = A;
-                B.q0 = k; B.nq = k + 1; B.out_shift = Q - k; B.taken = dtaken;
-                k_node_topk<<<1, 128, 0, st>>>(B, m->d_keys);
-                OVS_LAUNCH_CHECK();
-                OVS_CUDA_CHECK(cudaMemcpyAsync(m->h_keys + (size_t)Q * kNodeK, m->d_keys + (size_t)Q * kNodeK, kNodeK * 4, cudaMemcpyDeviceToHost, st));
-                OVS_CUDA_CHECK(ovs::sync_stream(st));
-                memcpy(keys, m->h_keys + (size_t)Q * kNodeK, sizeof(keys));
-                continue;
-            }
-            if (OVS_HAMMING_DIST_THR_LOW < best) break;
-            if (lowe_ratio * (float)(unsigned)second < (float)best) break;
-            taken[best_r] = 1;
-            match_b_of_a[qa[k]] = rankb[best_r];
-            visit_order.push_back(qa[k]);
-            break;
-        }
+        // the re-query's list goes to the spare row Q
+        const auto requery = [&](unsigned* fresh) -> int {
+            ++m->num_requeries;
+            const size_t len = (size_t)(seg[k].y - seg[k].x);
+            OVS_CUDA_CHECK(cudaMemcpyAsync(dtaken + seg[k].x, taken + seg[k].x, len, cudaMemcpyHostToDevice, st));
+            NodeArgs B = A;
+            B.q0 = k; B.nq = k + 1; B.out_shift = Q - k; B.taken = dtaken;
+            k_node_topk<<<1, 128, 0, st>>>(B, m->d_keys);
+            OVS_LAUNCH_CHECK();
+            OVS_CUDA_CHECK(cudaMemcpyAsync(m->h_keys + (size_t)Q * kNodeK, m->d_keys + (size_t)Q * kNodeK, kNodeK * 4, cudaMemcpyDeviceToHost, st));
+            OVS_CUDA_CHECK(ovs::sync_stream(st));
+            memcpy(fresh, m->h_keys + (size_t)Q * kNodeK, kNodeK * 4);
+            return OVS_OK;
+        };
+        ovs::ReplayPick p;
+        rc = ovs::replay_query<kNodeK>(m->h_keys + (size_t)k * kNodeK, OVS_HAMMING_DIST_THR_LOW, complete_at, decode, not_taken, ratio, requery, &p);
+        if (rc != OVS_OK) return rc;
+        if (p.id < 0) continue;
+        taken[p.id] = 1;
+        match_b_of_a[qa[k]] = rankb[p.id];
+        visit_order.push_back(qa[k]);
     }
     return OVS_OK;
 }
@@ -1632,17 +1489,13 @@ extern "C" int ovs_bow_tree_match_frame_and_keyframe_host(ovs_matcher* m, int n_
     const int rc = bow_core(m, n_kf, desc_kf, lm_valid_kf, bow_node_kf, n_frm, desc_frm, nullptr, bow_node_frm, lowe_ratio, match, order);
     if (rc != OVS_OK) return rc;
     int num = 0;
-    std::vector<float> deltas; std::vector<int> delta_idx;
+    ovs::OrientationCheck orientation;
     for (int k : order) {
         const int f = match[k];
         matched_keyfrm_idx_of_frm[f] = k; ++num;
-        if (check_orientation) { deltas.push_back(angle_kf[k] - angle_frm[f]); delta_idx.push_back(f); }
+        if (check_orientation) orientation.add(angle_kf[k] - angle_frm[f], f);
     }
-    if (check_orientation && !deltas.empty()) {
-        std::vector<uint8_t> invalid;
-        angle_checker_invalid(deltas, invalid);
-        for (size_t k = 0; k < deltas.size(); ++k) if (invalid[k]) { matched_keyfrm_idx_of_frm[delta_idx[k]] = -1; --num; }
-    }
+    orientation.unset_invalid([&](int f) { matched_keyfrm_idx_of_frm[f] = -1; --num; });
     *num_matches = num;
     return OVS_OK;
 }
@@ -1662,16 +1515,12 @@ extern "C" int ovs_bow_tree_match_keyframes_host(ovs_matcher* m, int n1, const u
     const int rc = bow_core(m, n1, desc_1, lm_valid_1, bow_node_1, n2, desc_2, lm_valid_2, bow_node_2, lowe_ratio, match, order);
     if (rc != OVS_OK) return rc;
     int num = 0;
-    std::vector<float> deltas; std::vector<int> delta_idx;
+    ovs::OrientationCheck orientation;
     for (int i1 : order) {
         matched_idx_2_of_1[i1] = match[i1]; ++num;
-        if (check_orientation) { deltas.push_back(angle_1[i1] - angle_2[match[i1]]); delta_idx.push_back(i1); }
+        if (check_orientation) orientation.add(angle_1[i1] - angle_2[match[i1]], i1);
     }
-    if (check_orientation && !deltas.empty()) {
-        std::vector<uint8_t> invalid;
-        angle_checker_invalid(deltas, invalid);
-        for (size_t k = 0; k < deltas.size(); ++k) if (invalid[k]) { matched_idx_2_of_1[delta_idx[k]] = -1; --num; }
-    }
+    orientation.unset_invalid([&](int i1) { matched_idx_2_of_1[i1] = -1; --num; });
     *num_matches = num;
     return OVS_OK;
 }
