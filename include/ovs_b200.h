@@ -774,13 +774,9 @@ int ovs_global_ba_host(ovs_optimizer* h, const ovs_camera* cam, int setup_is_mon
                        int L, double* points, int M, const int32_t* obs_kf, const int32_t* obs_lm, const float* obs_xy,
                        const float* obs_x_right, const float* inv_sigma_sq, int num_iter, int use_huber_kernel,
                        const volatile uint8_t* force_stop_flag, ovs_ba_stats* stats);
-/* Development aid: SM clock stamps of the phases of the last reduced-system factorisation (192 values). */
-int ovs_optimizer_debug_clocks(ovs_optimizer* h, long long* out192);
 /* Test hook: the stable radix sort of the BA graph preparation (co-observations by keyframe pair: k_sort_hist /
  * k_sort_tile_prefix / k_sort_scatter) on host arrays, by the low end_bit bits of the keys. */
 int ovs_debug_sort_pairs(int device, const uint32_t* keys, const uint64_t* vals, int n, int end_bit, uint32_t* keys_out, uint64_t* vals_out);
-/* CTAs per thread-block cluster of the reduced-system solver on this device (8, or 16 when 4 such clusters can be co-resident). */
-int ovs_optimizer_cluster_width(const ovs_optimizer* h);
 /* Local / global BA: CTAs per cluster of the reduced-system solver (1, 2, 4 or 8; default 8).  8 gives the lowest latency of a
  * single call; 2 is meant for several optimisers sharing the GPU: each call occupies fewer SMs, so more calls run at once.
  * The result does not depend on the width. */

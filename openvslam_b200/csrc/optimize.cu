@@ -656,12 +656,11 @@ __host__ __device__ __forceinline__ size_t chol_back_doubles(int n) { return (si
 
 __global__ void __launch_bounds__(kCholThreads, 1)
 k_ba_cholesky_solve(const LmCtl* __restrict__ ctl, double* __restrict__ A, size_t A_stride, int n, double* __restrict__ x, double* __restrict__ invL, size_t invL_stride,
-                    int* __restrict__ fail, long long* __restrict__ dbg_clk, int dbuf) {
+                    int* __restrict__ fail, int dbuf) {
     {
         const int bt = blockIdx.x / (int)cluster_size();   // one cluster per speculative trial
         if (bt >= ctl->nbatch) return;                      // the whole cluster leaves together
         A += (size_t)bt * A_stride; x += (size_t)bt * n; invL += (size_t)bt * invL_stride; fail += bt;
-        if (bt != 0) dbg_clk = nullptr;
     }
     extern __shared__ __align__(16) double sh[];
     const int npad = ((n + 1 + 31) / 32) * 32;
@@ -673,17 +672,12 @@ k_ba_cholesky_solve(const LmCtl* __restrict__ ctl, double* __restrict__ A, size_
     double* P = IL + 32 * kPP;              // panel, row-major, pitch kPP                  // panel, row-major, pitch kPP
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     const int rank = (int)cluster_rank();
-    const int ncta = (int)cluster_size();   // cluster width is a launch attribute (8, or 16 where the device can co-schedule it)
+    const int ncta = (int)cluster_size();   // cluster width is a launch attribute (1, 2, 4 or 8)
     const int g = lane >> 2, q = lane & 3;
     __shared__ int s_fail;
     if (tid == 0) s_fail = 0;
     __syncthreads();
     const int nblk = (n + kNB - 1) / kNB;
-    // phase clocks of CTA 0 (development aid, read through ovs_optimizer_debug_clocks): per block step
-    // [start, panel loaded, panel solved, look-ahead done, barrier done]; first trailing tile (warp 2) at 50 + 4 blk;
-    // look-ahead detail at 168 + 2 blk; back-substitution from 94
-    auto stamp = [&](int slot) { if (dbg_clk && rank == 0 && tid == 0 && slot < 192) dbg_clk[slot] = clock64(); };
-    auto stamp1 = [&](int slot) { if (dbg_clk && rank == 0 && tid == 64 && slot < 192) dbg_clk[slot] = clock64(); };
 
     // factorisation of the 32 x 32 block held one row per lane in a[] (warp 0 only).  Column j of the factor goes to
     // cs[j * 32 + lane] as soon as it is final (that store is also how the lanes exchange it), so a[j] is dead after
@@ -725,7 +719,6 @@ k_ba_cholesky_solve(const LmCtl* __restrict__ ctl, double* __restrict__ A, size_
         const int rem = n - kb - nb;          // matrix rows below the block; the rhs row is row `rem` of the panel
         const int prow = rem + 1;             // panel rows including the rhs row
         const int nbn = min(kNB, rem);        // width of the next diagonal block (rows/cols 0..nbn-1 of the trailing matrix)
-        if (!pro) stamp(5 * blk);
         // ---- panel rows (and the rhs row): one warp per row, lane = column: a coalesced 256 B global read and a
         //      conflict-free shared write per instruction
         if (wid >= 2 && !pro) {
@@ -743,7 +736,6 @@ k_ba_cholesky_solve(const LmCtl* __restrict__ ctl, double* __restrict__ A, size_
         }
         if (!pro) {
             __syncthreads();                  // panel loaded; LdT / invd / s_fail of this block (look-ahead) visible
-            stamp(5 * blk + 1);
             if (s_fail) break;
         }
         // ---- panel: L21 = A21 L11^-T (rows below + rhs row) by substitution, one row per thread.  Warp 0 takes the
@@ -784,7 +776,6 @@ k_ba_cholesky_solve(const LmCtl* __restrict__ ctl, double* __restrict__ A, size_
                 for (int c = 0; c < kNB; c += 2) *reinterpret_cast<double2*>(row + c) = make_double2(xr[c], xr[c + 1]);
             }
             __syncwarp();
-            if (!pro) stamp(5 * blk + 2);
             if (rem == 0) {
                 // last block: only the rhs row was left; there is no cluster barrier before the back-substitution,
                 // so CTA 0 writes it itself
@@ -825,10 +816,8 @@ k_ba_cholesky_solve(const LmCtl* __restrict__ ctl, double* __restrict__ A, size_
             double a[kNB];
 #pragma unroll
             for (int c = 0; c < kNB; ++c) a[c] = (lane < nbn && c <= lane) ? scr[lane * 33 + c] : ((c == lane) ? 1.0 : 0.0);
-            if (blk < 12 && !pro) { asm volatile("" :: "d"(a[0]), "d"(a[kNB - 1])); stamp(168 + 2 * blk); }
             __syncwarp();                                        // every lane has its row: scr becomes the column store
             const double my_inv = factor_block(a, scr);
-            if (blk < 12 && !pro) { asm volatile("" :: "d"(my_inv)); stamp(169 + 2 * blk); }
             if (!pro) asm volatile("bar.sync 2, 64;\n" ::: "memory");      // warp 1 is done reading LdT / invd
 #pragma unroll
             for (int c = 0; c < kNB; ++c) LdT[c * 32 + lane] = scr[c * 32 + lane];
@@ -912,7 +901,6 @@ k_ba_cholesky_solve(const LmCtl* __restrict__ ctl, double* __restrict__ A, size_
                     for (;; ++mi) { const int cnt = min(nmc, (16 * mi + 15) / 32 + 1); if (w < base + cnt) break; base += cnt; }
                     const int mj = w - base;
                     const int R0 = mi * 16, C0 = mj * 32;
-                    if (w == 0) stamp1(50 + 4 * blk);
                     double acc[2][4][2];
 #pragma unroll
                     for (int ti = 0; ti < 2; ++ti)
@@ -924,7 +912,6 @@ k_ba_cholesky_solve(const LmCtl* __restrict__ ctl, double* __restrict__ A, size_
                                 const bool mine = rr < prow && cc < rem && cc <= rr && !(rr < nbn);   // rows < nbn: next diagonal block (warp 0)
                                 acc[ti][tj][e] = mine ? A[(size_t)(kb + nb + rr) * n + kb + nb + cc] : 0.0;
                             }
-                    if (w == 0) { asm volatile("" :: "d"(acc[0][0][0]), "d"(acc[1][3][1]), "d"(acc[1][0][0]), "d"(acc[0][3][1])); stamp1(51 + 4 * blk); }
                     const double* pa0 = P + (size_t)min(R0 + g, prow - 1) * kPP + q;
                     const double* pa1 = P + (size_t)min(R0 + 8 + g, prow - 1) * kPP + q;
                     const double* pb[4];
@@ -942,7 +929,6 @@ k_ba_cholesky_solve(const LmCtl* __restrict__ ctl, double* __restrict__ A, size_
                             dmma_m8n8k4(acc[1][tj][0], acc[1][tj][1], af1, bf[tj]);
                         }
                     }
-                    if (w == 0) { asm volatile("" :: "d"(acc[0][0][0]), "d"(acc[1][3][1])); stamp1(52 + 4 * blk); }
 #pragma unroll
                     for (int ti = 0; ti < 2; ++ti)
 #pragma unroll
@@ -953,15 +939,12 @@ k_ba_cholesky_solve(const LmCtl* __restrict__ ctl, double* __restrict__ A, size_
                                 const bool mine = rr < prow && cc < rem && cc <= rr && !(rr < nbn);
                                 if (mine) A[(size_t)(kb + nb + rr) * n + kb + nb + cc] = acc[ti][tj][e];
                             }
-                    if (w == 0) stamp1(53 + 4 * blk);
                 }
             }
         }
         if (rem == 0) break;
         if (pro) continue;
-        stamp(5 * blk + 3);
         cluster_sync_all();   // the trailing matrix (global) is complete and visible to every CTA
-        stamp(5 * blk + 4);
     }
     __syncthreads();
     if (s_fail) { if (tid == 0 && rank == 0) *fail = 1; return; }
@@ -995,7 +978,6 @@ k_ba_cholesky_solve(const LmCtl* __restrict__ ctl, double* __restrict__ A, size_
         asm volatile("cp.async.commit_group;\n" ::);
     };
     __syncthreads();   // LdT / panel are free
-    stamp(94);
     stage(nblk - 1, 0);
     for (int blk = nblk - 1; blk >= 0; --blk) {
         const int kb = blk * kNB;
@@ -1008,7 +990,6 @@ k_ba_cholesky_solve(const LmCtl* __restrict__ ctl, double* __restrict__ A, size_
             asm volatile("cp.async.wait_group 0;\n" ::);
         }
         __syncthreads();
-        stamp(96 + 3 * (nblk - 1 - blk));
         const double* Lc = cur ? L1buf : LdT;
         const double* rows = cur ? R1buf : R0buf;
         if (wid == 0) {
@@ -1023,7 +1004,6 @@ k_ba_cholesky_solve(const LmCtl* __restrict__ ctl, double* __restrict__ A, size_
             if (lane < nb) vec[kb + lane] = acc0 + acc1;
         }
         __syncthreads();
-        stamp(97 + 3 * (nblk - 1 - blk));
         for (int i = tid; i < kb; i += kCholThreads) {
             double s0 = 0, s1 = 0;
 #pragma unroll 8
@@ -1034,11 +1014,9 @@ k_ba_cholesky_solve(const LmCtl* __restrict__ ctl, double* __restrict__ A, size_
             vec[i] -= s0 + s1;
         }
         __syncthreads();
-        stamp(98 + 3 * (nblk - 1 - blk));
         if (!dbuf && blk > 0) stage(blk - 1, 0);
     }
     for (int i = tid; i < n; i += kCholThreads) x[i] = vec[i];
-    stamp(95);
 }
 
 // ---- Reduced systems too large for the shared-memory panel of k_ba_cholesky_solve (n > kMaxReducedDim, i.e. more than
@@ -2278,7 +2256,7 @@ struct ovs_optimizer {
     uint8_t* d_work = nullptr; size_t w_cap = 0;    // local BA: buffers sized by the number of free keyframes / co-observations
     int* h_mirror = nullptr;                         // pinned, mapped: [0] nbatch, [1] active (written by the device), [2] stop word (host)
     int* d_mirror = nullptr;
-    int chol_cluster = kCholCluster;                 // CTAs per Cholesky cluster (8 portable, 16 when co-schedulable)
+    int chol_cluster = kCholCluster;                 // CTAs per Cholesky cluster (1, 2, 4 or 8)
 };
 
 namespace {
@@ -2953,7 +2931,7 @@ struct ovs_ba_plan {
     int4 *dchunks = nullptr, *ddchunks = nullptr; int *dpair_chunk_begin = nullptr, *dkf_chunk_begin = nullptr;
     int* dnchunks = nullptr;                                    // [0] chunks of the Schur stage, [1] chunks of the Hpp stage
     double *dspart = nullptr, *dppart = nullptr; int max_chunks = 0, max_dchunks = 0;
-    double *dpchi = nullptr, *dpscale = nullptr; int* dfail = nullptr; double* dmaxdiag = nullptr; long long* dclk = nullptr;
+    double *dpchi = nullptr, *dpscale = nullptr; int* dfail = nullptr; double* dmaxdiag = nullptr;
     int cur = 0;   // index of the buffer holding the current estimate after run
 };
 
@@ -2962,7 +2940,7 @@ namespace {
 // The dense FP64 solver of one trial batch: kSpec systems (n + 1) x n (lower triangle + rhs row, S_stride apart), factorised in
 // place, solutions to x (n apart).  The cluster kernel up to the shared-memory panel limit, the multi-launch path above it.
 struct DenseSolve {
-    double* S; size_t S_stride; int n; double* x; double* invL; size_t invL_stride; int* fail; long long* clk;
+    double* S; size_t S_stride; int n; double* x; double* invL; size_t invL_stride; int* fail;
     int chol_big, chol_dbuf; size_t chol_smem;
 };
 
@@ -3016,7 +2994,7 @@ int prepare_impl(ovs_optimizer* h, const ovs_camera* cam, int setup_is_mono, int
         pl.dlblocks = S.dev<int4>((size_t)nlseg * kLbSegCap); pl.dnlblocks = S.dev<int>(nlseg);
         pl.dHll = S.dev<double>(6 * sL); pl.dbl = S.dev<double>(3 * sL);
         pl.dpchi = S.dev<double>(kSpec * (size_t)nb_obs); pl.dpscale = S.dev<double>(kSpec * (size_t)nb_upd);
-        pl.dfail = S.dev<int>(kSpec); pl.dmaxdiag = S.dev<double>(2); pl.dclk = S.dev<long long>(192); pl.dnchunks = S.dev<int>(2);
+        pl.dfail = S.dev<int>(kSpec); pl.dmaxdiag = S.dev<double>(2); pl.dnchunks = S.dev<int>(2);
     });
     if (rc != OVS_OK) return rc;
     pl.exec_cap = exec_cap;
@@ -3214,7 +3192,7 @@ int launch_dense_solve(ovs_optimizer* h, cudaStream_t st, LmCtl* ctl, const Dens
         at[0].id = cudaLaunchAttributeClusterDimension;
         at[0].val.clusterDim.x = (unsigned)h->chol_cluster; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
         cfg.attrs = at; cfg.numAttrs = 1;
-        OVS_CUDA_CHECK(cudaLaunchKernelEx(&cfg, k_ba_cholesky_solve, (const LmCtl*)ctl, ds.S, ds.S_stride, n, ds.x, ds.invL, ds.invL_stride, ds.fail, ds.clk, ds.chol_dbuf));
+        OVS_CUDA_CHECK(cudaLaunchKernelEx(&cfg, k_ba_cholesky_solve, (const LmCtl*)ctl, ds.S, ds.S_stride, n, ds.x, ds.invL, ds.invL_stride, ds.fail, ds.chol_dbuf));
         ovs::count_launch();
     } else {
         for (int kb = 0; kb < n; kb += kNB) {
@@ -3409,7 +3387,7 @@ int run_impl(ovs_optimizer* h, int rounds, int huber_first, int num_first_iter, 
         k_ba_schur_final<<<dim3(npairs, kSpec), 64, 0, st>>>(n, ctl, pl.dpair_chunk_begin, pl.dpab, pl.dspart, pl.spart_stride, pl.dHpp, pl.dbp, pl.dS, pl.S_stride);
         OVS_LAUNCH_CHECK();
         if (ev) OVS_CUDA_CHECK(cudaEventRecord(h->solver_ev[4 * slot + 1], st));     // end of the Schur complement = start of the solver
-        const DenseSolve ds{pl.dS, pl.S_stride, n, pl.dx, pl.dinvL, pl.invL_stride, pl.dfail, pl.dclk, pl.chol_big, pl.chol_dbuf, pl.chol_smem};
+        const DenseSolve ds{pl.dS, pl.S_stride, n, pl.dx, pl.dinvL, pl.invL_stride, pl.dfail, pl.chol_big, pl.chol_dbuf, pl.chol_smem};
         const int rc_solve = launch_dense_solve(h, st, ctl, ds);
         if (rc_solve != OVS_OK) return rc_solve;
         if (ev) OVS_CUDA_CHECK(cudaEventRecord(h->solver_ev[4 * slot + 3], st));
@@ -3539,8 +3517,6 @@ extern "C" int ovs_global_ba_host(ovs_optimizer* h, const ovs_camera* cam, int s
     return ovs_local_ba_fetch(h, poses, points, nullptr);
 }
 
-extern "C" int ovs_optimizer_cluster_width(const ovs_optimizer* h) { return h ? h->chol_cluster : 0; }
-
 // CTAs per thread-block cluster of the reduced-system solver: 8 (default) minimises the latency of one call; a process that
 // runs several optimisers concurrently on one GPU gets more calls per second with 2 (the solver is latency bound: a wider
 // cluster shortens it little but occupies 4x the SMs, which the other streams' kernels could use).  Same results for every width.
@@ -3571,13 +3547,6 @@ extern "C" int ovs_optimizer_set_graphs(ovs_optimizer* h, int enable) {
 extern "C" int ovs_optimizer_set_host_sync(ovs_optimizer* h, int mode) {
     OVS_REQUIRE(h && mode >= -1 && mode <= 1, OVS_ERR_INVALID_ARG, "host-sync mode must be -1 (auto), 0 or 1");
     h->lm_host_sync = mode;
-    return OVS_OK;
-}
-
-extern "C" int ovs_optimizer_debug_clocks(ovs_optimizer* h, long long* out192) {
-    OVS_REQUIRE(h && out192 && h->plan->valid, OVS_ERR_INVALID_ARG, "no prepared bundle-adjustment problem");
-    OVS_CUDA_CHECK(cudaSetDevice(h->device));
-    OVS_CUDA_CHECK(cudaMemcpy(out192, h->plan->dclk, 192 * sizeof(long long), cudaMemcpyDeviceToHost));
     return OVS_OK;
 }
 
@@ -3666,33 +3635,6 @@ extern "C" int ovs_optimizer_create(int device, ovs_optimizer** out) {
         ovs::set_error("optimizer handle setup failed: %s", cudaGetErrorString(cudaGetLastError()));
         ovs_optimizer_destroy(h);
         return OVS_ERR_CUDA;
-    }
-    // Cluster width of the reduced-system solver: 8 (portable) by default.  OVS_B200_CHOL_CLUSTER=16 selects the
-    // non-portable size when the device can keep one such cluster per speculative trial resident (development aid).
-    {
-        if (const char* e = getenv("OVS_B200_GRAPHS")) h->use_graphs = atoi(e);
-        if (const char* e = getenv("OVS_B200_LM_HOST_SYNC")) h->lm_host_sync = atoi(e) ? 1 : 0;   // development aid
-        if (const char* e = getenv("OVS_B200_SPEC2")) h->spec_width2 = std::min(kSpec, std::max(0, atoi(e)));   // development aid
-        if (const char* e = getenv("OVS_B200_SPEC")) h->spec_width = std::min(kSpec, std::max(1, atoi(e)));   // development aid: 0 = plain launches
-        int want = kCholCluster;   // the pivot chain, not the trailing update, bounds a block step: wider clusters mostly occupy more SMs
-        if (const char* e = getenv("OVS_B200_CHOL_CLUSTER")) want = atoi(e);
-        if (want > kCholCluster && cudaFuncSetAttribute(k_ba_cholesky_solve, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess) {
-            cudaLaunchConfig_t cfg = {};
-            cfg.gridDim = dim3((unsigned)(want * kSpec));
-            cfg.blockDim = dim3(kCholThreads);
-            cfg.dynamicSmemBytes = kCholMaxDynSmem;
-            cudaLaunchAttribute at[1];
-            at[0].id = cudaLaunchAttributeClusterDimension;
-            at[0].val.clusterDim.x = (unsigned)want; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-            cfg.attrs = at; cfg.numAttrs = 1;
-            int nclusters = 0;
-            const cudaError_t qe = cudaOccupancyMaxActiveClusters(&nclusters, k_ba_cholesky_solve, &cfg);
-            if (qe == cudaSuccess && nclusters >= kSpec) h->chol_cluster = want;
-            if (getenv("OVS_B200_DEBUG")) fprintf(stderr, "ovs_b200: %d-CTA clusters: query %s, %d co-resident (need %d) -> using %d\n", want, cudaGetErrorString(qe), nclusters, kSpec, h->chol_cluster);
-        } else if (want >= 1 && want <= kCholCluster) {
-            h->chol_cluster = want;
-        }
-        cudaGetLastError();
     }
     *out = h;
     return OVS_OK;
@@ -4031,7 +3973,7 @@ extern "C" int ovs_graph_optimize_host(ovs_optimizer* h, int K, double* sim3_cw,
         if ((rc = ovs::grow_dev(&h->d_work, &h->w_cap, W.off)) != OVS_OK) return rc;
         W = Arena{h->d_work, 0};
         carve_work(W);
-        ds.fail = dfail; ds.clk = nullptr;
+        ds.fail = dfail;
     }
     memcpy(hS, sim3_cw, 104 * sK);
     memcpy(hfree, free_idx.data(), 4 * sK);

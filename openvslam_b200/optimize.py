@@ -258,14 +258,6 @@ class prepared_local_ba(_optimizer_handle):
         _lib.check(_lib.lib().ovs_local_ba_run(self._h, int(num_first_iter), int(num_second_iter), None, C.byref(st)))
         return _stats(st)
 
-    def cluster_width(self):
-        return int(_lib.lib().ovs_optimizer_cluster_width(self._h))
-
-    def debug_clocks(self):
-        out = np.zeros(192, np.int64)
-        _lib.check(_lib.lib().ovs_optimizer_debug_clocks(self._h, out.ctypes.data_as(C.c_void_p)))
-        return out
-
     def fetch(self):
         poses = np.zeros((self.K, 12)); points = np.zeros((self.L, 3)); out = np.zeros(self.M, np.uint8)
         _lib.check(_lib.lib().ovs_local_ba_fetch(self._h, poses.ctypes.data_as(C.c_void_p), points.ctypes.data_as(C.c_void_p),

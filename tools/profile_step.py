@@ -2,7 +2,6 @@
 """One hot-path step (extract, brute-force match, pose optimiser, local BA) to run under a profiler (e.g. torch.profiler).
 usage: python tools/profile_step.py [ba|extract|match|pose|all] [repeat]"""
 import os, sys
-import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from openvslam_b200 import feature, match, optimize, synth  # noqa: E402
@@ -34,19 +33,3 @@ if what in ("ba", "all"):
         print('run: trials', st['num_trials'], 'last_chi2', st['last_chi2'], 'chi2 of fetched state (inliers)',
               synth.reprojection_chi2(q['cam'], poses, points, q['obs_kf'], q['obs_lm'], q['obs_xy'], None, q['inv_sigma_sq'], ~outl), 'outliers', int(outl.sum()))
     print(st)
-    print('cholesky cluster width', ba.cluster_width())
-    clk = ba.debug_clocks()
-    import numpy as np
-    c = clk[:50].reshape(10, 5)
-    print('cholesky phase cycles per block step [panel load, panel solve, look-ahead (warp 0), barrier] and step totals:')
-    for b in range(10):
-        if c[b, 0] == 0: break
-        print(b, [int(c[b, k + 1] - c[b, k]) for k in range(4) if c[b, k + 1] > 0], int((c[b + 1, 0] if b < 9 and c[b + 1, 0] > 0 else clk[95]) - c[b, 0]))
-    print('total cycles', int(clk[95] - clk[0]))
-    print('look-ahead detail per step [tile update, factor loop]:', [(int(clk[168 + 2 * b] - c[b, 2]), int(clk[169 + 2 * b] - clk[168 + 2 * b])) for b in range(10) if clk[168 + 2 * b] > 0])
-    print('back-substitution: start->first block ready', int(clk[96] - clk[94]), 'per block [matvec, update, wait next]:',
-          [(int(clk[97 + 3 * j] - clk[96 + 3 * j]), int(clk[98 + 3 * j] - clk[97 + 3 * j]), int(clk[99 + 3 * j] - clk[98 + 3 * j]) if clk[99 + 3 * j] > 0 and j < 9 else 0) for j in range(10) if clk[96 + 3 * j] > 0])
-    for b in range(9):
-        q = clk[50 + 4 * b: 54 + 4 * b]
-        if q[0] == 0: break
-        print('tile0 of step', b, 'since panel solved', int(q[0] - c[b, 2]), 'loads', int(q[1] - q[0]), 'kloop', int(q[2] - q[1]), 'stores', int(q[3] - q[2]))
