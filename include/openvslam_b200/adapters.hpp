@@ -2,6 +2,8 @@
 // of openvslam_b200.hpp (which works on array views).  This is the binding a maintainer adds to the reference tree:
 //
 //   feature::orb_extractor::extract(const cv::_InputArray&, const cv::_InputArray&, std::vector<cv::KeyPoint>&, const cv::_OutputArray&)
+//   util::stereo_rectifier(camera, StereoRectifier block) and rectify(const cv::Mat&, const cv::Mat&, cv::Mat&, cv::Mat&) const
+//     (util/stereo_rectifier.h; the config / YAML parsing stays with the caller, which passes stereo_rectifier::params)
 //   match::robust::brute_force_match(data::frame&, data::keyframe*, std::vector<std::pair<int, int>>&)           (match/robust.h)
 //   match::projection::match_frame_and_landmarks(data::frame&, const std::vector<data::landmark*>&, float)      (match/projection.h)
 //   optimize::pose_optimizer::optimize(data::frame&)                                                             (optimize/pose_optimizer.h)
@@ -818,6 +820,27 @@ inline std::vector<Vec3_t> initialize::base::get_triangulated_pts() const {
 
 inline std::vector<bool> initialize::base::get_triangulated_flags() const {
     return std::vector<bool>(last_.is_triangulated.begin(), last_.is_triangulated.end());
+}
+
+template <class Camera>
+inline util::stereo_rectifier::stereo_rectifier(const Camera* camera, const params& p, const int device)
+    : stereo_rectifier(static_cast<int>(camera->cols_), static_cast<int>(camera->rows_),
+                       std::array<double, 9>{camera->fx_, 0.0, camera->cx_, 0.0, camera->fy_, camera->cy_, 0.0, 0.0, 1.0}, p, device) {}
+
+namespace adapters {
+// cv::Mat::channels(); a matrix type without it (the single-channel stand-in the tests compile against) has one channel
+template <class Mat>
+inline auto mat_channels(const Mat& m, int) -> decltype(m.channels()) { return m.channels(); }
+template <class Mat>
+inline int mat_channels(const Mat&, long) { return 1; }
+}  // namespace adapters
+
+inline void util::stereo_rectifier::rectify(const cv::Mat& in_img_l, const cv::Mat& in_img_r, cv::Mat& out_img_l, cv::Mat& out_img_r) const {
+    CV_Assert(in_img_l.rows == in_img_r.rows && in_img_l.cols == in_img_r.cols && in_img_l.type() == in_img_r.type());
+    CV_Assert(in_img_l.step == in_img_r.step);
+    cv::Mat l(in_img_l.rows, in_img_l.cols, in_img_l.type()), r(in_img_r.rows, in_img_r.cols, in_img_r.type());
+    rectify(in_img_l.data, in_img_r.data, in_img_l.rows, in_img_l.cols, in_img_l.step, adapters::mat_channels(in_img_l, 0), l.data, r.data, l.step);
+    out_img_l = l; out_img_r = r;
 }
 
 }  // namespace openvslam

@@ -2,6 +2,7 @@
 // libovs_b200.so (include/ovs_b200.h).  Header only.
 //
 //   openvslam::feature::orb_params / orb_extractor        (src/openvslam/feature/orb_params.h, orb_extractor.h)
+//   openvslam::util::stereo_rectifier                     (src/openvslam/util/stereo_rectifier.h)
 //   openvslam::match::robust / projection / area / stereo (src/openvslam/match/*.h)
 //   openvslam::optimize::pose_optimizer / local_bundle_adjuster / transform_optimizer / graph_optimizer (src/openvslam/optimize/*.h)
 //   openvslam::solve::sim3_solver                         (src/openvslam/solve/sim3_solver.h)
@@ -47,6 +48,64 @@ inline void check(int rc) {
     if (rc != OVS_OK) throw std::runtime_error(std::string("ovs_b200: ") + ovs_last_error());
 }
 }  // namespace detail
+
+namespace util {
+
+//! util::stereo_rectifier: the rectification maps of both cameras of a stereo rig, built once on the device from the
+//! StereoRectifier block (K_left, D_left, R_left, K_right, D_right, R_right, model) and the camera's cols, rows and K, the
+//! rectified camera matrix.  Matrices are row-major 3 x 3; D is {k1, k2, p1, p2, k3} (perspective) or {k1..k4} (fisheye).
+//! Immutable after construction: extractors on several threads may read one rectifier at once.
+class stereo_rectifier {
+public:
+    //! The parsed StereoRectifier block of the config.
+    struct params {
+        int model = OVS_CAMERA_PERSPECTIVE;   // OVS_CAMERA_PERSPECTIVE or OVS_CAMERA_FISHEYE
+        std::array<double, 9> K_left{}, R_left{}, K_right{}, R_right{};
+        std::vector<double> D_left, D_right;
+    };
+
+    stereo_rectifier(const int cols, const int rows, const std::array<double, 9>& K_rect, const params& p, const int device = 0) {
+        const std::size_t nd = p.model == OVS_CAMERA_FISHEYE ? 4 : 5;
+        if (p.D_left.size() != nd || p.D_right.size() != nd) throw std::runtime_error("stereo_rectifier: wrong number of distortion parameters");
+        detail::check(ovs_stereo_rectifier_create(device, p.model, cols, rows, p.K_left.data(), p.D_left.data(), p.R_left.data(), p.K_right.data(),
+                                                  p.D_right.data(), p.R_right.data(), K_rect.data(), &h_));
+        cols_ = cols; rows_ = rows;
+    }
+#ifdef OVS_B200_WITH_REFERENCE_TYPES
+    //! util::stereo_rectifier(camera, StereoRectifier block): K_rect is the camera's K (body in adapters.hpp)
+    template <class Camera>
+    stereo_rectifier(const Camera* camera, const params& p, const int device = 0);
+#endif
+    ~stereo_rectifier() { ovs_stereo_rectifier_destroy(h_); }
+    stereo_rectifier(const stereo_rectifier&) = delete;
+    stereo_rectifier& operator=(const stereo_rectifier&) = delete;
+
+    //! rectify(in_l, in_r, out_l, out_r) on u8 images with `channels` (1, 3, 4) interleaved channels; outputs keep them
+    void rectify(const std::uint8_t* in_l, const std::uint8_t* in_r, const int rows, const int cols, const std::size_t step, const int channels,
+                 std::uint8_t* out_l, std::uint8_t* out_r, const std::size_t out_step) const {
+        detail::check(ovs_stereo_rectify_host(h_, in_l, in_r, cols, rows, step, channels, out_l, out_r, out_step));
+    }
+#ifdef OVS_B200_WITH_OPENCV
+    //! The reference's signature.
+    void rectify(const cv::Mat& in_img_l, const cv::Mat& in_img_r, cv::Mat& out_img_l, cv::Mat& out_img_r) const;
+#endif
+
+    //! The float maps of side 0 (left) or 1 (right), rows x cols each, as cv::initUndistortRectifyMap returns them
+    void maps(const int side, std::vector<float>& map_x, std::vector<float>& map_y) const {
+        map_x.resize(static_cast<std::size_t>(rows_) * cols_); map_y.resize(map_x.size());
+        detail::check(ovs_stereo_rectifier_maps(h_, side, map_x.data(), map_y.data()));
+    }
+
+    int cols() const { return cols_; }
+    int rows() const { return rows_; }
+    ovs_stereo_rectifier* handle() const { return h_; }
+
+private:
+    ovs_stereo_rectifier* h_ = nullptr;
+    int cols_ = 0, rows_ = 0;
+};
+
+}  // namespace util
 
 namespace feature {
 
@@ -119,6 +178,21 @@ public:
         int n = 0;
         detail::check(ovs_extract_host_color(h_, image, cols, rows, step, channels, color_order, mask, mask_step, keypts.data(), descriptors.data(),
                                              cap, &n));
+        keypts.resize(n); descriptors.resize(static_cast<std::size_t>(n) * 32);
+    }
+
+    //! rectifier.rectify() of one side (0 left, 1 right), util::convert_to_grayscale and extract() in one call: the raw image
+    //! (1, 3 or 4 channels; color_order as extract_color) is rectified on the device straight into the pyramid.  The mask is in
+    //! rectified coordinates.  The stereo frame's two extractors may run this on two threads with one rectifier.
+    void extract(const util::stereo_rectifier& rectifier, const int side, const std::uint8_t* image, const int rows, const int cols,
+                 const std::size_t step, const int channels, const int color_order, const std::uint8_t* mask, const std::size_t mask_step,
+                 std::vector<ovs_keypoint>& keypts, std::vector<std::uint8_t>& descriptors) {
+        keypts.clear(); descriptors.clear();
+        const int cap = ovs_extractor_max_keypoints(h_);
+        keypts.resize(cap); descriptors.resize(static_cast<std::size_t>(cap) * 32);
+        int n = 0;
+        detail::check(ovs_extract_host_rectified(h_, rectifier.handle(), side, image, cols, rows, step, channels, color_order, mask, mask_step,
+                                                 keypts.data(), descriptors.data(), cap, &n));
         keypts.resize(n); descriptors.resize(static_cast<std::size_t>(n) * 32);
     }
 

@@ -51,6 +51,9 @@ uint64_t ovs_kernel_launch_count(void);
  * sched_yield() -- near-spin latency while cores are free, fair sharing once host threads outnumber cores.
  * Process-wide; call it before creating the handles it should apply to. */
 int ovs_set_wait_mode(int mode);
+/* Number of times the calling process's threads have waited inside this library for the device to finish (stream or event
+ * synchronisations), so far. */
+uint64_t ovs_host_wait_count(void);
 
 /* ------------------------------------------------------------------ feature::orb_extractor */
 
@@ -127,6 +130,38 @@ int ovs_extractor_debug_candidates(ovs_extractor* h, int level, int32_t* xys_out
  * [0] upload [1] pyramid [2] fast score [3] cell nms+compact [4] host tree distribution (wall)
  * [5] orientation+descriptor [6] download [7] total wall. */
 int ovs_extractor_last_timings(const ovs_extractor* h, float* out_us /* [8] */);
+
+/* ------------------------------------------------------------------------- util::stereo_rectifier */
+
+typedef struct ovs_stereo_rectifier ovs_stereo_rectifier;
+
+/* util::stereo_rectifier(camera, StereoRectifier params): the rectification maps of both cameras of a stereo rig, as
+ * cv::initUndistortRectifyMap (model OVS_CAMERA_PERSPECTIVE, dist = k1, k2, p1, p2, k3) or cv::fisheye::initUndistortRectifyMap
+ * (OVS_CAMERA_FISHEYE, dist = k1..k4) build them with CV_32FC1 maps, for cols x rows images (1 .. 32767 each).  K_*, R_* and
+ * K_rect are row-major 3 x 3; K_rect is the rectified camera matrix (the camera's own K).  The maps are built on `device`
+ * (float64, evaluated as OpenCV writes it; the fisheye model's atan is within an ulp of the host's) and the handle is
+ * immutable once create returns, so any number of threads may read it at once.  A singular K_rect R, an unknown model or
+ * a null array return OVS_ERR_INVALID_ARG. */
+int ovs_stereo_rectifier_create(int device, int model, int cols, int rows, const double* K_l, const double* D_l, const double* R_l,
+                                const double* K_r, const double* D_r, const double* R_r, const double* K_rect,
+                                ovs_stereo_rectifier** out);
+void ovs_stereo_rectifier_destroy(ovs_stereo_rectifier* h);
+/* The float maps of side 0 (left) or 1 (right): map_x[rows * cols], map_y[rows * cols], host buffers. */
+int ovs_stereo_rectifier_maps(const ovs_stereo_rectifier* h, int side, float* map_x, float* map_y);
+/* util::stereo_rectifier::rectify(in_l, in_r, out_l, out_r): cv::remap(INTER_LINEAR, BORDER_CONSTANT 0) of both u8 images
+ * (1, 3 or 4 interleaved channels, `pitch` bytes per row) through their maps, bit-exact with OpenCV 4; the outputs have the
+ * input's channels, `out_pitch` bytes per row.  Calls on one handle from several threads run one after the other. */
+int ovs_stereo_rectify_host(ovs_stereo_rectifier* h, const uint8_t* left, const uint8_t* right, int width, int height, size_t pitch,
+                            int channels, uint8_t* out_left, uint8_t* out_right, size_t out_pitch);
+/* rectify one side, util::convert_to_grayscale (color_order as ovs_extract_host_color; ignored for 1 channel) and
+ * orb_extractor::extract in one call: the raw image is uploaded and remapped straight into level 0 of the pyramid, with one
+ * host synchronisation.  The mask is in rectified coordinates.  Call it per side on the stereo frame's two extractors, from
+ * two threads if wanted: both may read one rectifier at once.  An image whose size differs from the rectifier's, channels
+ * other than 1 / 3 / 4, side outside {0, 1}, a null pointer, or a rectifier on another device than the extractor return
+ * OVS_ERR_INVALID_ARG before any launch. */
+int ovs_extract_host_rectified(ovs_extractor* h, const ovs_stereo_rectifier* rectifier, int side, const uint8_t* image, int width,
+                               int height, size_t pitch, int channels, int color_order, const uint8_t* mask, size_t mask_pitch,
+                               ovs_keypoint* keypts_out, uint8_t* descriptors_out, int capacity, int* num_out);
 
 /* ------------------------------------------------------------------------------- match::* */
 

@@ -33,6 +33,7 @@
 
 #include "orb_math.cuh"
 #include "ovs_common.h"
+#include "stereo_rectify.h"
 
 namespace {
 
@@ -1071,7 +1072,7 @@ struct ovs_extractor {
     uint8_t* d_mask_call = nullptr;   // a caller's mask of the current call
     bool last_masked = false;
     uint8_t* h_img = nullptr;         // pinned staging for pageable input
-    uint8_t* h_color = nullptr; uint8_t* d_color = nullptr; size_t color_bytes = 0;   // colour input staging (extract_host_color)
+    ovs::HostUpload color;            // colour / raw stereo input staging (extract_host_color, extract_host_rectified)
     uint8_t* d_und = nullptr; size_t und_bytes = 0;                                   // scratch of ovs_undistort_keypoints_host
     size_t h_img_bytes = 0;
 
@@ -1494,6 +1495,32 @@ int collect_timings(ovs_extractor* h, std::chrono::steady_clock::time_point t_be
     return OVS_OK;
 }
 
+// The host entries once level 0 has been queued on the handle's stream: the pipeline, the copies of what the caller can take,
+// one host wait, the verdict and the outputs.
+int extract_to_host(ovs_extractor* h, const uint8_t* mask, size_t mask_pitch, ovs_keypoint* keypts_out, uint8_t* descriptors_out,
+                    int capacity, int* num_out, std::chrono::steady_clock::time_point t_begin) {
+    cudaStream_t st = h->stream;
+    OVS_CUDA_CHECK(cudaEventRecord(h->ev[1], st));
+    // the number of keypoints is known to the device only: the copies cover what the caller can take
+    const int bound = std::min(capacity, h->max_out);
+    int rc = run_pipeline(h, mask, mask_pitch, h->d_kps, h->d_desc, bound);
+    if (rc != OVS_OK) return rc;
+    if (bound) {
+        OVS_CUDA_CHECK(cudaMemcpyAsync(h->h_kps, h->d_kps, (size_t)bound * sizeof(ovs_keypoint), cudaMemcpyDeviceToHost, st));
+        OVS_CUDA_CHECK(cudaMemcpyAsync(h->h_desc, h->d_desc, (size_t)bound * 32, cudaMemcpyDeviceToHost, st));
+    }
+    OVS_CUDA_CHECK(cudaEventRecord(h->ev[7], st));
+    OVS_CUDA_CHECK(ovs::sync_event(h->ev[7]));
+    rc = finish_pipeline(h, bound, num_out);
+    if (rc != OVS_OK) return rc;
+    const int n = *num_out;
+    if (n) {
+        memcpy(keypts_out, h->h_kps, (size_t)n * sizeof(ovs_keypoint));
+        memcpy(descriptors_out, h->h_desc, (size_t)n * 32);
+    }
+    return collect_timings(h, t_begin);
+}
+
 }  // namespace
 
 // ================================================================================ C ABI
@@ -1577,7 +1604,7 @@ extern "C" void ovs_extractor_destroy(ovs_extractor* h) {
     if (h->stream) ovs::sync_stream(h->stream);
     free_geometry(h);
     cudaFree(h->d_status); cudaFreeHost(h->h_status);
-    cudaFreeHost(h->h_color); cudaFree(h->d_color); cudaFree(h->d_und);
+    ovs::free_upload(h->color); cudaFree(h->d_und);
     cudaFree(h->d_kps); cudaFree(h->d_desc);
     cudaFreeHost(h->h_kps); cudaFreeHost(h->h_desc);
     for (auto& e : h->ev) if (e) cudaEventDestroy(e);
@@ -1609,25 +1636,7 @@ extern "C" int ovs_extract_host(ovs_extractor* h, const uint8_t* image, int widt
         for (int y = 0; y < height; ++y) memcpy(h->h_img + (size_t)y * width, image + (size_t)y * pitch, width);
         OVS_CUDA_CHECK(cudaMemcpy2DAsync(h->d_pyr, h->T.pitch[0], h->h_img, width, width, height, cudaMemcpyHostToDevice, st));
     }
-    OVS_CUDA_CHECK(cudaEventRecord(h->ev[1], st));
-    // the number of keypoints is known to the device only: the copies cover what the caller can take
-    const int bound = std::min(capacity, h->max_out);
-    rc = run_pipeline(h, mask, mask_pitch, h->d_kps, h->d_desc, bound);
-    if (rc != OVS_OK) return rc;
-    if (bound) {
-        OVS_CUDA_CHECK(cudaMemcpyAsync(h->h_kps, h->d_kps, (size_t)bound * sizeof(ovs_keypoint), cudaMemcpyDeviceToHost, st));
-        OVS_CUDA_CHECK(cudaMemcpyAsync(h->h_desc, h->d_desc, (size_t)bound * 32, cudaMemcpyDeviceToHost, st));
-    }
-    OVS_CUDA_CHECK(cudaEventRecord(h->ev[7], st));
-    OVS_CUDA_CHECK(ovs::sync_event(h->ev[7]));
-    rc = finish_pipeline(h, bound, num_out);
-    if (rc != OVS_OK) return rc;
-    const int n = *num_out;
-    if (n) {
-        memcpy(keypts_out, h->h_kps, (size_t)n * sizeof(ovs_keypoint));
-        memcpy(descriptors_out, h->h_desc, (size_t)n * 32);
-    }
-    return collect_timings(h, t_begin);
+    return extract_to_host(h, mask, mask_pitch, keypts_out, descriptors_out, capacity, num_out, t_begin);
 }
 
 // camera->undistort_keypoints + camera->convert_keypoints_to_bearings on DEVICE arrays (the extractor's device output);
@@ -1699,45 +1708,48 @@ extern "C" int ovs_extract_host_color(ovs_extractor* h, const uint8_t* image, in
     int rc = configure(h, width, height);
     if (rc != OVS_OK) return rc;
     cudaStream_t st = h->stream;
-    const size_t row = (size_t)width * channels, need = row * height;
-    if (need > h->color_bytes) {
-        cudaFreeHost(h->h_color); cudaFree(h->d_color); h->h_color = nullptr; h->d_color = nullptr; h->color_bytes = 0;
-        OVS_CUDA_CHECK(cudaHostAlloc(&h->h_color, need, cudaHostAllocDefault));
-        OVS_CUDA_CHECK(cudaMalloc(&h->d_color, need));
-        h->color_bytes = need;
-    }
+    const size_t row = (size_t)width * channels;
+    rc = ovs::reserve_upload(h->color, row * height);
+    if (rc != OVS_OK) return rc;
     OVS_CUDA_CHECK(cudaEventRecord(h->ev[0], st));
-    cudaPointerAttributes attr;
-    const bool pinned = cudaPointerGetAttributes(&attr, image) == cudaSuccess && attr.type == cudaMemoryTypeHost;
-    cudaGetLastError();
-    if (pinned) {
-        OVS_CUDA_CHECK(cudaMemcpy2DAsync(h->d_color, row, image, pitch, row, height, cudaMemcpyHostToDevice, st));
-    } else {
-        for (int y = 0; y < height; ++y) memcpy(h->h_color + (size_t)y * row, image + (size_t)y * pitch, row);
-        OVS_CUDA_CHECK(cudaMemcpyAsync(h->d_color, h->h_color, need, cudaMemcpyHostToDevice, st));
-    }
-    k_color_to_gray<<<dim3((width + 1023) / 1024, height), 256, 0, st>>>(h->d_color, row, width, height, channels, color_order == OVS_COLOR_ORDER_RGB,
+    rc = ovs::upload_image(h->color, image, pitch, row, height, st);
+    if (rc != OVS_OK) return rc;
+    k_color_to_gray<<<dim3((width + 1023) / 1024, height), 256, 0, st>>>(h->color.d, row, width, height, channels, color_order == OVS_COLOR_ORDER_RGB,
                                                                        h->d_pyr, h->T.pitch[0]);
     OVS_LAUNCH_CHECK();
-    OVS_CUDA_CHECK(cudaEventRecord(h->ev[1], st));
-    // the number of keypoints is known to the device only: the copies cover what the caller can take
-    const int bound = std::min(capacity, h->max_out);
-    rc = run_pipeline(h, mask, mask_pitch, h->d_kps, h->d_desc, bound);
+    return extract_to_host(h, mask, mask_pitch, keypts_out, descriptors_out, capacity, num_out, t_begin);
+}
+
+// util::stereo_rectifier::rectify of one side, util::convert_to_grayscale and extract(): the raw image is uploaded as it is
+// and remapped (and reduced to gray) on the device, straight into level 0 of the pyramid.  The rectifier is only read.
+extern "C" int ovs_extract_host_rectified(ovs_extractor* h, const ovs_stereo_rectifier* rectifier, int side, const uint8_t* image, int width,
+                                          int height, size_t pitch, int channels, int color_order, const uint8_t* mask, size_t mask_pitch,
+                                          ovs_keypoint* keypts_out, uint8_t* descriptors_out, int capacity, int* num_out) {
+    OVS_REQUIRE(h && rectifier && image && num_out && (capacity == 0 || (keypts_out && descriptors_out)), OVS_ERR_INVALID_ARG, "null argument");
+    OVS_REQUIRE(side == 0 || side == 1, OVS_ERR_INVALID_ARG, "side must be 0 (left) or 1 (right), got %d", side);
+    OVS_REQUIRE(channels == 1 || channels == 3 || channels == 4, OVS_ERR_INVALID_ARG, "images have 1, 3 or 4 channels (got %d)", channels);
+    OVS_REQUIRE(color_order == OVS_COLOR_ORDER_BGR || color_order == OVS_COLOR_ORDER_RGB, OVS_ERR_INVALID_ARG, "bad colour order");
+    OVS_REQUIRE(rectifier->device == h->device, OVS_ERR_INVALID_ARG, "rectifier on device %d, extractor on device %d", rectifier->device,
+                h->device);
+    OVS_REQUIRE(width == rectifier->cols && height == rectifier->rows, OVS_ERR_INVALID_ARG, "image %dx%d differs from the rectifier's %dx%d",
+                width, height, rectifier->cols, rectifier->rows);
+    OVS_REQUIRE(pitch >= (size_t)width * channels, OVS_ERR_INVALID_ARG, "bad image geometry");
+    OVS_REQUIRE(!mask || mask_pitch >= (size_t)width, OVS_ERR_INVALID_ARG, "bad mask pitch");
+    const auto t_begin = std::chrono::steady_clock::now();
+    OVS_CUDA_CHECK(cudaSetDevice(h->device));
+    int rc = configure(h, width, height);
     if (rc != OVS_OK) return rc;
-    if (bound) {
-        OVS_CUDA_CHECK(cudaMemcpyAsync(h->h_kps, h->d_kps, (size_t)bound * sizeof(ovs_keypoint), cudaMemcpyDeviceToHost, st));
-        OVS_CUDA_CHECK(cudaMemcpyAsync(h->h_desc, h->d_desc, (size_t)bound * 32, cudaMemcpyDeviceToHost, st));
-    }
-    OVS_CUDA_CHECK(cudaEventRecord(h->ev[7], st));
-    OVS_CUDA_CHECK(ovs::sync_event(h->ev[7]));
-    rc = finish_pipeline(h, bound, num_out);
+    cudaStream_t st = h->stream;
+    const size_t row = (size_t)width * channels;
+    rc = ovs::reserve_upload(h->color, row * height);
     if (rc != OVS_OK) return rc;
-    const int n = *num_out;
-    if (n) {
-        memcpy(keypts_out, h->h_kps, (size_t)n * sizeof(ovs_keypoint));
-        memcpy(descriptors_out, h->h_desc, (size_t)n * 32);
-    }
-    return collect_timings(h, t_begin);
+    OVS_CUDA_CHECK(cudaEventRecord(h->ev[0], st));
+    rc = ovs::upload_image(h->color, image, pitch, row, height, st);
+    if (rc == OVS_OK)
+        rc = ovs::launch_stereo_remap(rectifier, side, h->color.d, row, channels, 1, color_order == OVS_COLOR_ORDER_RGB, h->d_pyr,
+                                      h->T.pitch[0], st);
+    if (rc != OVS_OK) return rc;
+    return extract_to_host(h, mask, mask_pitch, keypts_out, descriptors_out, capacity, num_out, t_begin);
 }
 
 extern "C" int ovs_extract_device(ovs_extractor* h, const uint8_t* d_image, int width, int height, size_t pitch,

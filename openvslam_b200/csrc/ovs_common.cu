@@ -20,10 +20,12 @@ void set_error(const char* fmt, ...) {
 void count_launch(int n) { g_launches.fetch_add((uint64_t)n, std::memory_order_relaxed); }
 
 static std::atomic<int> g_blocking{0};
+alignas(64) static std::atomic<uint64_t> g_waits{0};   // its own cache line: every host wait of every thread writes it
 bool blocking_waits() { return g_blocking.load(std::memory_order_relaxed) == 1; }
 unsigned event_flags() { return blocking_waits() ? (unsigned)cudaEventBlockingSync : (unsigned)cudaEventDefault; }
 
 cudaError_t sync_event(cudaEvent_t ev) {
+    g_waits.fetch_add(1, std::memory_order_relaxed);
     if (g_blocking.load(std::memory_order_relaxed) != 2) return cudaEventSynchronize(ev);
     cudaError_t q;
     while ((q = cudaEventQuery(ev)) == cudaErrorNotReady) sched_yield();
@@ -31,6 +33,7 @@ cudaError_t sync_event(cudaEvent_t ev) {
 }
 
 cudaError_t sync_stream(cudaStream_t st) {
+    g_waits.fetch_add(1, std::memory_order_relaxed);
     const int mode = g_blocking.load(std::memory_order_relaxed);
     if (mode == 0) return cudaStreamSynchronize(st);
     if (mode == 2) {
@@ -82,4 +85,5 @@ int select_device(int device) {
 extern "C" const char* ovs_last_error(void) { return ovs::g_err; }
 extern "C" const char* ovs_version(void) { return "ovs_b200 0.1 sm_90a"; }
 extern "C" uint64_t ovs_kernel_launch_count(void) { return ovs::g_launches.load(); }
+extern "C" uint64_t ovs_host_wait_count(void) { return ovs::g_waits.load(); }
 extern "C" int ovs_set_wait_mode(int mode) { ovs::g_blocking.store(mode == 1 ? 1 : mode == 2 ? 2 : 0); return OVS_OK; }

@@ -63,13 +63,18 @@ class orb_extractor:
             pass
 
     # -- orb_extractor::extract(in_image, in_image_mask, keypts, out_descriptors)
-    def extract(self, image, mask=None, color_order="BGR"):
-        """image: H x W (gray) or H x W x {3, 4} u8 (colour: converted like util::convert_to_grayscale with `color_order`)."""
+    def extract(self, image, mask=None, color_order="BGR", rectifier=None, side=0):
+        """image: H x W (gray) or H x W x {3, 4} u8 (colour: converted like util::convert_to_grayscale with `color_order`).
+        rectifier: a util.stereo_rectifier; the raw image of `side` (0 left, 1 right) is rectified on the device first, as
+        util::stereo_rectifier::rectify does before the stereo frame is built.  The mask is in rectified coordinates."""
         image = np.asarray(image)
         if image.size == 0:
             return np.zeros(0, KEYPOINT_DTYPE), np.zeros((0, 32), np.uint8)
         color = image.ndim == 3
-        if color:
+        if rectifier is not None:
+            assert image.dtype == np.uint8 and (image.ndim == 2 or image.shape[2] in (1, 3, 4)), "image must be CV_8UC1 / 3 / 4"
+            image = np.ascontiguousarray(image)
+        elif color:
             assert image.dtype == np.uint8 and image.shape[2] in (3, 4), "colour image must be CV_8UC3 / CV_8UC4"
             image = np.ascontiguousarray(image)
         else:
@@ -86,6 +91,13 @@ class orb_extractor:
         n = C.c_int(0)
 
         def call():
+            if rectifier is not None:
+                return _lib.lib().ovs_extract_host_rectified(self._h, rectifier.handle, int(side), image.ctypes.data_as(C.c_void_p),
+                                                             image.shape[1], image.shape[0], C.c_size_t(image.strides[0]),
+                                                             1 if image.ndim == 2 else image.shape[2],
+                                                             1 if color_order.upper().startswith("RGB") else 0, mp, C.c_size_t(ms),
+                                                             self._kps.ctypes.data_as(C.c_void_p), self._desc.ctypes.data_as(C.c_void_p),
+                                                             self._cap, C.byref(n))
             if color:
                 return _lib.lib().ovs_extract_host_color(self._h, image.ctypes.data_as(C.c_void_p), image.shape[1], image.shape[0],
                                                          C.c_size_t(image.strides[0]), image.shape[2], 1 if color_order.upper().startswith("RGB") else 0,
