@@ -188,7 +188,8 @@ __global__ void __launch_bounds__(128) k_stereo_match(StereoArgs A, unsigned* __
     if (act) { x_left = A.lx[il]; y_left = A.ly[il]; lvl = A.loct[il]; qa = __ldg(A.ldesc + 2 * (size_t)il); qb = __ldg(A.ldesc + 2 * (size_t)il + 1); }
     const int row = (int)y_left;
     const float min_x_right = __fsub_rn(x_left, A.max_disp), max_x_right = __fsub_rn(x_left, A.min_disp);
-    const bool usable = act && row >= 0 && row < A.rows0 && !(max_x_right < 0);
+    // a keypoint with a coordinate that is not finite takes no part (the reference's conversions are undefined there)
+    const bool usable = act && isfinite(x_left) && isfinite(y_left) && row >= 0 && row < A.rows0 && !(max_x_right < 0);
     unsigned best = ((unsigned)A.hamm_thr << 16) | 0xffffu;   // sentinel: distance == threshold
     for (int t0 = 0; t0 < A.n_right; t0 += 256) {
         const int n = min(256, A.n_right - t0);
@@ -199,7 +200,8 @@ __global__ void __launch_bounds__(128) k_stereo_match(StereoArgs A, unsigned* __
             const float r = __fmul_rn(2.0f, A.scale[o]);
             const float yy = A.ry[ir];
             s_rx[i] = A.rx[ir]; s_oct[i] = o;
-            s_lo[i] = (float)cv_floor_f(__fsub_rn(yy, r)); s_hi[i] = (float)cv_ceil_f(__fadd_rn(yy, r));
+            const bool finite = isfinite(yy) && isfinite(A.rx[ir]);   // else an empty band: no candidate
+            s_lo[i] = finite ? (float)cv_floor_f(__fsub_rn(yy, r)) : INFINITY; s_hi[i] = finite ? (float)cv_ceil_f(__fadd_rn(yy, r)) : -INFINITY;
             s_desc[2 * i] = __ldg(A.rdesc + 2 * (size_t)ir); s_desc[2 * i + 1] = __ldg(A.rdesc + 2 * (size_t)ir + 1);
         }
         __syncthreads();
@@ -237,8 +239,9 @@ __global__ void __launch_bounds__(128) k_stereo_subpixel(StereoArgs A, const uns
         const int sxr = __float2int_rn(__fmul_rn(A.rx[ir], inv_s));
         constexpr int win = 5, slide = 5;
         const int W = A.pw[lvl], Hh = A.ph[lvl], S = A.pitch[lvl];
-        const int ini_x = sxr - slide - win, end_x = sxr + slide + win + 1;
-        const bool fits = !(ini_x < 0 || W <= end_x) && !(sxl - win < 0 || W <= sxl + win || syl - win < 0 || Hh <= syl + win);
+        // ini_x = sxr - slide - win >= 0, end_x = sxr + slide + win + 1 < W and the left window, without overflow: the
+        // conversions saturate, so a coordinate past the int range lands outside every window
+        const bool fits = !(sxr < slide + win || W - (slide + win + 1) <= sxr) && !(sxl < win || W - win <= sxl || syl < win || Hh - win <= syl);
         if (fits) {
             const uint8_t* L = A.lpyr[lvl]; const uint8_t* R = A.rpyr[lvl];
             const int cl = L[(size_t)syl * S + sxl];

@@ -584,6 +584,15 @@ int om_area_match_in_consistent_area(const om_frame* f1, const om_frame* f2, flo
 }
 
 /* match::stereo::compute */
+/* cvRound for the SAD window origins, saturating like the kernel's __float2int_rn: a coordinate past the int range lands
+ * outside every window instead of wrapping into one. */
+static int round_sat(float v) {
+    if (v != v) return 0;
+    if (v >= 2147483648.f) return INT_MAX;
+    if (v < -2147483648.f) return INT_MIN;
+    return (int)lrintf(v);
+}
+
 typedef struct { unsigned corr; int idx; } corr_idx;
 static int corr_cmp(const void* a, const void* b) {
     const corr_idx* A = (const corr_idx*)a; const corr_idx* B = (const corr_idx*)b;
@@ -605,12 +614,15 @@ int om_stereo_compute(const uint8_t* const* left_pyr, const uint8_t* const* righ
     for (int il = 0; il < n_left; ++il) {
         const int lvl = loct[il];
         const float y_left = ly[il], x_left = lx[il];
+        /* a keypoint with a coordinate that is not finite takes no part (the reference's conversions are undefined there) */
+        if (!isfinite(x_left) || !isfinite(y_left)) continue;
+        if (!(-1.0f < y_left && y_left < (float)rows0)) continue;
         const int row = (int)y_left;   /* indices_right_in_row.at(y_left) */
-        if (row < 0 || row >= rows0) continue;
         const float min_x_right = x_left - max_disp, max_x_right = x_left - min_disp;
         if (max_x_right < 0) continue;
         unsigned best_dist = hamm_dist_thr; int best_ir = 0; int any = 0;
         for (int ir = 0; ir < n_right; ++ir) {
+            if (!isfinite(rx[ir]) || !isfinite(ry[ir])) continue;
             /* get_right_keypoint_indices_in_each_row(2.0): rows [floor(y - r), ceil(y + r)] */
             const float r = 2.0f * scale_factors[roct[ir]];
             const int max_r = cv_ceil(ry[ir] + r), min_r = cv_floor(ry[ir] - r);
@@ -625,12 +637,12 @@ int om_stereo_compute(const uint8_t* const* left_pyr, const uint8_t* const* righ
         if (hamm_dist_thr <= best_dist) continue;
         /* compute_subpixel_disparity */
         const float inv_s = inv_scale_factors[lvl];
-        const int sxl = cv_round_f(x_left * inv_s), syl = cv_round_f(y_left * inv_s), sxr = cv_round_f(rx[best_ir] * inv_s);
+        const int sxl = round_sat(x_left * inv_s), syl = round_sat(y_left * inv_s), sxr = round_sat(rx[best_ir] * inv_s);
         enum { win = 5, slide = 5 };
         const int W = pyr_w[lvl], Hh = pyr_h[lvl], S = pyr_stride[lvl];
-        const int ini_x = sxr - slide - win, end_x = sxr + slide + win + 1;
-        if (ini_x < 0 || W <= end_x) continue;
-        if (sxl - win < 0 || W <= sxl + win || syl - win < 0 || Hh <= syl + win) continue;
+        /* ini_x = sxr - slide - win < 0 || W <= end_x = sxr + slide + win + 1, and the left window, without overflow */
+        if (sxr < slide + win || W - (slide + win + 1) <= sxr) continue;
+        if (sxl < win || W - win <= sxl || syl < win || Hh - win <= syl) continue;
         const uint8_t* Limg = left_pyr[lvl]; const uint8_t* Rimg = right_pyr[lvl];
         const int cl = Limg[(size_t)syl * S + sxl];
         unsigned best_corr = UINT_MAX; int best_off = 0; float corrs[2 * slide + 1];
