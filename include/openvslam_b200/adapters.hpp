@@ -28,6 +28,9 @@
 //   match::projection::match_current_and_last_frames(data::frame&, const data::frame&, float)                   (match/projection.h)
 //   the body of tracking_module::search_local_landmarks over data::frame and data::landmark, as adapters::search_local_landmarks
 //     (both templates deduced from their arguments; tests/cpp/test_tracking_search.cpp runs them on the GPU)
+//   match::fuse::replace_duplication(data::keyframe*, const T&, float)                                          (match/fuse.h)
+//   the body of mapping_module::fuse_landmark_duplication (module/mapping_module.cc), as adapters::fuse_landmark_duplication
+//     (both templates deduced from their arguments; tests/cpp/test_fuse.cpp runs them on the GPU)
 //
 // Include it INSTEAD of openvslam_b200.hpp in a translation unit that can see the reference's headers (here: the stand-ins
 // under tests/cpp/standin, which declare the members used below with the names recalled in SURVEY.md section 2 / 8b;
@@ -48,6 +51,8 @@
 #include <cstring>
 #include <map>
 #include <mutex>
+#include <type_traits>
+#include <unordered_set>
 #include <utility>
 #include <vector>
 
@@ -350,6 +355,211 @@ inline unsigned int match::projection::match_current_and_last_frames(Frame& curr
         if (matched[i] >= 0) curr_frm.landmarks_.at(i) = last_frm.landmarks_.at(static_cast<std::size_t>(matched[i]));
     return num;
 }
+
+// ------------------------------------------------------------------------------------------------------- match::fuse
+namespace adapters {
+
+// The fuse adapters are templates deduced from their arguments (data::keyframe / data::landmark in the reference tree), like the
+// tracking adapters above.
+//
+// replace_duplication(keyfrm, landmarks_to_check, margin) runs its geometry and search on the device and replays its data-model
+// updates on the host, in the container's order, with the reference's live skips (no landmark, will_be_erased(),
+// is_observed_in_keyframe(keyfrm)).  That replay is exact with one device call per target because a query's answer depends only on
+// the landmark's position, mean normal, valid distances and descriptor and on the target's own arrays, and the only update that
+// changes any of these is landmark::replace, through other->compute_descriptor() on the survivor.  Within one target the survivor
+// of a replace is either the query's own landmark, which the container does not hold twice, or the landmark already in the
+// target's keypoint, which is observed in the target and so skipped by every later query of it.  So no descriptor changes under a
+// later query of the same target.  Across targets it can: fuse_landmark_duplication keeps the set of landmarks that survived a
+// replace since its snapshot and, before replaying each target, re-queries that target's queries on such landmarks, in one call,
+// with their current descriptors.
+
+//! What replace_duplication reads of a keyframe, as an ovs_fuse_target over copies owned here: camera_, img_bounds_,
+//! get_cam_pose(), get_cam_center(), num_scale_levels_, log_scale_factor_, scale_factors_, inv_level_sigma_sq_, undist_keypts_,
+//! stereo_x_right_, descriptors_ and the camera's grid.
+struct fuse_target_arrays {
+    frame_arrays arrays;
+    ovs_fuse_target target{};
+    template <class Keyframe>
+    explicit fuse_target_arrays(const Keyframe& keyfrm) : arrays(keyfrm) {
+        ovs_frame_geometry& g = target.geometry;
+        g.camera = to_camera(keyfrm.camera_);
+        const camera::image_bounds& b = keyfrm.camera_->img_bounds_;
+        g.min_x = b.min_x_; g.max_x = b.max_x_; g.min_y = b.min_y_; g.max_y = b.max_y_;
+        double pose12[12];
+        to_Rt(keyfrm.get_cam_pose(), pose12);
+        for (int k = 0; k < 9; ++k) g.rot_cw[k] = pose12[k];
+        for (int k = 0; k < 3; ++k) g.trans_cw[k] = pose12[9 + k];
+        const Vec3_t c = keyfrm.get_cam_center();
+        for (int k = 0; k < 3; ++k) g.cam_center[k] = c(k);
+        g.num_scale_levels = static_cast<std::int32_t>(keyfrm.num_scale_levels_);
+        g.log_scale_factor = keyfrm.log_scale_factor_;
+        target.scale_factors = keyfrm.scale_factors_.data();
+        target.inv_level_sigma_sq = keyfrm.inv_level_sigma_sq_.data();
+        const match::frame_view& v = arrays.view;
+        target.num_keypts = v.num_keypts; target.x = v.x; target.y = v.y; target.octave = v.octave; target.x_right = v.stereo_x_right;
+        target.descriptors = v.descriptors; target.grid = v.grid;
+    }
+};
+
+//! The landmark table of a fuse call: one row per landmark added, read through get_pos_in_world(), get_obs_mean_normal(),
+//! get_unscaled_valid_distances() and get_descriptor().
+template <class Landmark>
+struct fuse_landmark_rows {
+    std::vector<Landmark*> lms;
+    std::vector<double> pos, nrm;
+    std::vector<float> lo, hi;
+    std::vector<std::uint8_t> desc;
+    int add(Landmark* lm) {
+        const Vec3_t p = lm->get_pos_in_world(), n = lm->get_obs_mean_normal();
+        for (int k = 0; k < 3; ++k) { pos.push_back(p(k)); nrm.push_back(n(k)); }
+        const std::pair<float, float> d = lm->get_unscaled_valid_distances();
+        lo.push_back(d.first); hi.push_back(d.second);
+        desc.resize(desc.size() + 32);
+        lms.push_back(lm);
+        refresh_descriptor(static_cast<int>(lms.size()) - 1);
+        return static_cast<int>(lms.size()) - 1;
+    }
+    void refresh_descriptor(const int row) {
+        const cv::Mat d = lms[static_cast<std::size_t>(row)]->get_descriptor();
+        std::memcpy(&desc[32 * static_cast<std::size_t>(row)], d.data, 32);
+    }
+    match::fuse::landmark_table table() const {
+        match::fuse::landmark_table t;
+        t.num_landmarks = static_cast<int>(lms.size());
+        t.pos_w = pos.data(); t.mean_normal = nrm.data(); t.min_valid_dist = lo.data(); t.max_valid_dist = hi.data(); t.descriptors = desc.data();
+        return t;
+    }
+};
+
+//! The reference's update for one query of replace_duplication that found best_idx in keyfrm; a replace's survivor goes into
+//! `changed` (its descriptor was recomputed).
+template <class Keyframe, class Landmark>
+void fuse_into_keyframe(Keyframe* keyfrm, Landmark* lm, const int best_idx, std::unordered_set<Landmark*>& changed) {
+    auto* lm_in_keyfrm = keyfrm->get_landmark(static_cast<unsigned int>(best_idx));
+    if (lm_in_keyfrm) {
+        if (!lm_in_keyfrm->will_be_erased()) {
+            if (lm->num_observations() < lm_in_keyfrm->num_observations()) {
+                lm->replace(lm_in_keyfrm);
+                changed.insert(lm_in_keyfrm);
+            } else {
+                lm_in_keyfrm->replace(lm);
+                changed.insert(lm);
+            }
+        }
+    } else {
+        lm->add_observation(keyfrm, static_cast<unsigned int>(best_idx));
+        keyfrm->add_landmark(lm, static_cast<unsigned int>(best_idx));
+    }
+}
+
+template <class Keyframe, class Landmark>
+bool fuse_skips(Keyframe* keyfrm, const Landmark* lm) {
+    return !lm || lm->will_be_erased() || lm->is_observed_in_keyframe(keyfrm);
+}
+
+}  // namespace adapters
+
+// replace_duplication: one device call over the landmarks that are usable now, then the reference's loop over the container.
+template <class Keyframe, class T>
+inline unsigned int match::fuse::replace_duplication(Keyframe* keyfrm, const T& landmarks_to_check, const float margin) const {
+    using Landmark = std::remove_pointer_t<typename T::value_type>;
+    adapters::fuse_landmark_rows<Landmark> rows;
+    std::vector<std::int32_t> q_lm;
+    for (Landmark* lm : landmarks_to_check) q_lm.push_back(adapters::fuse_skips(keyfrm, lm) ? -1 : rows.add(lm));
+    const adapters::fuse_target_arrays tgt(*keyfrm);   // owns the arrays tgt.target points at
+    const std::vector<ovs_fuse_target> targets(1, tgt.target);
+    std::vector<std::int32_t> best;
+    replace_duplication(targets, rows.table(), {0, static_cast<std::int32_t>(q_lm.size())}, q_lm, margin, best);
+    unsigned int num_fused = 0;
+    std::unordered_set<Landmark*> changed;
+    std::size_t q = 0;
+    for (Landmark* lm : landmarks_to_check) {
+        const int best_idx = best[q++];
+        if (adapters::fuse_skips(keyfrm, lm) || best_idx < 0) continue;
+        adapters::fuse_into_keyframe(keyfrm, lm, best_idx, changed);
+        ++num_fused;
+    }
+    return num_fused;
+}
+
+namespace adapters {
+
+//! The body of mapping_module::fuse_landmark_duplication(fuse_tgt_keyfrms) (module/mapping_module.cc) with the reference's
+//! replace_duplication(keyfrm, landmarks, margin):
+//!   - forward: cur_keyfrm->get_landmarks() into every target, in the container's order: one device call for all targets, then
+//!     the replay target by target, each preceded by one re-query call if some of its queries are on landmarks that survived a
+//!     replace since the call (their descriptors changed);
+//!   - backward: every non-null, non-erased landmark of every target, gathered target by target into a
+//!     std::unordered_set<Landmark*> as the reference does, into cur_keyfrm: replace_duplication above.
+//! Host waits: 2 + the number of targets with re-queries (fuse.num_requery_calls()).
+template <class Keyframe, class Targets>
+void fuse_landmark_duplication(const match::fuse& fuse, Keyframe* cur_keyfrm, const Targets& fuse_tgt_keyfrms, const float margin = 3.0) {
+    using Landmark = std::remove_pointer_t<typename decltype(cur_keyfrm->get_landmarks())::value_type>;
+    const auto cur_landmarks = cur_keyfrm->get_landmarks();
+    {
+        std::vector<Keyframe*> tgts;
+        std::vector<fuse_target_arrays> arrays;
+        for (Keyframe* t : fuse_tgt_keyfrms) tgts.push_back(t);
+        arrays.reserve(tgts.size());   // no reallocation: targets[] points into these
+        std::vector<ovs_fuse_target> targets;
+        for (Keyframe* t : tgts) { arrays.emplace_back(*t); targets.push_back(arrays.back().target); }
+        const std::size_t J = cur_landmarks.size();
+        fuse_landmark_rows<Landmark> rows;
+        std::vector<std::int32_t> row_of(J, -1);
+        for (std::size_t j = 0; j < J; ++j)
+            if (cur_landmarks[j] && !cur_landmarks[j]->will_be_erased()) row_of[j] = rows.add(cur_landmarks[j]);
+        std::vector<std::int32_t> q_off(1, 0), q_lm;
+        for (Keyframe* t : tgts) {
+            for (std::size_t j = 0; j < J; ++j) q_lm.push_back(row_of[j] >= 0 && !cur_landmarks[j]->is_observed_in_keyframe(t) ? row_of[j] : -1);
+            q_off.push_back(static_cast<std::int32_t>(q_lm.size()));
+        }
+        std::vector<std::int32_t> best;
+        fuse.replace_duplication(targets, rows.table(), q_off, q_lm, margin, best);
+        std::unordered_set<Landmark*> changed;
+        for (std::size_t t = 0; t < tgts.size(); ++t) {
+            Keyframe* tgt = tgts[t];
+            const std::size_t q0 = static_cast<std::size_t>(q_off[t]);
+            // the queries of this target on landmarks whose descriptor changed since the call, again with the current descriptors
+            std::vector<std::int32_t> rq_lm;
+            std::vector<std::size_t> rq;
+            for (std::size_t j = 0; j < J; ++j) {
+                Landmark* lm = cur_landmarks[j];
+                if (q_lm[q0 + j] < 0 || !changed.count(lm) || fuse_skips(tgt, lm)) continue;
+                rows.refresh_descriptor(row_of[j]);
+                rq_lm.push_back(row_of[j]); rq.push_back(q0 + j);
+            }
+            if (!rq.empty()) {
+                std::vector<std::int32_t> rbest;
+                fuse.count_requery_call();
+                fuse.replace_duplication(std::vector<ovs_fuse_target>(1, targets[t]), rows.table(), {0, static_cast<std::int32_t>(rq_lm.size())}, rq_lm,
+                                         margin, rbest);
+                for (std::size_t k = 0; k < rq.size(); ++k) best[rq[k]] = rbest[k];
+            }
+            for (std::size_t j = 0; j < J; ++j) {
+                Landmark* lm = cur_landmarks[j];
+                const int best_idx = best[q0 + j];
+                if (q_lm[q0 + j] < 0 || fuse_skips(tgt, lm) || best_idx < 0) continue;
+                fuse_into_keyframe(tgt, lm, best_idx, changed);
+            }
+        }
+    }
+    std::unordered_set<Landmark*> candidates_to_fuse;
+    for (Keyframe* t : fuse_tgt_keyfrms)
+        for (Landmark* lm : t->get_landmarks()) {
+            if (!lm || lm->will_be_erased()) continue;
+            candidates_to_fuse.insert(lm);
+        }
+    fuse.replace_duplication(cur_keyfrm, candidates_to_fuse, margin);
+}
+
+//! The same with a matcher made for the call, as the reference's match::fuse fuse(0.6).
+template <class Keyframe, class Targets>
+void fuse_landmark_duplication(Keyframe* cur_keyfrm, const Targets& fuse_tgt_keyfrms, const float margin = 3.0) {
+    const match::fuse fuse(0.6);
+    fuse_landmark_duplication(fuse, cur_keyfrm, fuse_tgt_keyfrms, margin);
+}
+
+}  // namespace adapters
 
 // --------------------------------------------------------------------------------------------- optimize::pose_optimizer
 inline unsigned int optimize::pose_optimizer::optimize(data::frame& frm) const {

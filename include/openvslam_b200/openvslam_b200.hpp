@@ -520,6 +520,56 @@ private:
     }
 };
 
+//! match::fuse (match/fuse.h): the compute of replace_duplication for many target keyframes in one call
+//! (ovs_fuse_replace_duplication_host).  The data-model updates stay with the caller: adapters.hpp replays them in the reference's
+//! order.
+class fuse final : public base {
+public:
+    explicit fuse(const float lowe_ratio = 0.6, const bool check_orientation = true, const int device = 0)
+        : base(lowe_ratio, check_orientation, device) {}
+    //! The landmark table the queries index: pos_w / mean_normal 3 doubles per landmark, the raw min_valid_dist_ / max_valid_dist_,
+    //! the 32-byte descriptors.
+    struct landmark_table {
+        int num_landmarks = 0;
+        const double* pos_w = nullptr; const double* mean_normal = nullptr;
+        const float* min_valid_dist = nullptr; const float* max_valid_dist = nullptr;
+        const std::uint8_t* descriptors = nullptr;
+    };
+    //! replace_duplication(keyfrm, landmarks_to_check, margin) without the data-model updates, for targets.size() target keyframes:
+    //! the queries of target t are q_lm[q_off[t] .. q_off[t + 1]) (a landmark row, or -1 to skip); best_idx[q] = the keypoint of
+    //! its target the landmark would be fused with, or -1.  Optional per-query geometry (nullptr: not wanted; reproj 2 floats).
+    //! Returns the number of queries with a best_idx.
+    unsigned int replace_duplication(const std::vector<ovs_fuse_target>& targets, const landmark_table& landmarks,
+                                     const std::vector<std::int32_t>& q_off, const std::vector<std::int32_t>& q_lm, const float margin,
+                                     std::vector<std::int32_t>& best_idx, std::uint8_t* passed = nullptr, float* reproj = nullptr,
+                                     float* x_right = nullptr, std::int32_t* pred_level = nullptr) const {
+        if (q_off.size() != targets.size() + 1 || q_off.back() != static_cast<std::int32_t>(q_lm.size()))
+            throw std::invalid_argument("replace_duplication: q_off needs one entry per target plus one, ending at q_lm.size()");
+        best_idx.assign(std::max<std::size_t>(1, q_lm.size()), -1);
+        int n = 0;
+        detail::check(ovs_fuse_replace_duplication_host(h_, static_cast<int>(targets.size()), targets.data(), landmarks.num_landmarks, landmarks.pos_w,
+                                                        landmarks.mean_normal, landmarks.min_valid_dist, landmarks.max_valid_dist,
+                                                        landmarks.descriptors, q_off.data(), q_lm.data(), margin, best_idx.data(), &n, passed,
+                                                        reproj, x_right, pred_level));
+        best_idx.resize(q_lm.size());
+        ++num_calls_;
+        return static_cast<unsigned int>(n);
+    }
+#ifdef OVS_B200_WITH_REFERENCE_TYPES
+    //! The reference's signature (match/fuse.h); body in adapters.hpp.  A template deduced from the arguments (data::keyframe and a
+    //! container of data::landmark* in the reference tree), compiled only where it is called.
+    template <class Keyframe, class T>
+    unsigned int replace_duplication(Keyframe* keyfrm, const T& landmarks_to_check, const float margin = 3.0) const;
+#endif
+    //! library calls made through this object, and the re-queries among them (adapters::fuse_landmark_duplication)
+    unsigned int num_device_calls() const { return num_calls_; }
+    unsigned int num_requery_calls() const { return num_requery_calls_; }
+    void count_requery_call() const { ++num_requery_calls_; }
+
+private:
+    mutable unsigned int num_calls_ = 0, num_requery_calls_ = 0;
+};
+
 class area final : public base {
 public:
     explicit area(const float lowe_ratio = 0.9, const bool check_orientation = true, const int device = 0)

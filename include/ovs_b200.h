@@ -862,6 +862,51 @@ int ovs_fuse_best_keypoints_host(ovs_frame_index* f, int nq, const uint8_t* usab
                                  const float* inv_level_sigma_sq, int num_scale_levels, float margin,
                                  int32_t* best_idx_of_lm, int* num_matches);
 
+/* ---- local mapping: match::fuse::replace_duplication with its reprojection (match/fuse.cc), for the forward and backward passes of
+ * mapping_module::fuse_landmark_duplication (module/mapping_module.cc) ---- */
+
+/* What replace_duplication reads of one target keyframe, from the keyframe's own vectors: the geometry (camera_, img_bounds_,
+ * rot_cw / trans_cw, get_cam_center() as the keyframe holds it, num_scale_levels_, log_scale_factor_), scale_factors_ and
+ * inv_level_sigma_sq_ (num_scale_levels entries each), num_keypts undist_keypts_ (x, y, octave), stereo_x_right_ (NULL:
+ * monocular), descriptors_ (32 B each) and the camera's grid. */
+typedef struct {
+    ovs_frame_geometry geometry;
+    const float* scale_factors;
+    const float* inv_level_sigma_sq;
+    int32_t num_keypts;
+    const float* x;
+    const float* y;
+    const int32_t* octave;
+    const float* x_right;
+    const uint8_t* descriptors;
+    ovs_grid grid;
+} ovs_fuse_target;
+
+/* Each of the number of targets, of landmarks, of queries, of all targets' keypoints and of all targets' grid cells is at most this
+ * (OVS_ERR_UNSUPPORTED beyond): the staged buffers stay far inside size_t and their offsets inside int. */
+#define OVS_FUSE_MAX_ITEMS (1 << 26)
+
+/* The compute of match::fuse::replace_duplication(keyfrm, landmarks_to_check, margin) for B targets at once, without its data-model
+ * updates: for every query, the keypoint best_idx of its target that the reference would fuse the landmark with, or -1.
+ * Landmarks (nlm rows): pos_w[nlm*3] = get_pos_in_world(), mean_normal[nlm*3] = get_obs_mean_normal(), min_valid_dist /
+ * max_valid_dist = the raw min_valid_dist_ / max_valid_dist_, lm_desc[nlm*32] = get_descriptor().  Queries: those of target t are
+ * q_lm[q_off[t] .. q_off[t+1]) (q_off[0] = 0, non-decreasing, Q = q_off[B]); q_lm[q] is a landmark row, or -1 for a query to
+ * skip (the caller's skip rule: no landmark, will_be_erased(), is_observed_in_keyframe()).  A query is answered from its own
+ * landmark row and its target only: reproject_to_image, the valid-distance and ray gates in double, predict_scale_level (DESIGN.md
+ * section 5), then the window margin * scale_factors[level] over the levels [level - 1, level], the chi-square gate of
+ * ovs_fuse_best_keypoints_host, the nearest descriptor (first in get_keypoints_in_cell order on ties) at <= HAMMING_DIST_THR_LOW.
+ * A query whose position or reprojection is not finite gets -1.  num_fused = the number of queries with a best_idx.  Optional
+ * per-query outputs (each may be NULL): passed (the geometry's gates), reproj_xy[Q*2] (rounded to float), x_right, pred_level;
+ * 0 where not passed.  At most 2 launches, one copy each way and one wait, whatever B is; Q = 0 or no query with q_lm >= 0 makes
+ * no launch.  Refused before any launch and any allocation: OVS_ERR_INVALID_ARG for B < 0, a null array that is needed, a target
+ * geometry that ovs_frame_can_observe_host refuses, a null scale table, a keypoint octave outside its target's scale table, a
+ * grid with no cell or more than 2^20 cells, a malformed q_off, a q_lm entry outside [-1, nlm), a margin that is not finite and
+ * positive; OVS_ERR_UNSUPPORTED for a target with 65536 keypoints or more, or a count above OVS_FUSE_MAX_ITEMS. */
+int ovs_fuse_replace_duplication_host(ovs_matcher* m, int B, const ovs_fuse_target* targets, int nlm, const double* pos_w,
+                                      const double* mean_normal, const float* min_valid_dist, const float* max_valid_dist,
+                                      const uint8_t* lm_desc, const int32_t* q_off, const int32_t* q_lm, float margin, int32_t* best_idx,
+                                      int* num_fused, uint8_t* passed, float* reproj_xy, float* x_right, int32_t* pred_level);
+
 /* Measured FP64 peaks of `device` (whole chip, TFLOP/s counting 2 per FMA): independent mma.sync.m8n8k4.f64 (DMMA) and
  * independent DFMA.  bench.py quotes the Cholesky roofline against the DMMA figure measured in the same run. */
 int ovs_probe_fp64_peaks(int device, double* dmma_tflops, double* dfma_tflops);

@@ -206,10 +206,10 @@ extern "C" void ovs_matcher_destroy(ovs_matcher* h) {
     cudaSetDevice(h->device);
     if (h->stream) ovs::sync_stream(h->stream);
     cudaFree(h->d_q); cudaFree(h->d_t); cudaFree(h->d_part); cudaFree(h->d_keys); cudaFree(h->d_mask); cudaFree(h->d_ess);
-    cudaFree(h->d_tv); cudaFree(h->d_tri); cudaFree(h->d_init); cudaFree(h->d_trk);
+    cudaFree(h->d_tv); cudaFree(h->d_tri); cudaFree(h->d_init); cudaFree(h->d_trk); cudaFree(h->d_fuse);
     for (auto& b : h->index_pool) cudaFree(b.base);
     cudaFreeHost(h->h_keys); cudaFreeHost(h->h_stage); cudaFreeHost(h->h_ess); cudaFreeHost(h->h_tv); cudaFreeHost(h->h_tri);
-    cudaFreeHost(h->h_init); cudaFreeHost(h->h_trk);
+    cudaFreeHost(h->h_init); cudaFreeHost(h->h_trk); cudaFreeHost(h->h_fuse);
     for (auto& e : h->ev) if (e) cudaEventDestroy(e);
     if (h->stream) cudaStreamDestroy(h->stream);
     delete h;

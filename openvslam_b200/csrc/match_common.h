@@ -1,5 +1,5 @@
 // match_common.h -- the matcher handle shared by match_bruteforce.cu, match_window.cu, two_view_ransac.cu,
-// two_view_triangulate.cu, initializer.cu and tracking_search.cu.  Its arenas
+// two_view_triangulate.cu, initializer.cu, tracking_search.cu and fuse.cu.  Its arenas
 // grow and are carved through staging.h.
 #pragma once
 #include <algorithm>
@@ -38,6 +38,9 @@ struct ovs_matcher {
     // the tracker's per-landmark geometry (tracking_search.cu): its kernel leaves the matchers' buffers untouched
     uint8_t* d_trk = nullptr; size_t d_trk_cap = 0;
     uint8_t* h_trk = nullptr; size_t h_trk_cap = 0;     // pinned
+    // match::fuse::replace_duplication's batched search (fuse.cu): every target's index and the queries, staged per call
+    uint8_t* d_fuse = nullptr; size_t d_fuse_cap = 0;
+    uint8_t* h_fuse = nullptr; size_t h_fuse_cap = 0;   // pinned
     cudaEvent_t ev[2]{};
     float last_kernel_us = 0.f;
     int num_requeries = 0;   // GPU re-queries issued by the greedy replays so far (diagnostic)
@@ -47,4 +50,10 @@ struct ovs_matcher {
 namespace ovs {
 // the matcher a frame index was built on (match_window.cu): the composed tracking calls (tracking_search.cu) run on its stream
 ovs_matcher* frame_index_matcher(const ovs_frame_index* f);
+// data::assign_keypoints_to_grid (match_window.cu): the rank order of n keypoints -- sorted by (cell_x, cell_y, index), the order
+// frame::get_keypoints_in_cell visits them; keypoints outside the grid get no rank -- and the CSR of cell starts (cols * rows + 1)
+std::vector<int> rank_keypoints(const ovs_grid& grid, int n, const float* x, const float* y, std::vector<int>& rank_to_idx,
+                                std::vector<int>& idx_to_rank, int* nranked);
+// the checks every call taking an ovs_frame_geometry makes (tracking_search.cu)
+int check_geometry(const ovs_frame_geometry* g);
 }  // namespace ovs

@@ -28,6 +28,7 @@
 #include "greedy_replay.h"
 #include "match_common.h"
 #include "two_view_triangulate.h"
+#include "window_walk.cuh"
 
 // ------------------------------------------------------------------------------- frame index
 struct ovs_frame_index {
@@ -58,14 +59,10 @@ __device__ __forceinline__ void topk_insert(unsigned (&k)[kTopK], unsigned key) 
     }
 }
 
-__device__ __forceinline__ int cv_floor_f(float v) { return __float2int_rd(v); }
-__device__ __forceinline__ int cv_ceil_f(float v) { return __float2int_ru(v); }
-
-// match::compute_descriptor_distance_32 by eight population counts
-__device__ __forceinline__ int hamming256(const uint4& qa, const uint4& qb, const uint4& ta, const uint4& tb) {
-    return __popc(qa.x ^ ta.x) + __popc(qa.y ^ ta.y) + __popc(qa.z ^ ta.z) + __popc(qa.w ^ ta.w)
-           + __popc(qb.x ^ tb.x) + __popc(qb.y ^ tb.y) + __popc(qb.z ^ tb.z) + __popc(qb.w ^ tb.w);
-}
+using ovs::cv_ceil_f;
+using ovs::cv_floor_f;
+using ovs::hamming256;
+using ovs::WindowFrame;
 
 // One chunk of a warp's running top-K (k_triangulation_topk, k_node_topk): lane r < K carries entry r in `extra`, every lane
 // holds up to K keys of the chunk in mine[]; returns lane r's entry r of the K smallest keys of both.  Keys are unique (they
@@ -89,13 +86,6 @@ __device__ __forceinline__ unsigned warp_merge_topk(unsigned extra, unsigned (&m
     return next_extra;
 }
 
-struct WindowFrame {
-    float min_x, min_y, inv_w, inv_h;
-    int cols, rows;
-    const float* x; const float* y; const float* xr; const signed char* oct; const uint4* desc;
-    const int* cell_start; const unsigned short* cap;
-};
-
 struct WindowQueries {
     int nq;
     const float2* ref; const float* margin; const int* min_level; const int* max_level; const float* xr; const uint4* desc;
@@ -109,54 +99,10 @@ __global__ void __launch_bounds__(128) k_window_topk(WindowFrame F, WindowQuerie
     const int q = blockIdx.x * 4 + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
     if (q >= Q.nq) return;
-    const float2 ref = Q.ref[q];
-    const float margin = Q.margin[q];
-    const int min_level = Q.min_level[q], max_level = Q.max_level[q];
     unsigned best[kTopK] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0xffffffffu};
-    // data::frame::get_keypoints_in_cell: cell range (float arithmetic as in the reference)
-    const int min_cx = max(0, cv_floor_f(__fmul_rn(__fsub_rn(__fsub_rn(ref.x, F.min_x), margin), F.inv_w)));
-    const int max_cx = min(F.cols - 1, cv_ceil_f(__fmul_rn(__fadd_rn(__fsub_rn(ref.x, F.min_x), margin), F.inv_w)));
-    const int min_cy = max(0, cv_floor_f(__fmul_rn(__fsub_rn(__fsub_rn(ref.y, F.min_y), margin), F.inv_h)));
-    const int max_cy = min(F.rows - 1, cv_ceil_f(__fmul_rn(__fadd_rn(__fsub_rn(ref.y, F.min_y), margin), F.inv_h)));
-    if (F.cols > min_cx && max_cx >= 0 && F.rows > min_cy && max_cy >= 0) {
-        const uint4 qa = __ldg(Q.desc + 2 * (size_t)q), qb = __ldg(Q.desc + 2 * (size_t)q + 1);
-        const bool check_level = (0 < min_level) || (0 <= max_level);
-        const float xr_q = Q.xr ? Q.xr[q] : -1.0f;
-        for (int cx = min_cx; cx <= max_cx; ++cx) {
-            const int r0 = F.cell_start[cx * F.rows + min_cy], r1 = F.cell_start[cx * F.rows + max_cy + 1];
-            for (int r = r0 + lane; r < r1; r += 32) {
-                if (check_level) {
-                    const int o = F.oct[r];
-                    if (o < min_level) continue;
-                    if (0 <= max_level && max_level < o) continue;
-                }
-                const float dist_x = __fsub_rn(F.x[r], ref.x), dist_y = __fsub_rn(F.y[r], ref.y);
-                if (!(fabsf(dist_x) < margin && fabsf(dist_y) < margin)) continue;
-                if (Q.fuse_gate) {
-                    const float ex = __fsub_rn(ref.x, F.x[r]), ey = __fsub_rn(ref.y, F.y[r]);
-                    const float w = Q.inv_sigma_sq[F.oct[r] & 15];
-                    const float e2 = __fadd_rn(__fmul_rn(ex, ex), __fmul_rn(ey, ey));
-                    const float kxr = F.xr ? F.xr[r] : -1.0f;
-                    if (kxr >= 0 && Q.xr) {
-                        const float er = __fsub_rn(xr_q, kxr);
-                        if (__fmul_rn(__fadd_rn(e2, __fmul_rn(er, er)), w) > 7.8f) continue;
-                    } else {
-                        if (__fmul_rn(e2, w) > 5.99f) continue;
-                    }
-                } else if (F.xr) {
-                    const float kxr = F.xr[r];
-                    if (0 < kxr) {
-                        const float reproj_error = fabsf(__fsub_rn(xr_q, kxr));
-                        if (margin < reproj_error) continue;
-                    }
-                }
-                const uint4 ta = __ldg(F.desc + 2 * (size_t)r), tb = __ldg(F.desc + 2 * (size_t)r + 1);
-                const int d = hamming256(qa, qb, ta, tb);
-                if (F.cap && !(d < (int)F.cap[r])) continue;
-                topk_insert(best, ((unsigned)d << 16) | (unsigned)r);
-            }
-        }
-    }
+    ovs::window_walk(F, Q.ref[q], Q.margin[q], Q.min_level[q], Q.max_level[q], Q.xr != nullptr, [&] { return Q.xr ? Q.xr[q] : -1.0f; }, Q.desc + 2 * (size_t)q,
+                     Q.fuse_gate != 0, [&](int o) { return Q.inv_sigma_sq[o & 15]; }, lane,
+                     [&](unsigned key) { topk_insert(best, key); });
     // merge the 32 sorted lists: 4 rounds of warp-wide minimum
 #pragma unroll
     for (int k = 0; k < kTopK; ++k) {
@@ -359,24 +305,28 @@ int requery(const ovs_frame_index* f, bool use_xr, const float* ref_xy, float ma
 
 }  // namespace
 
-namespace {
-
-// data::assign_keypoints_to_grid on the host mirrors already stored in f (hx, hy): counting sort by cell (cx major, cy
-// minor), index order kept inside a cell.  Fills rank_to_idx / idx_to_rank / nranked and returns the cell CSR.
-std::vector<int> rank_keypoints(ovs_frame_index* f) {
-    const ovs_grid& grid = f->grid;
-    const int n = f->n, ncells = grid.num_grid_cols * grid.num_grid_rows;
+// data::assign_keypoints_to_grid: counting sort by cell (cx major, cy minor), index order kept inside a cell.  Fills rank_to_idx /
+// idx_to_rank / nranked and returns the cell CSR.
+std::vector<int> ovs::rank_keypoints(const ovs_grid& grid, int n, const float* x, const float* y, std::vector<int>& rank_to_idx,
+                                     std::vector<int>& idx_to_rank, int* nranked) {
+    const int ncells = grid.num_grid_cols * grid.num_grid_rows;
     std::vector<int> cell(n, -1), start(ncells + 1, 0);
     for (int i = 0; i < n; ++i) {
         int cx, cy;
-        if (cell_of(grid, f->hx[i], f->hy[i], &cx, &cy)) { cell[i] = cx * grid.num_grid_rows + cy; start[cell[i] + 1]++; }
+        if (cell_of(grid, x[i], y[i], &cx, &cy)) { cell[i] = cx * grid.num_grid_rows + cy; start[cell[i] + 1]++; }
     }
     for (int c = 0; c < ncells; ++c) start[c + 1] += start[c];
-    f->nranked = start[ncells];
-    f->rank_to_idx.assign(std::max(f->nranked, 1), 0); f->idx_to_rank.assign(std::max(n, 1), -1);
+    *nranked = start[ncells];
+    rank_to_idx.assign(std::max(*nranked, 1), 0); idx_to_rank.assign(std::max(n, 1), -1);
     std::vector<int> pos(start.begin(), start.end() - 1);
-    for (int i = 0; i < n; ++i) if (cell[i] >= 0) { const int r = pos[cell[i]]++; f->rank_to_idx[r] = i; f->idx_to_rank[i] = r; }
+    for (int i = 0; i < n; ++i) if (cell[i] >= 0) { const int r = pos[cell[i]]++; rank_to_idx[r] = i; idx_to_rank[i] = r; }
     return start;
+}
+
+namespace {
+
+std::vector<int> rank_keypoints(ovs_frame_index* f) {
+    return ovs::rank_keypoints(f->grid, f->n, f->hx.data(), f->hy.data(), f->rank_to_idx, f->idx_to_rank, &f->nranked);
 }
 
 bool alloc_index_arrays(ovs_frame_index* f, size_t R, int ncells) {

@@ -71,6 +71,26 @@ OVS_BA_HD bool can_observe(const CameraD& cam, const ImgBounds& b, const double*
     return true;
 }
 
+// match::fuse::replace_duplication's per-landmark geometry (fuse_observe(...) in DESIGN.md section 5): the in-image test, then the
+// valid-distance range and the ray test as that loop writes them -- both in double, unlike can_observe: dist < (double)(float)(0.7 *
+// min_valid_dist_) or (double)(float)(1.3 * max_valid_dist_) < dist rejects, and dot(cam_to_lm_vec, mean_normal) < 0.5 * dist
+// rejects, with no division -- then the predicted level of (float)dist.  dist and the dot are summed as in can_observe.  A position
+// or a reprojection that is not finite is rejected first: those gates let a NaN through, and the reference is undefined there.
+OVS_BA_HD bool fuse_observe(const CameraD& cam, const ImgBounds& b, const double* rot_cw, const double* trans_cw, const double* cam_center,
+                            const double* pos_w, const double* mean_normal, float min_valid_dist, float max_valid_dist, float log_scale_factor,
+                            int num_levels, double* uv, float* x_right, int* pred_level) {
+    if (!(isfinite(pos_w[0]) && isfinite(pos_w[1]) && isfinite(pos_w[2]))) return false;
+    if (!reproject_to_image(cam, b, rot_cw, trans_cw, pos_w, uv, x_right)) return false;
+    if (!(isfinite(uv[0]) && isfinite(uv[1]))) return false;
+    const double v[3] = {pos_w[0] - cam_center[0], pos_w[1] - cam_center[1], pos_w[2] - cam_center[2]};
+    const double dist = sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
+    const float min_dist = (float)(0.7 * (double)min_valid_dist), max_dist = (float)(1.3 * (double)max_valid_dist);
+    if (dist < (double)min_dist || (double)max_dist < dist) return false;
+    if (v[0] * mean_normal[0] + v[1] * mean_normal[1] + v[2] * mean_normal[2] < 0.5 * dist) return false;
+    *pred_level = predict_scale_level((float)dist, max_valid_dist, log_scale_factor, num_levels);
+    return true;
+}
+
 // The motion model's direction (match::projection::match_current_and_last_frames): trans_wc = -R_cw^T t_cw, trans_lc = R_lw trans_wc
 // + t_lw, each row summed x, y, z; forward when trans_lc.z > true_baseline, backward when -trans_lc.z > true_baseline; monocular
 // gives neither.

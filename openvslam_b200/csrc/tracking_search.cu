@@ -54,22 +54,6 @@ __global__ void __launch_bounds__(128) k_track_geometry(TrackArgs A) {
     if (A.level) A.level[l] = ok ? level : 0;
 }
 
-int check_geometry(const ovs_frame_geometry* g) {
-    OVS_REQUIRE(g, OVS_ERR_INVALID_ARG, "null frame geometry");
-    const int model = g->camera.model;
-    OVS_REQUIRE(model == OVS_CAMERA_PERSPECTIVE || model == OVS_CAMERA_EQUIRECTANGULAR || model == OVS_CAMERA_FISHEYE ||
-                model == OVS_CAMERA_RADIAL_DIVISION, OVS_ERR_INVALID_ARG, "unknown camera model %d", model);
-    OVS_REQUIRE(g->num_scale_levels >= 1 && g->num_scale_levels <= 16, OVS_ERR_INVALID_ARG, "num_scale_levels %d outside 1 .. 16",
-                g->num_scale_levels);
-    OVS_REQUIRE(std::isfinite(g->log_scale_factor) && g->log_scale_factor > 0.0f, OVS_ERR_INVALID_ARG,
-                "log_scale_factor must be positive and finite");
-    bool finite = true;
-    for (int k = 0; k < 9; ++k) finite = finite && std::isfinite(g->rot_cw[k]);
-    for (int k = 0; k < 3; ++k) finite = finite && std::isfinite(g->trans_cw[k]) && std::isfinite(g->cam_center[k]);
-    OVS_REQUIRE(finite, OVS_ERR_INVALID_ARG, "the frame's pose or camera centre is not finite");
-    return OVS_OK;
-}
-
 TrackArgs track_args(const ovs_frame_geometry& g) {
     TrackArgs A{};
     const ovs_camera& c = g.camera;
@@ -136,6 +120,22 @@ int check_can_observe_args(const ovs_frame_geometry* g, int nlm, const double* p
 }
 
 }  // namespace
+
+int check_geometry(const ovs_frame_geometry* g) {
+    OVS_REQUIRE(g, OVS_ERR_INVALID_ARG, "null frame geometry");
+    const int model = g->camera.model;
+    OVS_REQUIRE(model == OVS_CAMERA_PERSPECTIVE || model == OVS_CAMERA_EQUIRECTANGULAR || model == OVS_CAMERA_FISHEYE ||
+                model == OVS_CAMERA_RADIAL_DIVISION, OVS_ERR_INVALID_ARG, "unknown camera model %d", model);
+    OVS_REQUIRE(g->num_scale_levels >= 1 && g->num_scale_levels <= 16, OVS_ERR_INVALID_ARG, "num_scale_levels %d outside 1 .. 16",
+                g->num_scale_levels);
+    OVS_REQUIRE(std::isfinite(g->log_scale_factor) && g->log_scale_factor > 0.0f, OVS_ERR_INVALID_ARG,
+                "log_scale_factor must be positive and finite");
+    bool finite = true;
+    for (int k = 0; k < 9; ++k) finite = finite && std::isfinite(g->rot_cw[k]);
+    for (int k = 0; k < 3; ++k) finite = finite && std::isfinite(g->trans_cw[k]) && std::isfinite(g->cam_center[k]);
+    OVS_REQUIRE(finite, OVS_ERR_INVALID_ARG, "the frame's pose or camera centre is not finite");
+    return OVS_OK;
+}
 
 }  // namespace ovs
 

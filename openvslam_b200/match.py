@@ -447,8 +447,66 @@ class bow_tree(_matcher_handle):
         return n.value, out[:len(a1)]
 
 
+class FuseTarget(C.Structure):
+    """ovs_fuse_target: what match::fuse::replace_duplication reads of one target keyframe."""
+    _fields_ = [("geometry", FrameGeometry), ("scale_factors", C.c_void_p), ("inv_level_sigma_sq", C.c_void_p), ("num_keypts", C.c_int32),
+                ("x", C.c_void_p), ("y", C.c_void_p), ("octave", C.c_void_p), ("x_right", C.c_void_p), ("descriptors", C.c_void_p),
+                ("grid", Grid)]
+
+
+class fuse_target:
+    """One target keyframe of fuse.replace_duplication: its frame_geometry, scale_factors_ and inv_level_sigma_sq_, undist_keypts_
+    (x, y, octave), descriptors_ (n, 32), the camera grid and stereo_x_right_ (None: monocular).  Holds the arrays the struct
+    points at."""
+
+    def __init__(self, geometry, scale_factors, inv_level_sigma_sq, x, y, octave, desc, grid, x_right=None):
+        self.scale_factors, psf = _f32(scale_factors); self.inv_level_sigma_sq, piw = _f32(inv_level_sigma_sq)
+        self.x, px = _f32(x); self.y, py = _f32(y); self.octave, po = _i32(octave); self.desc, pd = _desc(desc)
+        n = len(self.x)
+        if len(self.y) != n or len(self.octave) != n or len(self.desc) != n:
+            raise ValueError("fuse_target: one y, octave and descriptor per keypoint")
+        if len(self.scale_factors) != geometry.num_scale_levels or len(self.inv_level_sigma_sq) != geometry.num_scale_levels:
+            raise ValueError("fuse_target: one scale factor and one inverse sigma^2 per level of the geometry")
+        pxr = None
+        self.x_right = None
+        if x_right is not None:
+            self.x_right, pxr = _f32(x_right)
+            if len(self.x_right) != n:
+                raise ValueError("fuse_target: one x_right per keypoint")
+        self.n = n
+        self.c = FuseTarget(geometry, psf, piw, n, px, py, po, pxr, pd, grid)
+
+
 class fuse(_matcher_handle):
-    """openvslam::match::fuse: the matching core (best keypoint per reprojected landmark)."""
+    """openvslam::match::fuse: the matching core (best keypoint per reprojected landmark), and replace_duplication's compute for
+    many target keyframes at once."""
+
+    def replace_duplication(self, targets, pos_w, mean_normal, min_valid_dist, max_valid_dist, lm_desc, q_off, q_lm, margin=3.0, geometry=False):
+        """ovs_fuse_replace_duplication_host: targets = [fuse_target]; landmark table (nlm rows): pos_w / mean_normal (nlm, 3), the raw
+        min_valid_dist_ / max_valid_dist_, lm_desc (nlm, 32); the queries of target t are q_lm[q_off[t]:q_off[t + 1]] (a landmark
+        row, or -1 to skip) -> (num_fused, best_idx (Q,)), and with geometry=True also passed (Q,) bool, reproj_xy (Q, 2) f32,
+        x_right (Q,) f32, pred_level (Q,) i32 (zeros where not passed)."""
+        pos, pp, nrm, pn, lo, plo, hi, phi, nlm = _landmark_arrays(pos_w, mean_normal, min_valid_dist, max_valid_dist)
+        d, pd = _desc(lm_desc)
+        if len(d) != nlm:
+            raise ValueError("replace_duplication: one descriptor per landmark")
+        B = len(targets)
+        arr = (FuseTarget * max(B, 1))(*[t.c for t in targets])
+        qo, pqo = _i32(q_off); ql, pql = _i32(q_lm)
+        if len(qo) != B + 1:
+            raise ValueError("replace_duplication: q_off needs B + 1 entries")
+        Q = len(ql)
+        if qo[-1] != Q:
+            raise ValueError("replace_duplication: q_off[-1] must be len(q_lm)")
+        n1 = max(Q, 1)
+        best = np.full(n1, -1, np.int32); n = C.c_int(0)
+        outs = (np.zeros(n1, np.uint8), np.zeros((n1, 2), np.float32), np.zeros(n1, np.float32), np.zeros(n1, np.int32)) if geometry else None
+        vp = lambda a: a.ctypes.data_as(C.c_void_p)
+        _lib.check(_lib.lib().ovs_fuse_replace_duplication_host(self._h, B, arr, nlm, pp, pn, plo, phi, pd, pqo, pql, C.c_float(margin), vp(best),
+                                                                C.byref(n), *((vp(a) for a in outs) if geometry else (None,) * 4)))
+        if not geometry:
+            return n.value, best[:Q]
+        return n.value, best[:Q], outs[0][:Q].astype(bool), outs[1][:Q], outs[2][:Q], outs[3][:Q]
 
     def best_keypoints(self, keyfrm, reproj_xy, reproj_x_right, pred_level, lm_desc, scale_factors, inv_level_sigma_sq, margin, usable=None):
         rp, prp = _f32(reproj_xy); lv, plv = _i32(pred_level); d, pd = _desc(lm_desc); sf, psf = _f32(scale_factors); iw, piw = _f32(inv_level_sigma_sq)
