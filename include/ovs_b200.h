@@ -292,6 +292,27 @@ int ovs_robust_match_frame_and_keyframe_device(ovs_matcher* h, const uint8_t* d_
 int ovs_matcher_num_requeries(const ovs_matcher* h, int* out);
 /* Device time (CUDA events, microseconds) of the Hamming kernels of the last call. */
 int ovs_matcher_last_kernel_us(const ovs_matcher* h, float* out_us);
+/* Development aids / test hooks: the kernels behind the greedy replays' GPU re-queries, on host arrays, with the launch geometry
+ * and the handle buffers of the entry points that use them; keys as in their candidate lists (8 per query, ascending,
+ * 0xFFFFFFFF past the end).
+ *  ovs_debug_hamming_one: the brute-force re-query of one 32-byte query over nt (1 .. 65535) train descriptors, train
+ *    descriptor j skipped where bit j & 31 of exclude_mask[j >> 5] is set; keys (distance << 16 | j) in keys_out[8].
+ *  ovs_debug_node_topk: the bow_tree lists; query k's candidates are ranks qseg[2k] .. qseg[2k + 1] - 1 of tdesc[R * 32],
+ *    keys (distance << 16 | rank).  q0 < 0: the list launch over all nq queries, a candidate r with taken[r] != 0 skipped
+ *    (taken may be NULL), keys_out[nq * 8].  q0 >= 0: the list launch without taken, then the re-query of query q0 alone with
+ *    taken, its list in the spare row nq, keys_out[(nq + 1) * 8].
+ *  ovs_debug_triangulation_topk: the match_for_triangulation lists (batched == 0: one problem, nprob == 1 and
+ *    queries_per_prob == nq) or create_new_landmarks' batched lists (nq == nprob * queries_per_prob; query q of problem
+ *    p = q / queries_per_prob reads keypoint entry q - p * queries_per_prob, E_12 prob_E[9 p], epipole prob_epipole[3 p] and
+ *    the candidates and taken flags from prob_tbase[p] on, qseg relative to that base); the distance, epipole and epipolar tests
+ *    of ovs_robust_match_for_triangulation_host, keys (distance << 16 | 0xFFFF - rank).  q0 and taken as ovs_debug_node_topk. */
+int ovs_debug_hamming_one(ovs_matcher* h, const uint8_t* query, const uint8_t* train, int nt, const uint32_t* exclude_mask, uint32_t* keys_out);
+int ovs_debug_node_topk(ovs_matcher* h, int nq, const uint8_t* qdesc, const int32_t* qseg, int R, const uint8_t* tdesc, const uint8_t* taken,
+                        int q0, uint32_t* keys_out);
+int ovs_debug_triangulation_topk(ovs_matcher* h, int batched, int nq, int queries_per_prob, const uint8_t* qdesc, const double* qbearing,
+                                 const float* qscale, const uint8_t* qstereo, const int32_t* qseg, int R, const uint8_t* tdesc,
+                                 const double* tbearing, const uint8_t* tstereo, int nprob, const double* prob_E, const double* prob_epipole,
+                                 const int32_t* prob_tbase, const uint8_t* taken, int q0, uint32_t* keys_out);
 
 /* ---- windowed search: match::projection / match::area (match/projection.cc, match/area.cc) ---- */
 

@@ -4,11 +4,11 @@
 //
 // k_hamming_topk    every query descriptor against a chunk of train descriptors staged in
 //                   shared memory (broadcast 128-bit reads); each thread keeps its query in 8
-//                   registers and a sorted top-4 of (distance << 16 | train index) keys.
+//                   registers and a sorted top-8 of (distance << 16 | train index) keys.
 //                   Grid = query blocks x train chunks so that 4000 x 4000 fills the 132 SMs of an H100.
-// k_topk_merge      merges the per-chunk top-4 lists of a query.
+// k_topk_merge      merges the per-chunk top-8 lists of a query.
 //
-// A sorted (distance, index) top-4 is what the reference's sequential `<` scan needs: best =
+// A sorted (distance, index) top-8 is what the reference's sequential `<` scan needs: best =
 // lowest index among the minimum distances, second best = next key.  robust::brute_force_match
 // also removes already-matched frame keypoints from later scans (a sequential dependency); the
 // host replays that greedy rule on the top-8 lists (greedy_replay.h) and re-queries the GPU (with an
@@ -55,11 +55,9 @@ __device__ __forceinline__ void topk_insert(unsigned (&k)[kTopK], unsigned key) 
 }
 
 // desc_q [nq][32 B], desc_t [nt][32 B] (16-byte aligned).  Train chunk c covers
-// [c * chunk, min(nt, (c+1) * chunk)).  out[(q * nchunks + c) * 4 + k].
-template <bool kHasMask>
+// [c * chunk, min(nt, (c+1) * chunk)).  out[(q * nchunks + c) * 8 + k].
 __global__ void __launch_bounds__(kQueriesPerBlock) k_hamming_topk(const uint4* __restrict__ desc_q, int nq,
                                                                    const uint4* __restrict__ desc_t, int nt, int chunk,
-                                                                   const unsigned* __restrict__ exclude,
                                                                    unsigned* __restrict__ out) {
     __shared__ uint4 tile[kTrainTile * 2];
     const int q = blockIdx.x * kQueriesPerBlock + threadIdx.x;
@@ -80,9 +78,7 @@ __global__ void __launch_bounds__(kQueriesPerBlock) k_hamming_topk(const uint4* 
         for (int j = 0; j < n; ++j) {
             const uint4 ta = tile[2 * j], tb = tile[2 * j + 1];
             const int d = hamming256(qa, qb, ta, tb);
-            const int idx = t0 + j;
-            if (kHasMask) { if (exclude[idx >> 5] & (1u << (idx & 31))) continue; }
-            topk_insert(best, ((unsigned)d << 16) | (unsigned)idx);
+            topk_insert(best, ((unsigned)d << 16) | (unsigned)(t0 + j));
         }
     }
     if (q < nq) {
@@ -146,8 +142,8 @@ namespace {
 using ovs::grow_dev;
 using ovs::grow_host;
 
-// Launches the top-4 search; result keys end up in d_out[nq * 4].
-int launch_topk(ovs_matcher* h, const uint8_t* d_q, int nq, const uint8_t* d_t, int nt, const unsigned* d_exclude, unsigned* d_out) {
+// Launches the top-8 search; result keys end up in d_out[nq * 8].
+int launch_topk(ovs_matcher* h, const uint8_t* d_q, int nq, const uint8_t* d_t, int nt, unsigned* d_out) {
     cudaStream_t st = h->stream;
     const int qblocks = (nq + kQueriesPerBlock - 1) / kQueriesPerBlock;
     // enough (query block, train chunk) pairs for ~8 resident blocks (32 warps) per SM -- a thread walks its chunk serially, so the
@@ -165,10 +161,7 @@ int launch_topk(ovs_matcher* h, const uint8_t* d_q, int nq, const uint8_t* d_t, 
         d_first = h->d_part;
     }
     dim3 grid(qblocks, nchunks);
-    if (d_exclude)
-        k_hamming_topk<true><<<grid, kQueriesPerBlock, 0, st>>>((const uint4*)d_q, nq, (const uint4*)d_t, nt, chunk, d_exclude, d_first);
-    else
-        k_hamming_topk<false><<<grid, kQueriesPerBlock, 0, st>>>((const uint4*)d_q, nq, (const uint4*)d_t, nt, chunk, nullptr, d_first);
+    k_hamming_topk<<<grid, kQueriesPerBlock, 0, st>>>((const uint4*)d_q, nq, (const uint4*)d_t, nt, chunk, d_first);
     OVS_LAUNCH_CHECK();
     if (nchunks > 1) {
         k_topk_merge<<<(nq + 127) / 128, 128, 0, st>>>(h->d_part, nq, nchunks, d_out);
@@ -224,7 +217,7 @@ extern "C" int ovs_match_bruteforce_topk_device(ovs_matcher* h, const uint8_t* d
     OVS_REQUIRE(((uintptr_t)d_query & 15) == 0 && ((uintptr_t)d_train & 15) == 0, OVS_ERR_INVALID_ARG, "descriptors must be 16-byte aligned");
     OVS_CUDA_CHECK(cudaSetDevice(h->device));
     OVS_CUDA_CHECK(cudaEventRecord(h->ev[0], h->stream));
-    int rc = launch_topk(h, d_query, nq, d_train, nt, nullptr, d_keys_out);
+    int rc = launch_topk(h, d_query, nq, d_train, nt, d_keys_out);
     if (rc != OVS_OK) return rc;
     OVS_CUDA_CHECK(cudaEventRecord(h->ev[1], h->stream));
     OVS_CUDA_CHECK(ovs::sync_event(h->ev[1]));
@@ -250,7 +243,7 @@ int topk_host_impl(ovs_matcher* h, const uint8_t* query, int nq, const uint8_t* 
     OVS_CUDA_CHECK(cudaMemcpyAsync(h->d_q, h->h_stage, (size_t)nq * 32, cudaMemcpyHostToDevice, st));
     if (nt) OVS_CUDA_CHECK(cudaMemcpyAsync(h->d_t, h->h_stage + (size_t)nq * 32, (size_t)nt * 32, cudaMemcpyHostToDevice, st));
     OVS_CUDA_CHECK(cudaEventRecord(h->ev[0], st));
-    rc = launch_topk(h, h->d_q, nq, h->d_t, nt, nullptr, h->d_keys);
+    rc = launch_topk(h, h->d_q, nq, h->d_t, nt, h->d_keys);
     if (rc != OVS_OK) return rc;
     OVS_CUDA_CHECK(cudaEventRecord(h->ev[1], st));
     OVS_CUDA_CHECK(cudaMemcpyAsync(h->h_keys, h->d_keys, (size_t)nq * kTopK * sizeof(unsigned), cudaMemcpyDeviceToHost, st));
@@ -368,7 +361,7 @@ extern "C" int ovs_robust_brute_force_match_device(ovs_matcher* h, const uint8_t
     if ((rc = grow_host(&h->h_keys, &h->h_keys_cap, (size_t)(n2 + 1) * kTopK)) != OVS_OK) return rc;
     cudaStream_t st = h->stream;
     OVS_CUDA_CHECK(cudaEventRecord(h->ev[0], st));
-    rc = launch_topk(h, d_desc_keyfrm, n2, d_desc_frm, n1, nullptr, h->d_keys);
+    rc = launch_topk(h, d_desc_keyfrm, n2, d_desc_frm, n1, h->d_keys);
     if (rc != OVS_OK) return rc;
     OVS_CUDA_CHECK(cudaEventRecord(h->ev[1], st));
     OVS_CUDA_CHECK(cudaMemcpyAsync(h->h_keys, h->d_keys, (size_t)n2 * kTopK * sizeof(unsigned), cudaMemcpyDeviceToHost, st));
@@ -387,5 +380,33 @@ extern "C" int ovs_matcher_num_requeries(const ovs_matcher* h, int* out) {
 extern "C" int ovs_matcher_last_kernel_us(const ovs_matcher* h, float* out_us) {
     OVS_REQUIRE(h && out_us, OVS_ERR_INVALID_ARG, "null argument");
     *out_us = h->last_kernel_us;
+    return OVS_OK;
+}
+
+// Development aid / test hook: the brute-force re-query (k_hamming_one, one block of 256, as robust_replay launches it) of one
+// query descriptor on host arrays, through the matcher's own buffers.  tests/test_candidate_lists_gpu.py compares its keys
+// with an exact numpy top-8.
+extern "C" int ovs_debug_hamming_one(ovs_matcher* h, const uint8_t* query, const uint8_t* train, int nt, const uint32_t* exclude_mask,
+                                     uint32_t* keys_out) {
+    OVS_REQUIRE(h && query && train && exclude_mask && keys_out && nt >= 1, OVS_ERR_INVALID_ARG, "bad argument");
+    OVS_REQUIRE(nt < 65536, OVS_ERR_UNSUPPORTED, "train set larger than 65535 descriptors");
+    OVS_CUDA_CHECK(cudaSetDevice(h->device));
+    const size_t words = ((size_t)nt + 31) / 32;
+    int rc;
+    if ((rc = grow_dev(&h->d_q, &h->d_q_cap, 32)) != OVS_OK) return rc;
+    if ((rc = grow_dev(&h->d_t, &h->d_t_cap, (size_t)nt * 32)) != OVS_OK) return rc;
+    if ((rc = grow_dev(&h->d_mask, &h->d_mask_cap, words)) != OVS_OK) return rc;
+    if ((rc = grow_dev(&h->d_keys, &h->d_keys_cap, (size_t)kTopK)) != OVS_OK) return rc;
+    if ((rc = grow_host(&h->h_keys, &h->h_keys_cap, (size_t)kTopK)) != OVS_OK) return rc;
+    cudaStream_t st = h->stream;
+    OVS_CUDA_CHECK(cudaMemcpyAsync(h->d_q, query, 32, cudaMemcpyHostToDevice, st));
+    OVS_CUDA_CHECK(cudaMemcpyAsync(h->d_t, train, (size_t)nt * 32, cudaMemcpyHostToDevice, st));
+    OVS_CUDA_CHECK(cudaMemcpyAsync(h->d_mask, exclude_mask, words * sizeof(unsigned), cudaMemcpyHostToDevice, st));
+    OVS_CUDA_CHECK(cudaMemsetAsync(h->d_keys, 0x5a, kTopK * sizeof(unsigned), st));   // a key the kernel leaves unwritten shows
+    k_hamming_one<<<1, 256, 0, st>>>(reinterpret_cast<const uint4*>(h->d_q), reinterpret_cast<const uint4*>(h->d_t), nt, h->d_mask, h->d_keys);
+    OVS_LAUNCH_CHECK();
+    OVS_CUDA_CHECK(cudaMemcpyAsync(h->h_keys, h->d_keys, kTopK * sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+    OVS_CUDA_CHECK(ovs::sync_stream(st));
+    memcpy(keys_out, h->h_keys, kTopK * sizeof(unsigned));
     return OVS_OK;
 }

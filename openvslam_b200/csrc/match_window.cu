@@ -1425,7 +1425,131 @@ int bow_core(ovs_matcher* m, int na, const uint8_t* desc_a, const uint8_t* valid
     return OVS_OK;
 }
 
+// Candidate segments [seg[2 k], seg[2 k + 1]) of the test hooks below, each inside [0, R - base[k / per_prob]).
+int check_segments(int nq, const int32_t* seg, int R, const int32_t* base, int per_prob) {
+    for (int k = 0; k < nq; ++k) {
+        const int b = base ? base[k / per_prob] : 0;
+        OVS_REQUIRE(0 <= seg[2 * k] && seg[2 * k] <= seg[2 * k + 1] && b + seg[2 * k + 1] <= R, OVS_ERR_INVALID_ARG,
+                    "segment of query %d outside the %d candidates", k, R);
+    }
+    return OVS_OK;
+}
+
 }  // namespace
+
+// Development aid / test hook: k_node_topk on host arrays, with bow_core's launch geometry and buffers.  q0 < 0: the list launch over
+// all nq queries, taken (null: none) applied to every query, keys_out[nq * 8].  q0 >= 0: the list launch without taken, then
+// bow_core's re-query of query q0 alone with taken, its list in the spare row nq, keys_out[(nq + 1) * 8].  Every key slot is filled
+// with 0x5a5a5a5a first, so a slot the kernels leave unwritten shows.  tests/test_candidate_lists_gpu.py compares the keys with an
+// exact numpy top-8.
+extern "C" int ovs_debug_node_topk(ovs_matcher* m, int nq, const uint8_t* qdesc, const int32_t* qseg, int R, const uint8_t* tdesc,
+                                   const uint8_t* taken, int q0, uint32_t* keys_out) {
+    OVS_REQUIRE(m && qdesc && qseg && keys_out && nq >= 1 && R >= 0 && (R == 0 || tdesc) && q0 < nq, OVS_ERR_INVALID_ARG, "bad argument");
+    OVS_REQUIRE(R < 65536, OVS_ERR_UNSUPPORTED, "more than 65535 candidate keypoints");
+    int rc = check_segments(nq, qseg, R, nullptr, 1);
+    if (rc != OVS_OK) return rc;
+    OVS_CUDA_CHECK(cudaSetDevice(m->device));
+    const size_t sQ = (size_t)nq, sR = (size_t)R, rows = sQ + (q0 >= 0 ? 1 : 0);
+    NodeArgs A{};
+    uint8_t *hqd, *htd, *htk, *dtk; int2* hsg;
+    ovs::Staging S;
+    rc = ovs::stage(S, m->h_stage, m->h_stage_cap, m->d_q, m->d_q_cap, [&](ovs::Staging& S) {
+        A.qdesc = (const uint4*)S.in(hqd, 32 * sQ); A.tdesc = (const uint4*)S.in(htd, 32 * sR); A.qseg = S.in(hsg, sQ);
+        dtk = S.in(htk, sR);
+    });
+    if (rc != OVS_OK) return rc;
+    if ((rc = ovs::grow_dev(&m->d_keys, &m->d_keys_cap, rows * kNodeK)) != OVS_OK) return rc;
+    if ((rc = ovs::grow_host(&m->h_keys, &m->h_keys_cap, rows * kNodeK)) != OVS_OK) return rc;
+    memcpy(hqd, qdesc, 32 * sQ);
+    if (R) memcpy(htd, tdesc, 32 * sR);
+    memcpy(hsg, qseg, 8 * sQ);
+    if (taken) memcpy(htk, taken, sR);
+    cudaStream_t st = m->stream;
+    OVS_CUDA_CHECK(S.upload(st));
+    OVS_CUDA_CHECK(cudaMemsetAsync(m->d_keys, 0x5a, rows * kNodeK * 4, st));
+    A.nq = nq; A.taken = taken && q0 < 0 ? dtk : nullptr;
+    k_node_topk<<<(nq + 3) / 4, 128, 0, st>>>(A, m->d_keys);
+    OVS_LAUNCH_CHECK();
+    if (q0 >= 0) {
+        NodeArgs B = A;
+        B.q0 = q0; B.nq = q0 + 1; B.out_shift = nq - q0; B.taken = taken ? dtk : nullptr;
+        k_node_topk<<<1, 128, 0, st>>>(B, m->d_keys);
+        OVS_LAUNCH_CHECK();
+    }
+    OVS_CUDA_CHECK(cudaMemcpyAsync(m->h_keys, m->d_keys, rows * kNodeK * 4, cudaMemcpyDeviceToHost, st));
+    OVS_CUDA_CHECK(ovs::sync_stream(st));
+    memcpy(keys_out, m->h_keys, rows * kNodeK * 4);
+    return OVS_OK;
+}
+
+// Development aid / test hook: k_triangulation_topk on host arrays, with the launch geometry and buffers of
+// ovs_robust_match_for_triangulation_host (batched == 0: one problem, nprob == 1, queries_per_prob == nq) or of
+// ovs_create_new_landmarks_host (batched != 0: nq == nprob * queries_per_prob queries, query q of problem p = q / queries_per_prob
+// reads keypoint entry q - p * queries_per_prob of qdesc / qbearing / qscale / qstereo, E_12 prob_E[9 p], epipole prob_epipole[3 p],
+// and candidates (and taken flags) from prob_tbase[p] on).  qseg[2 nq] ranges are relative to the problem's base.  q0 and taken
+// as ovs_debug_node_topk.
+extern "C" int ovs_debug_triangulation_topk(ovs_matcher* m, int batched, int nq, int queries_per_prob, const uint8_t* qdesc,
+                                            const double* qbearing, const float* qscale, const uint8_t* qstereo, const int32_t* qseg, int R,
+                                            const uint8_t* tdesc, const double* tbearing, const uint8_t* tstereo, int nprob,
+                                            const double* prob_E, const double* prob_epipole, const int32_t* prob_tbase, const uint8_t* taken,
+                                            int q0, uint32_t* keys_out) {
+    OVS_REQUIRE(m && qdesc && qbearing && qscale && qstereo && qseg && keys_out && prob_E && prob_epipole && nq >= 1 && R >= 0 &&
+                (R == 0 || (tdesc && tbearing && tstereo)) && q0 < nq, OVS_ERR_INVALID_ARG, "bad argument");
+    OVS_REQUIRE(R < 65536, OVS_ERR_UNSUPPORTED, "more than 65535 candidate keypoints");
+    if (batched) OVS_REQUIRE(prob_tbase && nprob >= 1 && queries_per_prob >= 1 && (int64_t)nprob * queries_per_prob == nq, OVS_ERR_INVALID_ARG,
+                             "batched: nq must be nprob * queries_per_prob");
+    else OVS_REQUIRE(nprob == 1 && queries_per_prob == nq, OVS_ERR_INVALID_ARG, "one problem: nprob 1 and queries_per_prob == nq");
+    int rc = check_segments(nq, qseg, R, batched ? prob_tbase : nullptr, queries_per_prob);
+    if (rc != OVS_OK) return rc;
+    OVS_CUDA_CHECK(cudaSetDevice(m->device));
+    const size_t sK = (size_t)queries_per_prob, sQ = (size_t)nq, sR = (size_t)R, NB = (size_t)nprob, rows = sQ + (q0 >= 0 ? 1 : 0);
+    TriArgs A{};
+    uint8_t *hqd, *htd, *hq8, *ht8, *htk, *dtk; double *hqb, *htb, *hE = nullptr, *hep = nullptr; int2* hsg; float* hqs; int* htb0 = nullptr;
+    unsigned *hkeys, *dkeys;
+    ovs::Staging S;
+    const auto carve = [&](ovs::Staging& S) {
+        A.qdesc = (const uint4*)S.in(hqd, 32 * sK); A.tdesc = (const uint4*)S.in(htd, 32 * sR);
+        A.qbearing = S.in(hqb, 3 * sK); A.tbearing = S.in(htb, 3 * sR); A.qseg = S.in(hsg, sQ); A.qscale = S.in(hqs, sK);
+        A.qstereo = S.in(hq8, sK); A.tstereo = S.in(ht8, sR);
+        if (batched) { A.prob_E = S.in(hE, 9 * NB); A.prob_epipole = S.in(hep, 3 * NB); A.prob_tbase = S.in(htb0, NB); }
+        dtk = S.in(htk, sR);
+        if (batched) dkeys = S.out(hkeys, rows * kTriK);
+    };
+    rc = batched ? ovs::stage(S, m->h_tri, m->h_tri_cap, m->d_tri, m->d_tri_cap, carve) : ovs::stage(S, m->h_stage, m->h_stage_cap, m->d_q, m->d_q_cap, carve);
+    if (rc != OVS_OK) return rc;
+    if (!batched) {
+        if ((rc = ovs::grow_dev(&m->d_keys, &m->d_keys_cap, rows * kTriK)) != OVS_OK) return rc;
+        if ((rc = ovs::grow_host(&m->h_keys, &m->h_keys_cap, rows * kTriK)) != OVS_OK) return rc;
+        dkeys = m->d_keys; hkeys = m->h_keys;
+    }
+    memcpy(hqd, qdesc, 32 * sK); memcpy(hqb, qbearing, 24 * sK); memcpy(hqs, qscale, 4 * sK); memcpy(hq8, qstereo, sK);
+    memcpy(hsg, qseg, 8 * sQ);
+    if (R) { memcpy(htd, tdesc, 32 * sR); memcpy(htb, tbearing, 24 * sR); memcpy(ht8, tstereo, sR); }
+    if (taken) memcpy(htk, taken, sR);
+    if (batched) { memcpy(hE, prob_E, 72 * NB); memcpy(hep, prob_epipole, 24 * NB); memcpy(htb0, prob_tbase, 4 * NB); }
+    for (int k = 0; k < 9; ++k) A.E[k] = prob_E[k];
+    for (int k = 0; k < 3; ++k) A.epipole[k] = prob_epipole[k];
+    A.nq = nq; A.queries_per_prob = queries_per_prob; A.taken = taken && q0 < 0 ? dtk : nullptr;
+    cudaStream_t st = m->stream;
+    OVS_CUDA_CHECK(S.upload(st));
+    OVS_CUDA_CHECK(cudaMemsetAsync(dkeys, 0x5a, rows * kTriK * 4, st));
+    const auto launch = [&](const TriArgs& a, int blocks) {
+        if (batched) k_triangulation_topk<true><<<blocks, 128, 0, st>>>(a, dkeys);
+        else k_triangulation_topk<false><<<blocks, 128, 0, st>>>(a, dkeys);
+    };
+    launch(A, (nq + 3) / 4);
+    OVS_LAUNCH_CHECK();
+    if (q0 >= 0) {
+        TriArgs B = A;
+        B.q0 = q0; B.nq = q0 + 1; B.out_shift = nq - q0; B.taken = taken ? dtk : nullptr;
+        launch(B, 1);
+        OVS_LAUNCH_CHECK();
+    }
+    OVS_CUDA_CHECK(cudaMemcpyAsync(hkeys, dkeys, rows * kTriK * 4, cudaMemcpyDeviceToHost, st));
+    OVS_CUDA_CHECK(ovs::sync_stream(st));
+    memcpy(keys_out, hkeys, rows * kTriK * 4);
+    return OVS_OK;
+}
 
 // bow_tree::match_frame_and_keyframe(keyfrm, frm, matched_lms_in_frm): matched_keyfrm_idx_of_frm[i] = the keyframe keypoint
 // whose landmark frame keypoint i receives, or -1.  lm_valid_kf[k]: keyfrm landmark k non-null and not will_be_erased().

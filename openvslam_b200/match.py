@@ -97,6 +97,12 @@ class robust(_matcher_handle):
                                                                   C.c_float(self.lowe_ratio_), pairs.ctypes.data_as(C.c_void_p), cap, C.byref(n)))
         return pairs[:n.value].copy()
 
+    def brute_force_topk_device(self, d_query, nq, d_train, nt, d_keys_out):
+        """ovs_match_bruteforce_topk_device: brute_force_topk's (nq, 8) uint32 keys written to d_keys_out, with the descriptors
+        in device memory (device pointers as ints, descriptors 16-byte aligned); returns when the keys are written."""
+        _lib.check(_lib.lib().ovs_match_bruteforce_topk_device(self._h, C.c_void_p(int(d_query)), int(nq), C.c_void_p(int(d_train)), int(nt),
+                                                               C.c_void_p(int(d_keys_out))))
+
     def match_frame_and_keyframe(self, desc_frm, bearings_frm, desc_keyfrm, bearings_keyfrm, lm_valid_2=None, max_num_iter=50, seed=0):
         """robust::match_frame_and_keyframe(frm, keyfrm, matched_lms_in_frm): brute_force_match, then the essential-matrix RANSAC on
         the pairs (find_via_ransac(max_num_iter, false)) -> (num_inlier_matches, matched_keyfrm_idx_of_frm[n1]): the keyframe keypoint
