@@ -689,7 +689,7 @@ int om_stereo_compute(const uint8_t* const* left_pyr, const uint8_t* const* righ
  * The matching core of fuse::replace_duplication / detect_duplication: each usable landmark (reprojected into the keyframe by
  * the caller, who also does the depth-range and viewing-angle tests and predict_scale_level) searches the window
  * margin * scale_factors[level] over the levels [level - 1, level]; a candidate keypoint is skipped when its reprojection
- * error exceeds the chi-square bound of its own octave (5.99 monocular, 7.81 stereo with the x_right term); the nearest
+ * error exceeds the chi-square bound of its own octave (5.99 monocular, 7.8 stereo with the x_right term); the nearest
  * descriptor wins (first in visiting order on ties) and is accepted at <= HAMMING_DIST_THR_LOW.  No first-taker rule: what
  * happens to a keypoint that already has a landmark (replace / merge) is the caller's data-model decision.
  * best_idx_of_lm[q] = keypoint index or -1. */

@@ -7,31 +7,9 @@ import pytest
 from oracle import fuse as OF
 from oracle import oracle as O
 import fuse_problems as FP
+from fuse_reference import fuse_observe_reference
 import tracking_problems as TP
 import tracking_reference as REF
-
-
-def fuse_observe_reference(g, pos_w, mean_normal, min_valid_dist, max_valid_dist):
-    """-> passed (n,) bool, reproj_xy (n, 2) f32, x_right (n,) f32, pred_level (n,) i32: not finite -> rejected; reproject_to_image;
-    dist = sqrt((x^2 + y^2) + z^2) in double against the float bounds (float)(0.7 min) and (float)(1.3 max) compared in double;
-    ((v.x n.x + v.y n.y) + v.z n.z) < 0.5 dist rejects; predict_scale_level((float)dist)."""
-    P = np.asarray(pos_w, np.float64).reshape(-1, 3)
-    N = np.asarray(mean_normal, np.float64).reshape(-1, 3)
-    lo_raw = np.asarray(min_valid_dist, np.float32); hi_raw = np.asarray(max_valid_dist, np.float32)
-    ok, uv, xr = REF.reproject(g, P)
-    C = np.array(g.cam_center[:], np.float64)
-    with np.errstate(all="ignore"):
-        ok &= np.isfinite(P).all(1) & np.isfinite(uv).all(1)
-        v = P - C
-        dist = np.sqrt((v[:, 0] * v[:, 0] + v[:, 1] * v[:, 1]) + v[:, 2] * v[:, 2])
-        lo = (0.7 * lo_raw.astype(np.float64)).astype(np.float32).astype(np.float64)
-        hi = (1.3 * hi_raw.astype(np.float64)).astype(np.float32).astype(np.float64)
-        ok &= ~((dist < lo) | (hi < dist))
-        dot = (v[:, 0] * N[:, 0] + v[:, 1] * N[:, 1]) + v[:, 2] * N[:, 2]
-        ok &= ~(dot < 0.5 * dist)
-        level = REF.predict_scale_level(dist.astype(np.float32), hi_raw, g.log_scale_factor, g.num_scale_levels)
-    return (ok, np.where(ok[:, None], uv, np.float32(0)).astype(np.float32), np.where(ok, xr, np.float32(0)).astype(np.float32),
-            np.where(ok, level, 0).astype(np.int32))
 
 
 def _same_bits(a, b):
