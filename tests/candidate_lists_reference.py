@@ -168,3 +168,57 @@ def triangulation_topk_batched(qdesc, qbearing, qscale, qstereo, qseg, tdesc, tb
         out.append(keys); margin = min(margin, m)
     out = np.concatenate(out)
     return (out, margin) if with_margin else out
+
+
+def node_order(bow_node, keep):
+    """The keypoints that take part (keep, a vocabulary node) node by node, in index order inside a node: the
+    reference's walk over the BoW feature vector."""
+    node = np.asarray(bow_node)
+    idx = np.flatnonzero(np.asarray(keep, bool) & (node >= 0))
+    return idx[np.argsort(node[idx], kind="stable")]
+
+
+def node_segments(query_nodes, ranked_nodes):
+    """(q, 2): the range of ranks whose node is each query's"""
+    ranked_nodes = np.asarray(ranked_nodes)
+    return np.stack([np.searchsorted(ranked_nodes, query_nodes, "left"), np.searchsorted(ranked_nodes, query_nodes, "right")], 1)
+
+
+def first_taker(lists, requery, num_candidates, skip=None):
+    """match_for_triangulation's sequential loop over candidate lists: query k (in visiting order, skipped where skip[k])
+    takes the first candidate (rank 0xFFFF - tie) of lists[k] not taken yet; a list whose K entries are all taken is
+    recomputed by requery(k, taken) with the taken candidates excluded, and that list decides.
+    -> rank taken by each query (-1: none), whether it came from a re-query, number of re-queries"""
+    taken = np.zeros(num_candidates, bool)
+    pick = np.full(len(lists), -1, np.int64)
+    requeried = np.zeros(len(lists), bool)
+    decode = lambda x: 0xFFFF - (int(x) & 0xFFFF)
+    for k in range(len(lists)):
+        if skip is not None and skip[k]:
+            continue
+        keys = [int(x) for x in lists[k] if x != EMPTY]
+        free = [decode(x) for x in keys if not taken[decode(x)]]
+        if not free and len(keys) == K:
+            requeried[k] = True
+            free = [decode(x) for x in requery(k, taken) if x != EMPTY]
+        if free:
+            taken[free[0]] = True
+            pick[k] = free[0]
+    return pick, requeried, int(requeried.sum())
+
+
+def match_for_triangulation(p, sf):
+    """robust::match_for_triangulation without the orientation check on a synth.triangulation_problem p, from the lists
+    above and first_taker.  -> matched_idx_2_of_1, number of re-queries"""
+    n1 = len(p["desc_1"])
+    rank2 = node_order(p["bow_node_2"], p["has_lm_2"] == 0)
+    q1 = node_order(p["bow_node_1"], p["has_lm_1"] == 0)
+    seg = node_segments(p["bow_node_1"][q1], p["bow_node_2"][rank2]).reshape(-1, 2)
+    args = (p["desc_1"][q1], p["bearing_1"][q1], sf[p["octave_1"][q1]], p["is_stereo_1"][q1], seg, p["desc_2"][rank2], p["bearing_2"][rank2],
+            p["is_stereo_2"][rank2], p["E_12"], p["epipole_in_2"])
+    lists = triangulation_topk(*args)
+    pick, _, requeries = first_taker(lists, lambda k, taken: triangulation_topk(*[a[k:k + 1] for a in args[:5]], *args[5:], taken=taken)[0],
+                                     len(rank2))
+    match = np.full(n1, -1, np.int32)
+    match[q1[pick >= 0]] = rank2[pick[pick >= 0]]
+    return match, requeries

@@ -1,6 +1,6 @@
 """CPU checks of tests/candidate_lists_reference.py, the numpy reference the device candidate lists are compared with
 (tests/test_candidate_lists_gpu.py): against the oracle's brute force (best and second best), against a direct Python loop on
-small cases, and -- through a sequential first-taker loop over its lists -- against the oracle's match_for_triangulation."""
+small cases, and -- through its sequential first-taker loop over its lists -- against the oracle's match_for_triangulation."""
 import numpy as np
 import pytest
 
@@ -73,34 +73,15 @@ def test_hamming_one_and_node_topk_equal_a_python_loop():
             assert got[i].tolist() == want, (i, b, e)
 
 
-def _first_taker(p, sf):
-    """match_for_triangulation's sequential loop over the reference's lists: keyframe-1 keypoints node by node in index order,
-    each takes the first candidate of its list not taken yet; a list whose entries are all taken is recomputed with the
-    taken candidates excluded.  -> matched_idx_2_of_1"""
-    n1, n2 = len(p["desc_1"]), len(p["desc_2"])
-    order = lambda node, keep: sorted((i for i in range(len(node)) if keep[i] and node[i] >= 0), key=lambda i: (node[i], i))
-    rank2 = order(p["bow_node_2"], ~p["has_lm_2"].astype(bool))
-    q1 = order(p["bow_node_1"], ~p["has_lm_1"].astype(bool))
-    node2 = p["bow_node_2"][rank2]
-    seg = np.array([[np.searchsorted(node2, p["bow_node_1"][i], "left"), np.searchsorted(node2, p["bow_node_1"][i], "right")] for i in q1])
-    args = (p["desc_1"][q1], p["bearing_1"][q1], sf[p["octave_1"][q1]], p["is_stereo_1"][q1], seg, p["desc_2"][rank2], p["bearing_2"][rank2],
-            p["is_stereo_2"][rank2], p["E_12"], p["epipole_in_2"])
-    lists = ref.triangulation_topk(*args)
-    taken = np.zeros(len(rank2), bool)
-    match = np.full(n1, -1, np.int32)
-    requeries = 0
-    for k, i1 in enumerate(q1):
-        keys = [int(x) for x in lists[k] if x != ref.EMPTY]
-        free = [0xFFFF - (x & 0xFFFF) for x in keys if not taken[0xFFFF - (x & 0xFFFF)]]
-        if not free and len(keys) == ref.K:
-            requeries += 1
-            one = ref.triangulation_topk(*[a[k:k + 1] for a in args[:5]], *args[5:], taken=taken)[0]
-            free = [0xFFFF - (int(x) & 0xFFFF) for x in one if x != ref.EMPTY]
-        if free:
-            taken[free[0]] = True
-            match[i1] = rank2[free[0]]
-    assert n2 == len(p["desc_2"])
-    return match, requeries
+def test_node_order_and_segments_equal_a_python_loop():
+    rng = np.random.default_rng(8)
+    node = rng.integers(-1, 6, 200).astype(np.int32)
+    keep = rng.random(200) < 0.7
+    got = ref.node_order(node, keep)
+    assert got.tolist() == sorted((i for i in range(200) if keep[i] and node[i] >= 0), key=lambda i: (node[i], i))
+    seg = ref.node_segments(np.array([-1, 0, 3, 5, 9]), node[got])
+    for (b, e), q in zip(seg, [-1, 0, 3, 5, 9]):
+        assert [int(x) for x in node[got][b:e]] == [q] * int(sum(node[got] == q))
 
 
 @pytest.mark.parametrize("n,seed,nodes,dup", [(300, 1, 20, False), (400, 2, 3, False), (300, 7, 2, True)])
@@ -117,7 +98,7 @@ def test_triangulation_lists_replay_to_the_oracle(oracle, n, seed, nodes, dup):
     keys = ("desc_1", "bearing_1", "octave_1", "angle_1", "has_lm_1", "is_stereo_1", "bow_node_1",
             "desc_2", "bearing_2", "angle_2", "has_lm_2", "is_stereo_2", "bow_node_2", "E_12", "epipole_in_2")
     onum, om = oracle.robust_match_for_triangulation(*[p[k] for k in keys], sf, False)
-    got, requeries = _first_taker(p, np.asarray(sf, np.float32))
+    got, requeries = ref.match_for_triangulation(p, np.asarray(sf, np.float32))
     assert np.array_equal(got, om) and onum > 20
     if dup:
         assert requeries > 0

@@ -6,6 +6,7 @@ import numpy as np
 import pytest
 
 import triangulation_problems as TP
+from triangulation_cases import planar_neighbourhood as _planar_neighbourhood
 from openvslam_b200 import _lib, match, module
 
 pytestmark = pytest.mark.gpu
@@ -144,23 +145,6 @@ def test_carrying_the_landmark_flags_changes_the_result(OT):
     rec = np.concatenate([np.column_stack([np.full(len(r), b), r[:, 1:]]) for b, (r, _) in enumerate(indep)])
     assert len(rec) > len(got[0]) and len(np.unique(got[0][:, 1])) == len(got[0])
     mt.close()
-
-
-def _planar_neighbourhood(seed, n1, B):
-    """every point on the plane of the camera centres and one descriptor per few hundred keypoints, in two nodes: every
-    candidate of a query passes the epipolar test, so the 8-entry lists run out and the replay has to re-query"""
-    rng = np.random.default_rng(seed)
-    scene = TP.make_scene(rng, int(n1 * 1.3))
-    scene["X"][:, 1] = 0.0
-    base = rng.integers(0, 256, (3, 32), dtype=np.uint8)
-    def kf(c):
-        k, _ = TP.make_keyframe(rng, scene, c, np.eye(3), 0.0, 2, outlier_frac=0.0, noise_px=0.2)
-        k.descriptors[:] = base[rng.integers(0, 3, k.num_keypts)]
-        return k
-    kf1 = TP._trim(kf(np.zeros(3)), n1)
-    nbs = [kf(np.array([0.3 * (b + 1) * (-1) ** b, 0.0, 0.05 * b])) for b in range(B)]
-    Es, eps = zip(*[TP.e12_epipole(kf1, n) for n in nbs])
-    return kf1, nbs, np.array(Es), np.array(eps)
 
 
 def test_exhausted_lists_are_requeried(OT):
